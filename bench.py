@@ -11,9 +11,15 @@ configuration BASELINE.json's metric is quoted on: benzene (ccECP, 30 valence el
 Psiformer (d=256, L=4, H=4, K=16), a GLOBAL batch of 4096 walkers split over the N GPUs as the
 reference splits electron_batch_size over its devices (parallel.py:296-317; "scaling": "strong";
 ``--scaling weak`` keeps 4096 walkers per GPU instead).  The engine chunks the walkers through its
-workspace, so the whole batch fits one B200.  ``--workload lih_psiformer`` = BASELINE configs[1],
+workspace, so the whole batch fits one H100 (80 GB).  ``--workload lih_psiformer`` = BASELINE configs[1],
 ``n2_ferminet`` = configs[2].  Synthetic walkers (atom-centred Gaussians, equilibrated by
 Metropolis sub-steps, untimed) and random-init weights.
+
+``--dump-outputs DIR`` writes, after the timed steps, what the last timed step returned to its caller
+(local energies and the per-walker statistics of every state) and the walkers it was given, as
+DIR/<name>.npy.  The walkers are then taken straight from the seeded generator (no equilibration unless
+``--equil-sweeps`` asks for it), so the inputs do not depend on the build and two builds can be compared
+output for output.
 """
 import argparse
 import json
@@ -72,7 +78,7 @@ def make_problem(wl, B, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ('clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
          'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
@@ -106,19 +112,6 @@ class ClockSampler:
         return {'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': max(mx) if mx else None,
                 'reasons': reasons, 'samples': len(sm)}
 
-
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from one
-# `ncu --set full` capture of the same command (profiles/, B200_PROFILING.md); None = not captured.
-TRAFFIC = {
-    # profiles/r02_ncu_trunk_f16_kernel_ts.csv (ncu --set full of `tools/prof_fwd.py 2 17760`): one whole-trunk launch over
-    # 17760 plain-forward walkers x 30 electrons = 532800 rows: dram read 0.705 GB + write 2.368 GB.  Algorithmic bytes of
-    # that launch = rows x 256 x 4 B in + the same out + 6.3 MB of weights = 1.097 GB: the extra ~1.8 GB of writes are
-    # evictions of the per-CTA Q/K/V operand scratch (57 MB, re-written every tile and layer) from L2.  (The quadrature
-    # forwards of the ECP pass read even less: the unmoved electrons' embedding rows come from the base walkers' table.)
-    'benzene_psiformer': {'bytes_per_launch': 3.0727e9, 'algorithmic_bytes_per_launch': 1.0975e9,
-                          'launch': 'trunk_f16_kernel<TS>, 532800 rows (17760 plain-forward walkers x 30 electrons), 4 layers',
-                          'source': 'profiles/r02_ncu_trunk_f16_kernel_ts.csv'},
-}
 
 _ORACLE = {}
 
@@ -220,6 +213,22 @@ def time_oracle(wl_name, per_worker, steps, warmup, seed=0):
     return n * len(times) / sum(times), workers, 1e3 * float(np.mean(times)), n
 
 
+def dump_outputs(out_dir, last, n_states):
+    """The last timed step's inputs and outputs as .npy files (float64 / float32 as computed; a few MB at most)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for st in range(n_states):
+        sfx = f'_state{st}' if n_states > 1 else ''
+        arrays['walkers' + sfx] = last['r'][st]
+        arrays['local_energy' + sfx] = last['E'][st]
+        for k, v in last['stats'][st].items():
+            if torch.is_tensor(v) and v.dim() >= 1:
+                arrays[k.replace('/', '_') + sfx] = v
+    for name, v in arrays.items():
+        x = v.detach().cpu().numpy()
+        np.save(os.path.join(out_dir, name + '.npy'), x if x.dtype in (np.float32, np.float64) else x.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
@@ -232,9 +241,15 @@ def main():
     ap.add_argument('--scaling', default='strong', choices=['strong', 'weak'],
                     help='strong (default): the global batch is split over the GPUs as the reference does; weak: per-GPU batch')
     ap.add_argument('--cpu-sample', type=int, default=None)
-    ap.add_argument('--no-cpu-baseline', action='store_true')
-    ap.add_argument('--gemm-backend', default='tcgen05', choices=['simt', 'tcgen05'])
+    # the CPU oracle leg takes minutes on the heavy workloads (a benzene walker costs about a minute of one core): opt-in, so
+    # that a GPU benchmark run takes time proportional to --steps
+    ap.add_argument('--cpu-baseline', dest='cpu_baseline', action='store_true', default=False,
+                    help='also time the CPU oracle port (--impl reference) in a subprocess and report it')
+    ap.add_argument('--no-cpu-baseline', dest='cpu_baseline', action='store_false')
+    ap.add_argument('--gemm-backend', default='tensor', choices=['simt', 'tensor'])
     ap.add_argument('--equil-sweeps', type=int, default=None)
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step (and its input walkers) as DIR/<name>.npy')
     a = ap.parse_args()
     wl = WORKLOADS[a.workload]
     rank = int(os.environ.get('RANK', '0'))
@@ -287,7 +302,7 @@ def main():
     dev = torch.device('cuda', local)
     mol, hamil, r_np, PN = make_problem(wl, B_global * n_states, seed=1000)
     r_np = r_np.reshape(n_states, B_global, *r_np.shape[1:])[:, rank * B:(rank + 1) * B]  # contiguous walker block of this rank
-    backend = 1 if (a.gemm_backend == 'tcgen05' and a.dtype == 'float32' and wl['kind'] != 'paulinet') else 0  # d = 8: CUDA cores
+    backend = 1 if (a.gemm_backend == 'tensor' and a.dtype == 'float32' and wl['kind'] != 'paulinet') else 0  # d = 8: CUDA cores
     ansatz = B200Ansatz(hamil, wl['kind'], dtype=a.dtype, device=local, gemm_backend=backend, **wl['hyper'])
     # one parameter tree per electronic state (excited-state runs: reference wf/base.py:27-44 stacks them on a state axis)
     params_all = [PN.perturb_params(ansatz.init(st), seed=st) for st in range(n_states)]
@@ -297,7 +312,7 @@ def main():
     n_ecp = len(hamil.pot.nuc_with_nl_pot)
     R = torch.as_tensor(mol.coords, dtype=tdt, device=dev)
     heavy = wl['ecp'] is not None
-    n_equil = a.equil_sweeps if a.equil_sweeps is not None else (5 if heavy else 20)
+    n_equil = a.equil_sweeps if a.equil_sweeps is not None else (0 if a.dump_outputs else (5 if heavy else 20))
     r_states = []
     for st in range(n_states):  # equilibrate the synthetic walkers of every state (untimed): sweeps x 10 Metropolis sub-steps
         r = torch.as_tensor(r_np[st], dtype=tdt, device=dev)
@@ -313,7 +328,7 @@ def main():
     pcs = [PhysicalConfiguration(R, rs, torch.zeros(B, device=dev)) for rs in r_states]
     pc = pcs[0]
     loc_ene = hamil.local_energy(ansatz.apply)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     n_sub = wl.get('mcmc_substeps', 0)
     smp_state = None
@@ -321,6 +336,8 @@ def main():
         sign0, log0 = eng.wf_forward(r, R)
         smp_state = dict(r=r.clone(), sign=sign0, log=log0, age=torch.zeros(B, dtype=torch.int32, device=dev),
                          tau=torch.tensor([0.5], dtype=tdt, device=dev))
+
+    last = {}  # what the most recent step handed back: walkers, local energies and per-walker statistics per state
 
     def step(seed, pcs_=None):
         pcs_ = pcs_ or pcs
@@ -334,6 +351,7 @@ def main():
         for st in range(n_states):
             E, stt = loc_ene(seed, params_all[st], pcs_[st])
             Es.append(E); sts.append(stt)
+        last.update(r=[p_.r for p_ in pcs_], E=Es, stats=sts)
         if n_states > 1:  # pairwise overlap penalty: every state's wave function on every state's walkers (loss/overlap.py:19-150)
             from deepqmc_b200.overlap import compute_mean_overlap, compute_psi_ratio
 
@@ -367,6 +385,8 @@ def main():
         torch.distributed.barrier()
     t_wall = time.perf_counter() - t_wall0
     launches = eng.launch_count - l0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, last, n_states)
     clk = clocks.stop() if rank == 0 else None
     per_step = [e0.elapsed_time(e1) for e0, e1 in evs]
     ms = torch.tensor([sum(per_step)], device=dev, dtype=torch.float64)
@@ -383,10 +403,9 @@ def main():
         pcs_h = [PhysicalConfiguration(Rd, rh.to(dev, non_blocking=True), torch.zeros(B, device=dev)) for rh in r_host]
         _, E = step(seed, pcs_h)
         return E.cpu()
-    # long steps (seconds): the pipeline is warm already, bound the e2e leg to a few steps
-    # (same number of steps as the device-timed leg unless that would take more than ~2 minutes)
+    # long steps (seconds): the pipeline is warm already -- no warm-up, and at most --steps steps but no more than ~1 minute
     slow = total_ms / a.steps > 500.0
-    e2e_warm, e2e_steps = (1, max(3, min(a.steps, int(120e3 / (total_ms / a.steps))))) if slow else (3, a.steps)
+    e2e_warm, e2e_steps = (0, max(1, min(a.steps, int(60e3 / (total_ms / a.steps))))) if slow else (3, a.steps)
     for w in range(e2e_warm):
         e2e_step(w)
     torch.cuda.synchronize()
@@ -405,7 +424,7 @@ def main():
     # ---- roofline of the dominant kernel (dense-layer GEMMs), timed live with CUDA events ------
     roof = None
     if rank == 0:
-        n_prof = 1 if slow else 3
+        n_prof = 1 if slow else min(3, a.steps)
         eng.profile_begin()
         for s in range(n_prof):
             for st in range(n_states):
@@ -413,26 +432,19 @@ def main():
         cls = eng.profile_end_classes()  # {class: (ms, algorithmic flops, launches)} of the tensor-core kernels, timed live
         gemm_ms = sum(v[0] for v in cls.values())
         n_gemm = sum(v[2] for v in cls.values())
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
-        except Exception:
-            pass
-        peak = peaks.get('bf16_tflops_sustained', 1590.0 * 0.88)
+        peak = 989.0  # H100 SXM data sheet, dense FP16 / BF16 at 700 W: a ceiling, not a measured rate
         dom = max(cls, key=lambda k: cls[k][0])  # the class the step spends most time in
         dms, dfl, dn = cls[dom]
         achieved = dfl / (dms * 1e-3) / 1e12 if dms > 0 else 0.0
-        names = {'row_gemm': 'dense-layer row GEMM (' + ('tc::gemm3xtf32_kernel, tcgen05 3xTF32' if backend else 'CUDA-core gemm_kernel') + ')',
-                 'mlp_block': 'fused MLP block (tc::mlp_block_f16_kernel, tcgen05 3xFP16)',
-                 'trunk': 'whole-trunk kernel (tc::trunk_f16_kernel: all layers, dense GEMMs + attention, tcgen05 3xFP16, '
+        names = {'row_gemm': 'dense-layer row GEMM (' + ('tc::gemm3x_kernel, wgmma 3xTF32 / 3xFP16' if backend else 'CUDA-core gemm_kernel') + ')',
+                 'mlp_block': 'fused MLP block (tc::mlp_block_f16_kernel, wgmma 3xFP16)',
+                 'trunk': 'whole-trunk kernel (tc::trunk_f16_kernel: all layers, dense GEMMs + attention, wgmma 3xFP16, '
                           'one persistent launch per forward chunk)'}
-        traffic = TRAFFIC.get(a.workload) if dom == 'trunk' else None
         step_ms = total_ms / a.steps
         roof = {'bound': 'tensor', 'kernel': names[dom], 'achieved': achieved,
                 'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak,
-                'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained' if peaks else 'fallback',
+                'peak_source': 'H100 SXM data sheet, dense FP16/BF16 (not measured)',
                 'scheme_ceiling_frac': 1.0 / 3.0,  # fp32-class accuracy = 3 half-precision products per multiply-add
-                'traffic': (traffic or {}).get('bytes_per_launch'), 'traffic_detail': traffic,
                 'kernel_share_of_step': (dms / n_prof) / step_ms,
                 'kernel_launches_per_step': dn // n_prof,
                 'classes': {k: {'ms_per_step': v[0] / n_prof, 'share_of_step': (v[0] / n_prof) / step_ms,
@@ -449,7 +461,7 @@ def main():
     if rank != 0:
         return 0
     cpu = None
-    if not a.no_cpu_baseline and world == 1:
+    if a.cpu_baseline and world == 1:
         # the CPU leg runs in a fresh process (fork-based worker pool; this process holds a CUDA context)
         try:
             cp = subprocess.run([sys.executable, os.path.abspath(__file__), '--impl', 'reference', '--workload', a.workload,
@@ -467,7 +479,7 @@ def main():
                    'l2': 'flushed between timed iterations (256 MiB memset) and activations >> L2',
                    'step': (f'{n_sub} Metropolis sub-steps (all-electron proposals, in-kernel Philox) + ' if n_sub else '')
                            + 'E_loc of all walkers (+ one all_gather of the packed statistics for N>1)',
-                   'gemm_backend': 'tcgen05 (3xFP16 whole-trunk kernel for plain forwards, 3xTF32 row GEMMs for the forward-Laplacian rows)' if backend else 'cuda-core'},
+                   'gemm_backend': 'wgmma (3xFP16 whole-trunk kernel for plain forwards, 3xTF32 row GEMMs for the forward-Laplacian rows)' if backend else 'cuda-core'},
         'clocks': clk, 'e2e': {'value': e2e_val, 'unit': unit, 'h2d_bytes_per_step': (n_states * B * N * 3 + M * 3) * esz,
                                'd2h_bytes_per_step': n_states * B * esz, 'steps': e2e_steps},
         'gpu_launches': int(launches), 'roofline': roof, 'cpu_baseline': cpu,

@@ -1,4 +1,4 @@
-"""deepqmc_b200 -- B200-native (sm_100a) local-energy / Metropolis hot path for DeepQMC-style
+"""deepqmc_b200 -- H100-native (sm_90a) local-energy / Metropolis hot path for DeepQMC-style
 neural wave functions, behind the reference's Ansatz / Hamiltonian / ElectronSampler plugin
 interfaces.  See DESIGN.md and INTEGRATION.md."""
 from .molecule import Molecule

@@ -1,6 +1,6 @@
 """ctypes binding of libdqmc_b200.so (C ABI declared in include/dqmc_b200.h).
 
-The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is
+The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is
 NO fallback: if the library is missing or a symbol cannot be resolved, importing the engine
 raises.  ``load(path)`` with an explicit path exists only so the development-time CPU emulator
 build (tools/emu_check.py) can drive the same host code; the product never passes a path.
@@ -57,7 +57,7 @@ def load(path: str | None = None) -> C.CDLL:
     if not os.path.exists(path):
         raise ImportError(
             f'{path} not found: the CUDA engine is not built. Run `python -c "import __graft_entry__ as g; '
-            'g.build()"` (nvcc, sm_100a). There is no CPU fallback.'
+            'g.build()"` (nvcc, sm_90a). There is no CPU fallback.'
         )
     lib = C.CDLL(path)
     for s in SYMBOLS:

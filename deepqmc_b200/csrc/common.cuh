@@ -1,4 +1,4 @@
-// Shared device helpers for the local-energy engine (sm_100a).
+// Shared device helpers for the local-energy engine (sm_90a).
 // Compiles under nvcc (product) and, with -DDQMC_EMU, under g++ against
 // tools/cuda_emu/cuda_emu.h (development-time logic checks only, never shipped).
 #pragma once

@@ -1,6 +1,6 @@
 // Host side of libdqmc_b200.so: engine object, parameter table, workspace planning, kernel
-// sequencing, C ABI (include/dqmc_b200.h).  Built by nvcc for sm_100a; with -DDQMC_EMU the same
-// file builds against tools/cuda_emu for CPU-side logic checks during development (never shipped).
+// sequencing, C ABI (include/dqmc_b200.h).  Built by nvcc for sm_90a (H100); with -DDQMC_EMU -DDQMC_NO_TCGEN05 the
+// same file builds against tools/cuda_emu for CPU-side logic checks of the SIMT kernels during development (never shipped).
 #include <algorithm>
 #include <array>
 #include <cstdio>
@@ -20,7 +20,7 @@
 #include "kernels_bwd.cuh"
 #include "attn_mma.cuh"
 #if !defined(DQMC_NO_TCGEN05)
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "fused_tc.cuh"
 #include "trunk_tc.cuh"
 #endif
@@ -340,28 +340,25 @@ struct Engine : EngineBase {
   bool trans = false;  // TransPsiformer: nuclear attention tokens + nucleus-dependent envelopes
   int Mn = 0, env_rep = 1;
   size_t max_smem = 0;
-  int n_sms = 148;
-#if !defined(DQMC_NO_TCGEN05)
-  struct TcWeight {
-    float* hi = nullptr; float* lo = nullptr; CUtensorMap mh, ml, mh2, ml2; int N = 0, K = 0, BN = 0;
-    // "3xFP16" operands of the plain-forward kernels: (W 2^e)^T as halves, hi / lo planes [N][K]; maps with BN-row boxes
-    // (row GEMM) and with all-N-row boxes (fused MLP block, N <= 256)
-    uint16_t* h16 = nullptr; CUtensorMap m16h, m16l, m16h_all, m16l_all; float wscale = 1.f; bool f16 = false, f16_all = false;
-    CUtensorMap m16h_128, m16l_128; bool f16_128 = false;  // 128-row boxes: weight slots of the whole-trunk kernel (trunk_tc.cuh)
-  };
+  int n_sms = 132;
   // non-local ECP group in flight: envelope table of its base walkers [nb][N][K N] (null outside the quadrature forwards),
   // index of the current chunk's first virtual walker, virtual walkers per base walker (J N 12)
   const T* ecp_env = nullptr;
   const T* ecp_emb = nullptr;  // ... and their embedding rows [nb][N][d] (whole-trunk kernel only)
   int64_t ecp_v0 = 0;
   int ecp_vper = 0;
+#if !defined(DQMC_NO_TCGEN05)
+  struct TcWeight {
+    float* hi = nullptr; float* lo = nullptr; CUtensorMap mh, ml; int N = 0, K = 0;
+    // "3xFP16" operands of the plain-forward kernels: (W 2^e)^T as halves, hi / lo planes [N][K]; maps with BN-row boxes
+    // (row GEMM) and with all-N-row boxes (fused MLP block, N <= 256)
+    uint16_t* h16 = nullptr; CUtensorMap m16h, m16l, m16h_all, m16l_all; float wscale = 1.f; bool f16 = false, f16_all = false;
+    CUtensorMap m16h_256, m16l_256; bool f16_256 = false;  // 256-row boxes: weight slots of the whole-trunk kernel (trunk_tc.cuh)
+  };
   bool fuse_trunk = true;  // all layers of a plain forward in one persistent launch (trunk_tc.cuh); DQMC_TC_TRUNK=0 disables
-  bool trunk_ts = true;    // ... with the A operand of its dense GEMMs in tensor memory (DQMC_TC_TRUNK_TS=0: shared memory)
   CUtensorMap* d_trunk_maps = nullptr;       // [L][4][2]
-  unsigned char* d_trunk_scratch = nullptr;  // n_sms x 384 KB Q / K / V planes
-  long long* d_trunk_trace = nullptr;        // DQMC_TRUNK_TRACE: 64 clock stamps of one tile (development aid)
-  bool gemm_2cta = false;  // CTA-pair (cta_group::2) variant of the dense-layer GEMM
-  bool f16_on = true;      // plain forwards (S = 1) on kind::f16 with hi / lo half operands; DQMC_TC_F16=0: stay on 3xTF32
+  unsigned char* d_trunk_scratch = nullptr;  // n_sms x 512 KB: Q / K / V and residual rows of a tile
+  bool f16_on = true;      // plain forwards (S = 1) on f16 wgmma with hi / lo half operands; DQMC_TC_F16=0: stay on 3xTF32
   bool fuse_mlp = true;    // W_o + residual -> W1 + tanh -> W2 + tanh + residual in one launch (S = 1); DQMC_TC_FUSE_MLP=0 disables
   static constexpr float kActScale = 16.f;  // 2^4: |activation| < 4094 representable, absolute floor 2^-29
   std::map<std::string, TcWeight> tcw;
@@ -371,16 +368,15 @@ struct Engine : EngineBase {
     if (!w.hi) {
       DQ_CHECK(cudaMalloc((void**)&w.hi, sizeof(float) * (size_t)Kc * Nc));
       DQ_CHECK(cudaMalloc((void**)&w.lo, sizeof(float) * (size_t)Kc * Nc));
-      w.N = Nc; w.K = Kc; w.BN = tc::pick_bn(Nc);
-      if (tc::make_weight_map(&w.mh, w.hi, Nc, Kc, w.BN) || tc::make_weight_map(&w.ml, w.lo, Nc, Kc, w.BN) ||
-          tc::make_weight_map(&w.mh2, w.hi, Nc, Kc, w.BN / 2) || tc::make_weight_map(&w.ml2, w.lo, Nc, Kc, w.BN / 2)) {
+      w.N = Nc; w.K = Kc;
+      if (tc::make_weight_map(&w.mh, w.hi, Nc, Kc, tc::kBN) || tc::make_weight_map(&w.ml, w.lo, Nc, Kc, tc::kBN)) {
         err = "cuTensorMapEncodeTiled failed for " + name;
         return 4;
       }
       if (Kc % 64 == 0) {
         DQ_CHECK(cudaMalloc((void**)&w.h16, sizeof(uint16_t) * 2 * (size_t)Kc * Nc));
         const uint16_t* lo16 = w.h16 + (size_t)Kc * Nc;
-        if (tc::make_kmajor_map(&w.m16h, w.h16, 2, Nc, Kc, 64, w.BN) || tc::make_kmajor_map(&w.m16l, lo16, 2, Nc, Kc, 64, w.BN)) {
+        if (tc::make_kmajor_map(&w.m16h, w.h16, 2, Nc, Kc, 64, tc::kBN) || tc::make_kmajor_map(&w.m16l, lo16, 2, Nc, Kc, 64, tc::kBN)) {
           err = "cuTensorMapEncodeTiled (half planes) failed for " + name;
           return 4;
         }
@@ -392,9 +388,9 @@ struct Engine : EngineBase {
           }
           w.f16_all = true;
         }
-        if (Kc == 256 && Nc % 128 == 0 &&
-            !tc::make_kmajor_map(&w.m16h_128, w.h16, 2, Nc, Kc, 64, 128) && !tc::make_kmajor_map(&w.m16l_128, lo16, 2, Nc, Kc, 64, 128))
-          w.f16_128 = true;
+        if (Kc == 256 && Nc % 256 == 0 &&
+            !tc::make_kmajor_map(&w.m16h_256, w.h16, 2, Nc, Kc, 64, 256) && !tc::make_kmajor_map(&w.m16l_256, lo16, 2, Nc, Kc, 64, 256))
+          w.f16_256 = true;
       }
     }
     DQ_LAUNCH(split_transpose_kernel, dim3((Kc * Nc + 255) / 256), dim3(256), 0, st, W, Kc, Nc, w.hi, w.lo);
@@ -569,29 +565,20 @@ struct Engine : EngineBase {
 #if !defined(DQMC_NO_TCGEN05)
       if (!std::is_same<T, float>::value) { err = "DQMC_GEMM_TCGEN05 needs dtype DQMC_F32"; return 2; }
       if (d % 32 != 0) { err = "DQMC_GEMM_TCGEN05 needs embedding_dim % 32 == 0"; return 2; }
-      DQ_CHECK(raise_dyn_smem((tc::gemm3xtf32_kernel<false, false>), tc::SmemLayout::total(256)));
-      DQ_CHECK(raise_dyn_smem((tc::gemm3xtf32_kernel<false, true>), tc::SmemLayout::total(256)));
-      DQ_CHECK(raise_dyn_smem(tc::mlp_block_f16_kernel, tc::MlpSmem::total()));
-      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<false>, tc::TrSmem::total()));
-      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<true>, tc::TrSmem::total()));
-#ifndef DQMC_EMU
-      DQ_CHECK(raise_dyn_smem((tc::gemm3xtf32_kernel<true, false>), tc::SmemLayoutT<true>::total(256)));
-      gemm_2cta = std::getenv("DQMC_GEMM_2CTA") != nullptr;
-#endif
+      DQ_CHECK(raise_dyn_smem(tc::gemm3x_kernel<false>, tc::SmemLayout::total()));
+      DQ_CHECK(raise_dyn_smem(tc::gemm3x_kernel<true>, tc::SmemLayout::total()));
+      DQ_CHECK(raise_dyn_smem(tc::mlp_block_f16_kernel<128>, tc::MlpSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::mlp_block_f16_kernel<256>, tc::MlpSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel, tc::TrSmem::total()));
       if (const char* ev = std::getenv("DQMC_TC_F16")) f16_on = std::atoi(ev) != 0;
       if (const char* ev = std::getenv("DQMC_TC_FUSE_MLP")) fuse_mlp = std::atoi(ev) != 0;
       if (const char* ev = std::getenv("DQMC_TC_TRUNK")) fuse_trunk = std::atoi(ev) != 0;
-      if (const char* ev = std::getenv("DQMC_TC_TRUNK_TS")) trunk_ts = std::atoi(ev) != 0;
       if (psif && !trans && d == 256 && H == 4 && N <= 32 && cfg.n_layers <= tc::kTrMaxLayers) {
         DQ_CHECK(cudaMalloc((void**)&d_trunk_maps, sizeof(CUtensorMap) * 8 * cfg.n_layers));
         DQ_CHECK(cudaMalloc((void**)&d_trunk_scratch, (size_t)n_sms * tc::kTrScratchPerCta));
-        if (std::getenv("DQMC_TRUNK_TRACE")) {
-          DQ_CHECK(cudaMalloc((void**)&d_trunk_trace, sizeof(long long) * 64));
-          DQ_CHECK(cudaMemset(d_trunk_trace, 0, sizeof(long long) * 64));
-        }
       }
 #else
-      err = "this build has no tcgen05 backend"; return 2;
+      err = "this build has no tensor-core backend"; return 2;
 #endif
     }
     return 0;
@@ -673,8 +660,8 @@ struct Engine : EngineBase {
           int g = 0;
           for (const char* n : {"wqkv", "wo", "w1", "w2"}) {
             const TcWeight& w = tcw.at(pfx + n);
-            hm[(size_t)8 * l + 2 * g] = w.m16h_128;
-            hm[(size_t)8 * l + 2 * g + 1] = w.m16l_128;
+            hm[(size_t)8 * l + 2 * g] = w.m16h_256;
+            hm[(size_t)8 * l + 2 * g + 1] = w.m16l_256;
             ++g;
           }
         }
@@ -900,42 +887,25 @@ struct Engine : EngineBase {
         const TcWeight& t1 = w1 ? tcw.at(w1) : t0;
         tc::Params p;
         p.A = A; p.lda = lda; p.bias = bias; p.Res = Res; p.ldr = ldr; p.C = C; p.ldc = ldc; p.M = Mr; p.N = Nc;
-        p.K = Kc; p.S = S; p.sliced = sliced; p.Nel = Nel; p.z_split = zsplit; p.BN = t0.BN; p.err_flag = nullptr;
+        p.K = Kc; p.S = S; p.sliced = sliced; p.Nel = Nel; p.z_split = zsplit; p.err_flag = nullptr;
         p.act = act;
         p.rpt = (act && S > 1) ? (128 / S) * S : tc::kBM;
         p.a_scale = 1.f; p.unscale = 1.f;
-        // plain forwards: half operands (hi / lo), kind::f16 -- twice the MMA rate, half the shared-memory bytes per k
-        const bool f16 = S == 1 && f16_on && Kc % 64 == 0 && t0.f16 && t1.f16 && t0.wscale == t1.wscale && !gemm_2cta;
+        // plain forwards: half operands (hi / lo), f16 wgmma -- twice the MMA rate, half the shared-memory bytes per k
+        const bool f16 = S == 1 && f16_on && Kc % 64 == 0 && t0.f16 && t1.f16 && t0.wscale == t1.wscale;
         if (f16) { p.a_scale = kActScale; p.unscale = 1.f / (kActScale * t0.wscale); }
-        int MT = (Mr + p.rpt - 1) / p.rpt, NT = (Nc + p.BN - 1) / p.BN;
-        int n_tiles = (sliced ? Nel : 1) * MT * NT;
-        int grid = n_tiles < n_sms ? n_tiles : n_sms;
+        const int MT = (Mr + p.rpt - 1) / p.rpt, NT = (Nc + tc::kBN - 1) / tc::kBN;
+        const int n_tiles = (sliced ? Nel : 1) * MT * NT;  // one tile per CTA
 #ifndef DQMC_EMU
         cudaEvent_t e0 = nullptr, e1 = nullptr;
         if (prof) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
-        if (gemm_2cta && n_sms >= 2) {
-          // CTA pairs: clusters of 2, each pair owns 256-row tiles; weight maps with half-tile boxes
-          const int MT2 = (MT + 1) / 2;
-          const int n_pt = (sliced ? Nel : 1) * MT2 * NT;
-          int pairs = n_sms / 2;
-          if (n_pt < pairs) pairs = n_pt;
-          cudaLaunchConfig_t lc = {};
-          lc.gridDim = dim3(2 * pairs); lc.blockDim = dim3(tc::kThreads);
-          lc.dynamicSmemBytes = tc::SmemLayoutT<true>::total(p.BN); lc.stream = st;
-          cudaLaunchAttribute at[1];
-          at[0].id = cudaLaunchAttributeClusterDimension;
-          at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-          lc.attrs = at; lc.numAttrs = 1;
-          DQ_CHECK(cudaLaunchKernelEx(&lc, tc::gemm3xtf32_kernel<true, false>, t0.mh2, t0.ml2, t1.mh2, t1.ml2, p));
-          ++launches;
-        } else
 #endif
         if (f16)
-          DQ_LAUNCH((tc::gemm3xtf32_kernel<false, true>), dim3(grid), dim3(tc::kThreads), tc::SmemLayout::total(p.BN), st, t0.m16h,
-                    t0.m16l, t1.m16h, t1.m16l, p);
+          DQ_LAUNCH(tc::gemm3x_kernel<true>, dim3(n_tiles), dim3(tc::kThreads), tc::SmemLayout::total(), st, t0.m16h, t0.m16l,
+                    t1.m16h, t1.m16l, p);
         else
-          DQ_LAUNCH((tc::gemm3xtf32_kernel<false, false>), dim3(grid), dim3(tc::kThreads), tc::SmemLayout::total(p.BN), st, t0.mh,
-                    t0.ml, t1.mh, t1.ml, p);
+          DQ_LAUNCH(tc::gemm3x_kernel<false>, dim3(n_tiles), dim3(tc::kThreads), tc::SmemLayout::total(), st, t0.mh, t0.ml,
+                    t1.mh, t1.ml, p);
 #ifndef DQMC_EMU
         if (prof) {
           cudaEventRecord(e1, st);
@@ -998,8 +968,12 @@ struct Engine : EngineBase {
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       if (prof) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
 #endif
-      DQ_LAUNCH(tc::mlp_block_f16_kernel, dim3(grid), dim3(tc::kMlpThreads), tc::MlpSmem::total(), st, wo.m16h_all, wo.m16l_all,
-                w1.m16h_all, w1.m16l_all, w2.m16h_all, w2.m16l_all, p);
+      if (d == 256)
+        DQ_LAUNCH(tc::mlp_block_f16_kernel<256>, dim3(grid), dim3(tc::kMlpThreads), tc::MlpSmem::total(), st, wo.m16h_all,
+                  wo.m16l_all, w1.m16h_all, w1.m16l_all, w2.m16h_all, w2.m16l_all, p);
+      else
+        DQ_LAUNCH(tc::mlp_block_f16_kernel<128>, dim3(grid), dim3(tc::kMlpThreads), tc::MlpSmem::total(), st, wo.m16h_all,
+                  wo.m16l_all, w1.m16h_all, w1.m16l_all, w2.m16h_all, w2.m16l_all, p);
 #ifndef DQMC_EMU
       if (prof) {
         cudaEventRecord(e1, st);
@@ -1028,7 +1002,7 @@ struct Engine : EngineBase {
     for (int l = 0; l < cfg.n_layers; ++l)
       for (const char* n : {"wqkv", "wo", "w1", "w2"}) {
         auto it = tcw.find("L" + std::to_string(l) + "." + n);
-        if (it == tcw.end() || !it->second.f16_128) return false;
+        if (it == tcw.end() || !it->second.f16_256) return false;
       }
     return true;
 #else
@@ -1052,9 +1026,7 @@ struct Engine : EngineBase {
       int np2 = 1;
       while (np2 < N) np2 *= 2;  // walker slot of the tile: electrons rounded up to a power of two (<= 32)
       p.walkers = rows / N; p.N = N; p.NP = np2; p.L = cfg.n_layers; p.a_scale = kActScale;
-      p.attn_scale = (float)(1.0 / std::sqrt((double)dh)); p.err_flag = nullptr; p.trace = d_trunk_trace;
-      p.ablate = 0;
-      if (const char* ev = std::getenv("DQMC_TRUNK_ABLATE")) p.ablate = std::atoi(ev);
+      p.attn_scale = (float)(1.0 / std::sqrt((double)dh)); p.err_flag = nullptr;
       for (int l = 0; l < cfg.n_layers; ++l) {
         const std::string pfx = "L" + std::to_string(l) + ".";
         p.b1[l] = P(pfx + "b1"); p.b2[l] = P(pfx + "b2");
@@ -1067,9 +1039,7 @@ struct Engine : EngineBase {
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       if (prof) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
 #endif
-      // DQMC_TC_TRUNK_TS=0: A operand of the dense GEMMs from shared memory (SS form) instead of tensor memory
-      if (trunk_ts) DQ_LAUNCH(tc::trunk_f16_kernel<true>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p);
-      else DQ_LAUNCH(tc::trunk_f16_kernel<false>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p);
+      DQ_LAUNCH(tc::trunk_f16_kernel, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p);
 #ifndef DQMC_EMU
       if (prof) {
         cudaEventRecord(e1, st);
@@ -1089,16 +1059,6 @@ struct Engine : EngineBase {
     int rc = trunk_block((const T*)X0, (T*)Out, rows, st);
     if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
-#ifndef DQMC_EMU
-    if (d_trunk_trace) {  // print the stamps relative to the first one
-      long long h[64];
-      DQ_CHECK(cudaStreamSynchronize(st));
-      DQ_CHECK(cudaMemcpy(h, d_trunk_trace, sizeof(h), cudaMemcpyDeviceToHost));
-      std::fprintf(stderr, "trunk trace (clocks since the start of layer 1 of the traced tile):");
-      for (int i = 0; i < 37; ++i) std::fprintf(stderr, " [%d]%lld", i, h[i] ? h[i] - h[0] : -1LL);
-      std::fprintf(stderr, "\n");
-    }
-#endif
     return 0;
   }
 
@@ -2390,7 +2350,7 @@ struct dqmc_engine {
 
 extern "C" {
 
-const char* dqmc_version(void) { return "dqmc_b200 0.1 (sm_100a)"; }
+const char* dqmc_version(void) { return "dqmc_b200 0.1 (sm_90a)"; }
 
 int dqmc_create(const dqmc_config* cfg, int device, dqmc_handle* out) {
   if (!cfg || !out) return 2;

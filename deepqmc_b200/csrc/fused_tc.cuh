@@ -1,4 +1,5 @@
-// Fused Psiformer MLP block of a plain forward (S = 1) on the 5th-gen tensor cores, "3xFP16" operands (see gemm_tcgen05.cuh):
+// Fused Psiformer MLP block of a plain forward (S = 1) on the Hopper tensor cores (wgmma), "3xFP16" operands (see
+// gemm_wgmma.cuh):
 //
 //     A  = X + O Wo                      (attention output projection + residual)
 //     M1 = tanh(A W1 + b1)
@@ -6,19 +7,15 @@
 //                                          conf/ansatz/psiformer.yaml:84-101 MLP; hkext.py:22-113, residual rule :116-137)
 //
 // for a tile of 128 rows (row = walker x electron) per CTA, persistent over tiles.  The three GEMMs of a tile run back to back
-// with every intermediate on chip: A stays in TMEM columns [0, d) as fp32 (it is the residual of the last stage), the operand
-// of the next GEMM is written by the epilogue of the previous one straight into the 128-byte-swizzled K-major operand buffer
-// in shared memory (split into hi / lo halves), and only O and X are read from / X' written to HBM: 3 x 4 d bytes per row
-// instead of 8 x 4 d with one launch per layer.
+// with the operand of the next GEMM written by the epilogue of the previous one straight from the accumulator registers into
+// the 128-byte-swizzled K-major operand buffer in shared memory (split into hi / lo halves): one launch per layer instead of
+// three, and M1 never leaves the SM.  A is written to the output rows and read back by the same thread in the last epilogue
+// (the accumulator of the next GEMM already fills the register file).
 //
-// warp roles (320 threads):
-//   warps 0-7  workers : stage the O tile (fp32 -> hi/lo halves), then the three epilogues.  Warp w owns TMEM lanes / tile rows
-//                        32 (w % 4) .. +31 and the column half w / 4 (k-blocks {0,1} or {2,3} of the next operand).
-//   warp  8    TMA     : streams the pre-split weight planes [d x 64 halves] (hi, lo per k-block) of Wo, W1, W2 through a
-//                        3-stage ring; runs ahead across GEMM / tile boundaries.
-//   warp  9    MMA     : tcgen05.mma kind::f16, M = 128, N = d: per k-block  a_lo w_hi + a_hi w_hi  (hi plane),  a_hi w_lo  (lo plane).
-// shared memory: operand buffer 4 k-blocks x {hi, lo} x 16 KB = 128 KB, weight ring 3 x 32 KB, biases, barriers.
-// TMEM (512 columns): [0, d) GEMM 1 accumulator -> A;  [256, 256 + d) accumulator of GEMM 2, then of GEMM 3.
+// 256 threads = two warpgroups; warpgroup w computes tile rows 64 w .. +63 over all d columns (wgmma m64 n = d, fp32
+// accumulators in registers).  Thread 0 streams the pre-split weight planes [d rows x 64 halves] (hi, lo per k-block) of
+// Wo, W1, W2 through a 3-slot ring (TMA): the planes of the next two k-steps land while the current one is multiplied.
+// shared memory: operand buffer 4 k-blocks x {hi, lo} x 16 KB = 128 KB, weight ring 3 x 32 KB, biases, barriers (226 KB).
 #pragma once
 #include <cstdint>
 
@@ -27,8 +24,8 @@
 namespace dq {
 namespace tc {
 
-constexpr int kMlpThreads = 320;
-constexpr int kMlpStages = 3;
+constexpr int kMlpThreads = 256;
+constexpr int kMlpSlots = 3;  // weight ring: a slot is refilled 3 slots ahead, i.e. under the MMAs of the next two
 
 struct MlpParams {
   const float* O; int ldo;     // attention output rows [M][d]
@@ -44,12 +41,12 @@ struct MlpParams {
 struct MlpSmem {
   static __host__ __device__ int abuf(int kb, int plane) { return (kb * 2 + plane) * 16384; }   // [128 rows][128 B]
   static __host__ __device__ int wring(int s) { return 131072 + s * 32768; }                      // [<= 256 rows][128 B]
-  static __host__ __device__ int bias() { return 131072 + kMlpStages * 32768; }                   // b1[256], b2[256]
+  static __host__ __device__ int bias() { return 131072 + kMlpSlots * 32768; }                    // b1[256], b2[256]
   static __host__ __device__ int bars() { return bias() + 2048; }
-  static __host__ __device__ int total() { return bars() + 256; }
+  static __host__ __device__ int total() { return bars() + 64; }
 };
 
-// tanh of the plain-forward epilogues (same as gemm_tcgen05.cuh tanh_fwd): absolute error <= ~3e-7
+// tanh of the plain-forward epilogues (same as gemm_wgmma.cuh tanh_fwd): absolute error <= ~3e-7
 __device__ __forceinline__ float mlp_tanh(float x) {
   const float x2 = x * x;
   const float poly = x + x * x2 * (-0.33333333333f + x2 * (0.13333333333f + x2 * (-0.05396825397f)));
@@ -60,9 +57,8 @@ __device__ __forceinline__ float mlp_tanh(float x) {
 
 // (x0, x1) -> packed hi halves and packed lo halves, x = hi + lo to 22 significant bits.  hi is formed in fp32 by Veltkamp's
 // splitting (c = 8193 x, hi = c - (c - x): x rounded to 11 bits, three full-rate instructions) instead of converting the packed
-// half back (F2F conversions issue at a fraction of the FMA rate and made up a fifth of the whole-trunk kernel's stall samples);
-// x - hi is exact, both packs are then plain cvt.rn.f16x2.  Values below the normal half range (2^-14 after scaling) keep
-// the absolute floor of 2^-25 that the split has anyway.
+// half back; x - hi is exact, both packs are then plain cvt.rn.f16x2.  Values below the normal half range (2^-14 after
+// scaling) keep the absolute floor of 2^-25 that the split has anyway.
 __device__ __forceinline__ void split_half2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   const float c0 = __fmul_rn(x0, 8193.f), c1 = __fmul_rn(x1, 8193.f);
   const float h0 = __fsub_rn(c0, __fsub_rn(c0, x0)), h1 = __fsub_rn(c1, __fsub_rn(c1, x1));
@@ -70,246 +66,223 @@ __device__ __forceinline__ void split_half2(float x0, float x1, uint32_t& hi, ui
   lo = pack_half2_rn(__fsub_rn(x0, h0), __fsub_rn(x1, h1));
 }
 
-// 32 consecutive columns [c0, c0 + 32) of tile row `row` (values v, already scaled by a_scale) -> hi / lo halves in the
-// K-major operand buffer: k-block c0 / 64, 16-byte chunks 4 (c0 / 32 % 2) .. +3 of the row's 128-byte line.
-__device__ __forceinline__ void store_operand_chunk(unsigned char* smem, int row, int c0, const float* v) {
-  const int kb = c0 >> 6, cbase = ((c0 >> 5) & 1) * 4;
-  unsigned char* ph = smem + MlpSmem::abuf(kb, 0) + (row >> 3) * 1024 + (row & 7) * 128;
-  unsigned char* pl = smem + MlpSmem::abuf(kb, 1) + (row >> 3) * 1024 + (row & 7) * 128;
+// byte offset of operand element (row, col) inside its k-block plane: 64 halves per 128-byte row, 16-byte chunks XOR row % 8
+__device__ __forceinline__ int operand_off(int row, int col) {
+  const int cc = col & 63;
+  return (row >> 3) * 1024 + (row & 7) * 128 + ((((cc >> 3) ^ row) & 7) << 4) + (cc & 7) * 2;
+}
+// two adjacent columns (col even) of tile row `row`, already scaled by a_scale
+__device__ __forceinline__ void store_operand_pair(unsigned char* smem, int row, int col, float a0, float a1) {
+  uint32_t h, l;
+  split_half2(a0, a1, h, l);
+  const int off = operand_off(row, col), kb = col >> 6;
+  *(uint32_t*)(smem + MlpSmem::abuf(kb, 0) + off) = h;
+  *(uint32_t*)(smem + MlpSmem::abuf(kb, 1) + off) = l;
+}
+// four adjacent columns (col % 4 == 0) of tile row `row`, already scaled
+__device__ __forceinline__ void store_operand_quad(unsigned char* smem, int row, int col, float4 a) {
+  uint32_t h01, l01, h23, l23;
+  split_half2(a.x, a.y, h01, l01);
+  split_half2(a.z, a.w, h23, l23);
+  const int off = operand_off(row, col), kb = col >> 6;
+  *(uint2*)(smem + MlpSmem::abuf(kb, 0) + off) = make_uint2(h01, h23);
+  *(uint2*)(smem + MlpSmem::abuf(kb, 1) + off) = make_uint2(l01, l23);
+}
+
+// acc = (operand buffer, K = D) x (rows y0 .. y0 + D - 1 of W^T), hi / lo planes through the 3-slot weight ring.  Called by all
+// 256 threads with the operand buffer complete (fenced + __syncthreads); returns with every MMA retired and the ring free.
+// `nslot` counts the ring slots used so far: slot g lives in ring stage g % 3 and completes phase (g / 3) & 1 of its barrier.
+template <int D>
+__device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* smem, uint64_t* full, uint32_t& nslot,
+                                          const CUtensorMap* mh, const CUtensorMap* ml, int y0, int* err) {
+  constexpr int KB = D / 64;
+  constexpr int NS = 2 * KB;  // slots of this GEMM: slot i = plane i % 2 (hi, lo) of k-block i / 2
+  static_assert(NS >= kMlpSlots, "the ring is filled at the start of a GEMM");
+  constexpr uint32_t kSlot = D * 128u;
+  const int tid = threadIdx.x, wg = tid >> 7;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint32_t h[4], l[4];
+  for (int i = 0; i < D / 2; ++i) acc[i] = 0.f;  // the previous contents are dead: registers free between GEMMs
+  auto stage = [&](int i) { return (int)((nslot + (uint32_t)i) % (uint32_t)kMlpSlots); };
+  auto load = [&](int i) {
+    const int st = stage(i);
+    mbar_expect_tx(&full[st], kSlot);
+    tma_load_2d((i & 1) ? ml : mh, &full[st], smem + MlpSmem::wring(st), (i >> 1) * 64, y0);
+  };
+  if (tid == 0)
+    for (int i = 0; i < kMlpSlots; ++i) load(i);
+  // waits for slot i and returns its shared-memory address
+  auto acquire = [&](int i) {
+    const int st = stage(i);
+    mbar_wait(&full[st], ((nslot + (uint32_t)i) / (uint32_t)kMlpSlots) & 1u, err);
+    return smem_u32(smem + MlpSmem::wring(st));
+  };
+  // slot i retired by both warpgroups -> its stage takes slot i + 3
+  auto release = [&](int i) {
+    __syncthreads();
+    if (tid == 0 && i + kMlpSlots < NS) load(i + kMlpSlots);
+  };
+  auto mma = [&](float (&d)[D / 2], uint32_t a, uint32_t w, int accumulate) {
+    if constexpr (D == 256) wgmma_f16_n256(d, make_desc(a), make_desc(w), accumulate);
+    else wgmma_f16_n128(d, make_desc(a), make_desc(w), accumulate);
+  };
+  // The MMAs of one slot are straight-line code (no branch between them): control flow between wgmmas that share the
+  // accumulator makes the compiler fence every instruction.
+#pragma unroll 1
+  for (int kb = 0; kb < KB; ++kb) {
+    const uint32_t ah = smem_u32(smem + MlpSmem::abuf(kb, 0)) + wg * 8192, al = smem_u32(smem + MlpSmem::abuf(kb, 1)) + wg * 8192;
+    const uint32_t whi = acquire(2 * kb);
+    wgmma_fence();
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      split_half2(v[8 * q + 2 * e], v[8 * q + 2 * e + 1], h[e], l[e]);
+    for (int k = 0; k < 4; ++k) {  // 16 halves = 32 bytes per instruction
+      mma(acc, al + 32 * k, whi + 32 * k, (kb | k) ? 1 : 0);
+      mma(acc, ah + 32 * k, whi + 32 * k, 1);
     }
-    const int off = ((cbase + q) ^ (row & 7)) << 4;
-    *(uint4*)(ph + off) = make_uint4(h[0], h[1], h[2], h[3]);
-    *(uint4*)(pl + off) = make_uint4(l[0], l[1], l[2], l[3]);
+    wgmma_commit();
+    wgmma_wait0();
+    fence_acc(acc);
+    release(2 * kb);
+    const uint32_t wlo = acquire(2 * kb + 1);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) mma(acc, ah + 32 * k, wlo + 32 * k, 1);
+    wgmma_commit();
+    wgmma_wait0();
+    fence_acc(acc);
+    release(2 * kb + 1);
+  }
+  nslot += NS;
+}
+
+// The rows a thread's accumulator fragment covers: tile rows fr and fr + 8, columns 8 j + fc + {0, 1}.
+struct Frag {
+  int fr, fc;
+  __device__ __forceinline__ Frag() {
+    const int tid = threadIdx.x, lane = tid & 31;
+    fr = 64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + (lane >> 2);
+    fc = 2 * (lane & 3);
+  }
+};
+
+// The three GEMMs of the MLP block with their epilogues, operand buffer holding O (scaled, split) on entry.  Per fragment row
+// h (tile rows fr, fr + 8): xin[h] residual X (nullptr: zero), aout[h] where A is parked (nullptr: row not stored), xout[h]
+// where X' goes (nullptr: not stored); operand_out: X' also becomes the operand buffer (next layer of the trunk).
+template <int D>
+__device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, uint64_t* full, uint32_t& nslot,
+                                     const CUtensorMap* wo_hi, const CUtensorMap* wo_lo, const CUtensorMap* w1_hi,
+                                     const CUtensorMap* w1_lo, const CUtensorMap* w2_hi, const CUtensorMap* w2_lo, float us0,
+                                     float us1, float us2, float a_scale, const float* sb1, const float* sb2,
+                                     const float* const (&xin)[2], float* const (&aout)[2], float* const (&xout)[2],
+                                     bool operand_out, int* err) {
+  const Frag f;
+  // Row loads are issued in batches of kJ fragment columns ahead of the stores: xin / aout / xout may alias, so the compiler
+  // would otherwise wait for every load behind the previous store.
+  constexpr int kJ = 4;
+  // ---- A = X + O Wo -> parked rows and the operand buffer
+  gemm_abuf<D>(acc, smem, full, nslot, wo_hi, wo_lo, 0, err);
+#pragma unroll
+  for (int jb = 0; jb < D / 8; jb += kJ) {
+    float2 x[kJ][2];
+#pragma unroll
+    for (int j = 0; j < kJ; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) x[j][h] = xin[h] ? *(const float2*)(xin[h] + 8 * (jb + j) + f.fc) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int j = 0; j < kJ; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = 8 * (jb + j) + f.fc;
+        const float a0 = x[j][h].x + acc[4 * (jb + j) + 2 * h] * us0, a1 = x[j][h].y + acc[4 * (jb + j) + 2 * h + 1] * us0;
+        if (aout[h]) *(float2*)(aout[h] + c) = make_float2(a0, a1);
+        store_operand_pair(smem, f.fr + 8 * h, c, a0 * a_scale, a1 * a_scale);
+      }
+  }
+  fence_proxy_async();
+  __syncthreads();
+  // ---- M1 = tanh(A W1 + b1) -> operand buffer
+  gemm_abuf<D>(acc, smem, full, nslot, w1_hi, w1_lo, 0, err);
+#pragma unroll
+  for (int j = 0; j < D / 8; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int c = 8 * j + f.fc;
+      const float m0 = mlp_tanh(acc[4 * j + 2 * h] * us1 + sb1[c]), m1 = mlp_tanh(acc[4 * j + 2 * h + 1] * us1 + sb1[c + 1]);
+      store_operand_pair(smem, f.fr + 8 * h, c, m0 * a_scale, m1 * a_scale);
+    }
+  fence_proxy_async();
+  __syncthreads();
+  // ---- X' = A + tanh(M1 W2 + b2)
+  gemm_abuf<D>(acc, smem, full, nslot, w2_hi, w2_lo, 0, err);
+#pragma unroll
+  for (int jb = 0; jb < D / 8; jb += kJ) {
+    float2 a[kJ][2];
+#pragma unroll
+    for (int j = 0; j < kJ; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) a[j][h] = aout[h] ? *(const float2*)(aout[h] + 8 * (jb + j) + f.fc) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int j = 0; j < kJ; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = 8 * (jb + j) + f.fc;
+        if (!aout[h]) continue;
+        const float x0 = a[j][h].x + mlp_tanh(acc[4 * (jb + j) + 2 * h] * us2 + sb2[c]);
+        const float x1 = a[j][h].y + mlp_tanh(acc[4 * (jb + j) + 2 * h + 1] * us2 + sb2[c + 1]);
+        if (xout[h]) *(float2*)(xout[h] + c) = make_float2(x0, x1);
+        if (operand_out) store_operand_pair(smem, f.fr + 8 * h, c, x0 * a_scale, x1 * a_scale);
+      }
   }
 }
 
+template <int D>
 __global__ void __launch_bounds__(kMlpThreads, 1)
 mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_constant__ CUtensorMap wo_lo,
                      const __grid_constant__ CUtensorMap w1_hi, const __grid_constant__ CUtensorMap w1_lo,
                      const __grid_constant__ CUtensorMap w2_hi, const __grid_constant__ CUtensorMap w2_lo, MlpParams p) {
   DQMC_TC_SMEM(smem);
   if ((smem_u32(smem) & 1023u) != 0u) tc_trap();
-  uint64_t* bars = (uint64_t*)(smem + MlpSmem::bars());
-  uint64_t* afull = bars;                 // [4] operand k-block kb written (128 worker threads each)
-  uint64_t* wfull = bars + 4;             // [kMlpStages] weight plane landed (TMA tx)
-  uint64_t* wempty = bars + 4 + kMlpStages;      // [kMlpStages] weight plane consumed (tcgen05.commit)
-  uint64_t* accfull = bars + 4 + 2 * kMlpStages;  // accumulator of the current GEMM complete (tcgen05.commit)
-  uint64_t* tmemfree = accfull + 1;       // all 256 workers are done with the tile's TMEM contents
-  uint32_t* tmem_slot = (uint32_t*)(tmemfree + 1);
+  uint64_t* full = (uint64_t*)(smem + MlpSmem::bars());  // [kMlpSlots] weight slot landed (TMA tx)
   float* sb1 = (float*)(smem + MlpSmem::bias());
   float* sb2 = sb1 + 256;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int d = p.d, KB = d / 64;
+  const int tid = threadIdx.x;
   const int MT = (p.M + 127) / 128;
 
-  if (threadIdx.x == 0) {
-    for (int k = 0; k < 4; ++k) mbar_init(&afull[k], 128);
-    for (int s = 0; s < kMlpStages; ++s) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], 1); }
-    mbar_init(accfull, 1);
-    mbar_init(tmemfree, 256);
+  if (tid == 0) {
+    for (int i = 0; i < kMlpSlots; ++i) mbar_init(&full[i], 1);
     fence_barrier_init();
-  }
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-    sb1[i] = i < d ? p.b1[i] : 0.f;
-    sb2[i] = i < d ? p.b2[i] : 0.f;
-  }
-  if (warp == 9) tmem_alloc(tmem_slot, 512);
-  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&wo_hi); tma_prefetch_desc(&wo_lo); tma_prefetch_desc(&w1_hi);
     tma_prefetch_desc(&w1_lo); tma_prefetch_desc(&w2_hi); tma_prefetch_desc(&w2_lo);
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 8) {
-    // ===================== weight planes: Wo, W1, W2 of every tile, k-block by k-block, hi then lo ==========
-    if (elect_one()) {
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
-        for (int g = 0; g < 3; ++g) {
-          const CUtensorMap* mh = g == 0 ? &wo_hi : (g == 1 ? &w1_hi : &w2_hi);
-          const CUtensorMap* ml = g == 0 ? &wo_lo : (g == 1 ? &w1_lo : &w2_lo);
-          for (int kb = 0; kb < KB; ++kb)
-            for (int plane = 0; plane < 2; ++plane, ++it) {
-              const int s = it % kMlpStages;
-              const uint32_t ph = (it / kMlpStages) & 1;
-              mbar_wait(&wempty[s], ph ^ 1, p.err_flag);
-              mbar_expect_tx(&wfull[s], (uint32_t)d * 128u);
-              tma_load_2d(plane == 0 ? mh : ml, &wfull[s], smem + MlpSmem::wring(s), kb * 64, 0);
-            }
-        }
-      }
-    }
-  } else if (warp == 9) {
-    // ===================== MMA issuer =========================================================================
-    const uint32_t idesc = make_idesc_f16(128, d);
-    uint32_t it = 0, tcount = 0, gcount = 0;
-    for (int tile = blockIdx.x; tile < MT; tile += gridDim.x, ++tcount) {
-      mbar_wait(tmemfree, (tcount & 1) ^ 1, p.err_flag);  // previous tile's epilogues have drained TMEM
-      tc_fence_after();
-      for (int g = 0; g < 3; ++g, ++gcount) {
-        const uint32_t d_tmem = tmem_base + (g == 0 ? 0u : 256u);
-        const uint32_t aph = gcount & 1;  // afull[kb] completes once per GEMM
-        if (g > 0)  // the operand comes from the previous epilogue, which also reads the accumulator this GEMM overwrites
-          for (int kb = 0; kb < KB; ++kb) mbar_wait(&afull[kb], aph, p.err_flag);
-        for (int kb = 0; kb < KB; ++kb) {
-          if (g == 0) mbar_wait(&afull[kb], aph, p.err_flag);
-          const uint32_t ah = smem_u32(smem + MlpSmem::abuf(kb, 0)), al = smem_u32(smem + MlpSmem::abuf(kb, 1));
-          for (int plane = 0; plane < 2; ++plane, ++it) {
-            const int s = it % kMlpStages;
-            const uint32_t ph = (it / kMlpStages) & 1;
-            mbar_wait(&wfull[s], ph, p.err_flag);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint32_t w = smem_u32(smem + MlpSmem::wring(s));
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint32_t ko = k * 32;  // 16 halves per instruction
-                if (plane == 0) {
-                  umma_f16(d_tmem, make_desc(al + ko), make_desc(w + ko), idesc, (kb | k) ? 1u : 0u);
-                  umma_f16(d_tmem, make_desc(ah + ko), make_desc(w + ko), idesc, 1u);
-                } else {
-                  umma_f16(d_tmem, make_desc(ah + ko), make_desc(w + ko), idesc, 1u);
-                }
-              }
-              umma_commit(&wempty[s]);
-              if (kb == KB - 1 && plane == 1) umma_commit(accfull);
-            }
-            __syncwarp();
-          }
-        }
-      }
-    }
-  } else {
-    // ===================== workers: warps 0-7 ===================================================================
-    const int q4 = warp & 3, half = warp >> 2;       // TMEM lane quarter / tile rows 32 q4 .. +31; column half
-    const int trow = 32 * q4 + lane;                  // this thread's tile row (= TMEM lane)
-    const uint32_t tlane = (uint32_t)(32 * q4) << 16;
-    const int nchunk = d / 32;                        // 32-column chunks per row
-    const int c_lo = half * (nchunk / 2), c_hi = (half + 1) * (nchunk / 2);  // this warp's chunks = its KB / 2 k-blocks
-    uint32_t gcount = 0;
-    for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
-      const int row = tile * 128 + trow;
-      const bool valid = row < p.M;
-      // ---- stage the O tile: coalesced float4 loads (8 lanes x 16 B per row), hi / lo split, k-blocks of this warp's half.
-      // Rows of one instruction differ in bit 2 within each half-warp: the 8-byte stores are then conflict-free.
-      {
-        const int cq = lane & 7, rs = lane >> 3;
-        for (int kb = half * (KB / 2); kb < (half + 1) * (KB / 2); ++kb) {  // KB is 2 or 4 (d = 128 | 256)
-          unsigned char* ph = smem + MlpSmem::abuf(kb, 0);
-          unsigned char* pl = smem + MlpSmem::abuf(kb, 1);
-#pragma unroll 4
-          for (int j = 0; j < 16; ++j) {                 // 8 row groups x 2 halves of the 64-float k-block
-            const int seg = j & 1, jj = j >> 1;
-            const int r = 32 * q4 + (jj >> 1) * 8 + 4 * (rs & 1) + (rs >> 1) + 2 * (jj & 1);
-            const int grow = tile * 128 + r;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (grow < p.M) v = __ldg((const float4*)(p.O + (size_t)grow * p.ldo + kb * 64 + seg * 32 + cq * 4));
-            const float sc = p.a_scale;
-            const float x0 = v.x * sc, x1 = v.y * sc, x2 = v.z * sc, x3 = v.w * sc;
-            const uint32_t h01 = pack_half2_rn(x0, x1), h23 = pack_half2_rn(x2, x3);
-            const uint32_t l01 = pack_half2_rn(x0 - half_bits_to_float(h01 & 0xFFFFu), x1 - half_bits_to_float(h01 >> 16));
-            const uint32_t l23 = pack_half2_rn(x2 - half_bits_to_float(h23 & 0xFFFFu), x3 - half_bits_to_float(h23 >> 16));
-            const int c16 = seg * 4 + (cq >> 1);
-            const int off = (r >> 3) * 1024 + (r & 7) * 128 + ((c16 ^ (r & 7)) << 4) + (cq & 1) * 8;
-            *(uint2*)(ph + off) = make_uint2(h01, h23);
-            *(uint2*)(pl + off) = make_uint2(l01, l23);
-          }
-          fence_proxy_async();
-          mbar_arrive(&afull[kb]);
-        }
-      }
-      // ---- epilogue 1: A = X + O Wo -> TMEM [0, d) (fp32) and the operand buffer
-      mbar_wait(accfull, gcount & 1, p.err_flag);
-      ++gcount;
-      tc_fence_after();
-      for (int c = c_lo; c < c_hi; ++c) {
-        float4 xr[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          xr[i] = valid ? __ldg((const float4*)(p.X + (size_t)row * p.ldx + c * 32 + 4 * i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        uint32_t v[32];
-        tmem_ld32(tmem_base + tlane + (uint32_t)(c * 32), v);
-        tmem_ld_wait();
-        float a[32];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          a[4 * i] = xr[i].x + __uint_as_float(v[4 * i]) * p.us0;
-          a[4 * i + 1] = xr[i].y + __uint_as_float(v[4 * i + 1]) * p.us0;
-          a[4 * i + 2] = xr[i].z + __uint_as_float(v[4 * i + 2]) * p.us0;
-          a[4 * i + 3] = xr[i].w + __uint_as_float(v[4 * i + 3]) * p.us0;
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(a[i]);
-        tmem_st32(tmem_base + tlane + (uint32_t)(c * 32), v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) a[i] *= p.a_scale;
-        store_operand_chunk(smem, trow, c * 32, a);
-        if (c & 1) {  // second chunk of a k-block: hand it to the MMA warp
-          tmem_st_wait();
-          fence_proxy_async();
-          tc_fence_before();
-          mbar_arrive(&afull[c >> 1]);
-        }
-      }
-      // ---- epilogue 2: M1 = tanh(A W1 + b1) -> operand buffer
-      mbar_wait(accfull, gcount & 1, p.err_flag);
-      ++gcount;
-      tc_fence_after();
-      for (int c = c_lo; c < c_hi; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + tlane + (uint32_t)(256 + c * 32), v);
-        tmem_ld_wait();
-        float a[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) a[i] = mlp_tanh(__uint_as_float(v[i]) * p.us1 + sb1[c * 32 + i]) * p.a_scale;
-        store_operand_chunk(smem, trow, c * 32, a);
-        if (c & 1) {
-          fence_proxy_async();
-          tc_fence_before();
-          mbar_arrive(&afull[c >> 1]);
-        }
-      }
-      // ---- epilogue 3: X' = A + tanh(M1 W2 + b2) -> HBM
-      mbar_wait(accfull, gcount & 1, p.err_flag);
-      ++gcount;
-      tc_fence_after();
-      for (int c = c_lo; c < c_hi; ++c) {
-        uint32_t v[32], r[32];
-        tmem_ld32(tmem_base + tlane + (uint32_t)(256 + c * 32), v);
-        tmem_ld32(tmem_base + tlane + (uint32_t)(c * 32), r);
-        tmem_ld_wait();
-        if (valid) {
-          float* op = p.Out + (size_t)row * p.ldout + c * 32;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float4 o;
-            o.x = __uint_as_float(r[4 * i]) + mlp_tanh(__uint_as_float(v[4 * i]) * p.us2 + sb2[c * 32 + 4 * i]);
-            o.y = __uint_as_float(r[4 * i + 1]) + mlp_tanh(__uint_as_float(v[4 * i + 1]) * p.us2 + sb2[c * 32 + 4 * i + 1]);
-            o.z = __uint_as_float(r[4 * i + 2]) + mlp_tanh(__uint_as_float(v[4 * i + 2]) * p.us2 + sb2[c * 32 + 4 * i + 2]);
-            o.w = __uint_as_float(r[4 * i + 3]) + mlp_tanh(__uint_as_float(v[4 * i + 3]) * p.us2 + sb2[c * 32 + 4 * i + 3]);
-            *(float4*)(op + 4 * i) = o;
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(tmemfree);
-    }
+  for (int i = tid; i < D; i += blockDim.x) {
+    sb1[i] = p.b1[i];
+    sb2[i] = p.b2[i];
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  const Frag f;
+  uint32_t nslot = 0;
+  float acc[D / 2];
+  for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
+    // ---- stage the O tile: coalesced float4 loads, hi / lo split
+    for (int idx = tid; idx < 128 * (D / 4); idx += kMlpThreads) {
+      const int r = idx / (D / 4), c = 4 * (idx % (D / 4));
+      const int grow = tile * 128 + r;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (grow < p.M) v = __ldg((const float4*)(p.O + (size_t)grow * p.ldo + c));
+      const float sc = p.a_scale;
+      store_operand_quad(smem, r, c, make_float4(v.x * sc, v.y * sc, v.z * sc, v.w * sc));
+    }
+    fence_proxy_async();
+    __syncthreads();  // also: every O row of the tile has been read before A is parked in the (possibly aliasing) Out rows
+    const float* xin[2];
+    float* aout[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int grow = tile * 128 + f.fr + 8 * h;
+      const bool valid = grow < p.M;
+      xin[h] = valid ? p.X + (size_t)grow * p.ldx : nullptr;
+      aout[h] = valid ? p.Out + (size_t)grow * p.ldout : nullptr;
+    }
+    mlp3<D>(acc, smem, full, nslot, &wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo, p.us0, p.us1, p.us2, p.a_scale, sb1, sb2,
+            xin, aout, aout, false, p.err_flag);
   }
 }
 

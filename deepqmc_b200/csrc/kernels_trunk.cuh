@@ -223,7 +223,7 @@ inline size_t embed_fwd_smem_bytes(int M, int d) {
 // ------------------------------------------------------------------------------------------
 // Row GEMM  C[row(m), :] = (Res[row(m), :]) + A[row(m), :] @ W + (bias on value rows)
 // Plain SIMT tiling (CUDA cores), used for the fp64 parity mode and as the reference
-// implementation the tcgen05 fp32 path is validated against.
+// implementation the tensor-core fp32 path is validated against.
 // sliced == 1: blockIdx.z = electron e, rows m = (b, s) -> physical row (b*Nel + e)*S + s,
 //              weights W0 for e < z_split else W1 (per-spin backflow heads, wf/omni.py:43-88).
 // ------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// Whole Psiformer trunk of a plain forward (S = 1) in ONE persistent launch on the 5th-gen tensor cores.
+// Whole Psiformer trunk of a plain forward (S = 1) in ONE persistent launch on the Hopper tensor cores (wgmma).
 //
 //   for every layer l:   QKV = X Wqkv                                   (reference: gnn/update_features.py:241-286,
 //                        O   = softmax(Q K^T / sqrt(dh)) V  per head      hk.MultiHeadAttention, algebra hkext.py:215-253;
@@ -6,35 +6,17 @@
 //                        X   = A + tanh(tanh(A W1 + b1) W2 + b2)          conf/ansatz/psiformer.yaml:70-101)
 //
 // A CTA owns a tile of G = 128 / NP walkers (NP = electrons per walker rounded up to a power of two, tile row = walker slot x
-// NP + electron) and carries it through ALL layers: the residual stream stays in TMEM columns [0, 256) as fp32, the operand of
-// the next GEMM is written by the previous stage straight into the 128-byte-swizzled K-major operand buffer in shared memory
-// ("3xFP16" hi / lo halves, see gemm_tcgen05.cuh), and HBM sees the embedding rows once on the way in and the trunk output
-// once on the way out (2 x 1 KB per row per forward instead of ~11 KB per row and LAYER with one launch per dense layer /
-// attention).  Only the weights stream (TMA, 16 KB slots of 128 W^T rows x 64 halves, 6-slot ring) -- and Q / K / V of the
-// tile, which make one round trip through a per-CTA scratch buffer (384 KB, re-used for every tile and layer, i.e. L2
-// resident): the QKV projection of ALL heads has to finish before the operand buffer can be re-used, and neither shared
-// memory (224 KB taken) nor TMEM (residual + accumulator) can park 128 x 768 values.  The drain writes them as ready-made
-// operand images (scaled, split into hi / lo halves, swizzled; V transposed), which come back per head by ONE bulk copy each
-// into the (then idle) weight ring.
+// NP + electron) and carries it through ALL layers.  The operand of every dense GEMM is written by the previous stage straight
+// into the 128-byte-swizzled K-major operand buffer in shared memory ("3xFP16" hi / lo halves, see gemm_wgmma.cuh); the
+// dense GEMMs are those of the fused MLP block (fused_tc.cuh: wgmma m64 n256, accumulators in registers, weights streamed
+// by TMA).  HBM sees the embedding rows once on the way in and the trunk output once on the way out; the residual stream
+// (128 x 256 fp32) and Q / K / V (128 x 768 fp32) of the tile live in a per-CTA scratch buffer (512 KB, re-used for every
+// tile and layer, i.e. L2 resident): the register file holds one accumulator, and shared memory (operand buffer + ring)
+// cannot park them.
 //
-// Attention on tcgen05 as well, one head at a time for the whole tile:
-//   S = Q_h K_h^T      M = 128 (all rows of the tile), N = 128 (all keys of the tile), K = 64: only the diagonal blocks
-//                      (keys of the row's own walker) are used -- the 4 .. 32x redundant products cost 12 instructions;
-//   P = softmax        thread <-> row: 32 accumulator columns (the row's 32-key window), masked to its walker, written
-//                      back IN PLACE as packed hi / lo halves with explicit zeros outside the window: P never leaves TMEM
-//                      (A operand from tensor memory);
-//   O_h = P V_h        M = 128, N = 64, K = 128 keys; B = V_h^T image; result normalised by the row sum in the epilogue
-//                      and written as k-block h of the Wo operand.
-//
-// warp roles (320 threads):
-//   warps 0-7  workers: tile load, QKV drain, softmax, attention-output and the three MLP epilogues.  Warp w owns TMEM lanes /
-//                       tile rows 32 (w % 4) .. +31 and the column half w / 4.
-//   warp  8    TMA    : weight slots of every GEMM in issue order, Q / K / V^T images of every head.
-//   warp  9    MMA    : tcgen05.mma kind::f16, M = 128, N = 128 throughout: QKV as six sub-chunks and Wo / W1 / W2 as two
-//                       output halves each, alternating between the two halves of the accumulator -- the drain / epilogue
-//                       of one half (by the workers of that column half) overlaps the MMAs of the next.
-// TMEM (512 columns): [0, 256) residual stream X, then A;  [256, 512) accumulator; during attention [256, 384) S -> P,
-//                     [384, 448) / [448, 512) O_h (alternating).
+// Attention, one head at a time for the whole tile: K_h and V_h of the tile are staged in the (then idle) weight ring as
+// fp32; two threads per tile row (32 head columns each) run an online softmax over the keys of the row's own walker and write
+// O_h straight into k-block h of the Wo operand.
 #pragma once
 #include <cstdint>
 
@@ -45,11 +27,11 @@
 namespace dq {
 namespace tc {
 
-constexpr int kTrThreads = 320;
-constexpr int kTrSlots = 6;
+constexpr int kTrThreads = 256;
 constexpr int kTrMaxLayers = 8;
-constexpr int kTrHeadImage = 96 * 1024;             // per head: Q hi, Q lo, K hi, K lo (16 KB each), V^T hi, V^T lo (16 KB each)
-constexpr int kTrScratchPerCta = 4 * kTrHeadImage;  // 4 heads
+constexpr int kTrQkvBytes = 128 * 768 * 4;                   // Q | K | V rows of the tile, fp32
+constexpr int kTrScratchPerCta = kTrQkvBytes + 128 * 256 * 4;  // + residual stream rows
+using TrSmem = MlpSmem;
 
 struct TrunkParams {
   const float* X0; int ldx;      // embedding rows [rows][256]  (vper > 0: [walkers][256], the moved electron's row only)
@@ -57,7 +39,7 @@ struct TrunkParams {
   long long v0; int vper;        //   [base][N][256]; walker w of this launch is virtual walker v0 + w = base (v0 + w) / vper
                                  //   with electron ((v0 + w) / 12) % N moved (ecp_points_kernel layout)
   float* Out; int ldout;         // trunk output rows [rows][256]
-  const CUtensorMap* maps;       // device array [L][4][2]: (Wqkv, Wo, W1, W2) x (hi, lo); boxes of 64 halves x 128 rows
+  const CUtensorMap* maps;       // device array [L][4][2]: (Wqkv, Wo, W1, W2) x (hi, lo); boxes of 64 halves x 256 rows
   const float* b1[kTrMaxLayers];
   const float* b2[kTrMaxLayers];
   float us[kTrMaxLayers][4];     // accumulator unscale of the four GEMMs of a layer: 1 / (a_scale * weight scale)
@@ -66,693 +48,167 @@ struct TrunkParams {
   float a_scale;                 // power of two applied to activations before the hi / lo split
   float attn_scale;              // 1 / sqrt(dh)
   int* err_flag;
-  long long* trace;              // development aid (DQMC_TRUNK_TRACE): clock64 stamps of block 0, one steady-state tile, layer 1
-  int ablate;                    // development aid (DQMC_TRUNK_ABLATE, results are garbage): 1 no weight loads, 2 no MMAs,
-                                 // 4 no Q/K/V image stores, 8 no image loads
 };
 
-struct TrSmem {
-  static __host__ __device__ int abuf(int kb, int plane) { return (kb * 2 + plane) * 16384; }  // [128 rows][128 B]
-  static __host__ __device__ int wring(int s) { return 131072 + s * 16384; }                     // [128 rows][128 B]
-  static __host__ __device__ int bias() { return 131072 + kTrSlots * 16384; }                    // b1[256], b2[256]
-  static __host__ __device__ int bars() { return bias() + 2048; }
-  static __host__ __device__ int total() { return bars() + 512; }
-};
-
-__device__ __forceinline__ void tr_split2(float x0, float x1, uint32_t& hi, uint32_t& lo) { split_half2(x0, x1, hi, lo); }
-
-// 32 columns (c0 .. c0 + 31 of a 64-wide head) of tile row `row` -> K-major operand image planes [128 rows][64 halves] in GLOBAL
-// memory (hi at img, lo at img + 16 KB) in the UNSWIZZLED canonical layout: 16-byte chunk c of row r at
-// (r / 8) 1024 + c 128 + (r % 8) 16 (core matrices of 8 rows x 16 bytes, leading byte offset 128, stride byte offset 1024).
-// A warp (lane = row) then writes 4 complete 128-byte lines per store instruction; with the swizzled row-major image every
-// instruction touched 32 lines, which made the Q / K drains 3x slower than the tensor pipe that feeds them.
-__device__ __forceinline__ void image_store32(unsigned char* img, int row, int c0, const float* x) {
-  unsigned char* ph = img + (row >> 3) * 1024 + (row & 7) * 16;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) tr_split2(x[8 * q + 2 * e], x[8 * q + 2 * e + 1], h[e], l[e]);
-    const int off = ((c0 >> 3) + q) * 128;
-    *(uint4*)(ph + off) = make_uint4(h[0], h[1], h[2], h[3]);
-    *(uint4*)(ph + 16384 + off) = make_uint4(l[0], l[1], l[2], l[3]);
-  }
-}
-// V^T image: element (row = head column c, k = key = tile row): two k-blocks of 64 keys, [64 rows][128 B] = 8 KB each per
-// plane (hi at img, lo at img + 16 KB)
-__device__ __forceinline__ void image_store_vt32(unsigned char* img, int key, int c0, const float* x) {
-  // lanes come in (even key, odd key) pairs: the even lane stores the packed pair for the even columns, the odd lane for
-  // the odd ones -- 32-bit stores, one shuffle per column
-  const bool odd = key & 1;
-  unsigned char* base = img + (key >> 6) * 8192 + ((key & 6) << 1);
-  const int kc = (key & 63) >> 3;
-#pragma unroll
-  for (int i = 0; i < 32; i += 2) {
-    const float mine = odd ? x[i + 1] : x[i], give = odd ? x[i] : x[i + 1];
-    const float got = __shfl_xor_sync(0xffffffffu, give, 1);  // the partner's value of MY column
-    uint32_t h, l;
-    split_half2(odd ? got : mine, odd ? mine : got, h, l);     // (even key, odd key)
-    const int c = c0 + i + (odd ? 1 : 0);
-    const int off = (c >> 3) * 1024 + (c & 7) * 128 + ((kc ^ (c & 7)) << 4);
-    *(uint32_t*)(base + off) = h;
-    *(uint32_t*)(base + 16384 + off) = l;
-  }
-}
-
-// 32 scaled values -> 16 packed hi pairs (v[0..15]) and 16 packed lo pairs (v[16..31])
-__device__ __forceinline__ void pack_operand32(const float* a, uint32_t* v) {
-#pragma unroll
-  for (int i = 0; i < 16; ++i) split_half2(a[2 * i], a[2 * i + 1], v[i], v[16 + i]);
-}
-// ... and those 32 words into the swizzled K-major operand buffer (columns c0 .. c0 + 31 of tile row `row`)
-__device__ __forceinline__ void store_operand_packed(unsigned char* smem, int row, int c0, const uint32_t* v) {
-  const int kb = c0 >> 6, cbase = ((c0 >> 5) & 1) * 4;
-  unsigned char* ph = smem + TrSmem::abuf(kb, 0) + (row >> 3) * 1024 + (row & 7) * 128;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int off = ((cbase + q) ^ (row & 7)) << 4;
-    *(uint4*)(ph + off) = make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-    *(uint4*)(ph + 16384 + off) = make_uint4(v[16 + 4 * q], v[16 + 4 * q + 1], v[16 + 4 * q + 2], v[16 + 4 * q + 3]);
-  }
-}
-
-// ---- TS variant: the A operand of the dense GEMMs lives in TENSOR MEMORY (columns [0, 128) hi halves, [128, 256) lo halves,
-// two K values per 32-bit cell), the residual stream moves to the shared memory the operand buffer occupied.  An M = 128,
-// N = 128, K = 16 kind::f16 instruction with both operands in shared memory fetches 8 KB per instruction; measured on the SS
-// kernel it retires one such instruction per 128 clocks (the tensor pipe itself needs 64: ncu shows it 50 % active while the
-// MMAs run back to back), i.e. operand fetch at ~64 B / clock bounds it.  With A in tensor memory only the weight slice (4 KB)
-// comes from shared memory.
-// residual rows in shared memory: [128 rows][256 fp32], 16-byte chunk q of row r at r 1024 + ((q & ~7) | ((q ^ r) & 7)) 16:
-// a warp (lane = row) reading the same logical chunk of 32 consecutive rows is conflict-free (8 lanes of a phase -> 8 bank groups)
-__device__ __forceinline__ float4* resid_chunk(unsigned char* smem, int row, int q) {
-  return (float4*)(smem + row * 1024 + (((q & ~7) | ((q ^ row) & 7)) << 4));
-}
-__device__ __forceinline__ void resid_load32(unsigned char* smem, int row, int c0, float* x) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4 v = *resid_chunk(smem, row, (c0 >> 2) + i);
-    x[4 * i] = v.x; x[4 * i + 1] = v.y; x[4 * i + 2] = v.z; x[4 * i + 3] = v.w;
-  }
-}
-__device__ __forceinline__ void resid_store32(unsigned char* smem, int row, int c0, const float* x) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i) *resid_chunk(smem, row, (c0 >> 2) + i) = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
-}
-// 32 packed words (16 hi pairs, 16 lo pairs of columns c0 .. c0 + 31) -> operand cells of this thread's TMEM lane
-__device__ __forceinline__ void store_operand_tmem(uint32_t tlane_base, int c0, const uint32_t* v) {
-  tmem_st16(tlane_base + (uint32_t)(c0 >> 1), v);
-  tmem_st16(tlane_base + 128u + (uint32_t)(c0 >> 1), v + 16);
-}
-
-template <bool TS>
 __global__ void __launch_bounds__(kTrThreads, 1)
 trunk_f16_kernel(TrunkParams p) {
   DQMC_TC_SMEM(smem);
   if ((smem_u32(smem) & 1023u) != 0u) tc_trap();
-  uint64_t* bars = (uint64_t*)(smem + TrSmem::bars());
-  uint64_t* afull = bars;                       // [4]  operand k-block written by an epilogue / the tile load (128 threads)
-  uint64_t* ofull = bars + 4;                   // [4]  operand k-block h = attention output of head h (256 threads)
-  uint64_t* wfull = bars + 8;                   // [kTrSlots] weight slot landed (TMA tx)
-  uint64_t* wempty = bars + 8 + kTrSlots;       // [kTrSlots] weight slot consumed (tcgen05.commit)
-  uint64_t* accfull = bars + 8 + 2 * kTrSlots;  // [2]  accumulator (half) complete (tcgen05.commit)
-  uint64_t* accfree = accfull + 2;              // [2]  accumulator half drained by all 256 workers
-  uint64_t* scr_full = accfree + 2;             // Q / K / V images of the tile are in the scratch buffer (1 elected arrival)
-  uint64_t* qk_full = scr_full + 1;             // Q_h, K_h images landed in ring slots 0-3 (TMA tx)
-  uint64_t* v_full = qk_full + 1;               // V_h^T image landed in ring slots 4-5 (TMA tx)
-  uint64_t* qk_free = v_full + 1;               // S = Q K^T issued and retired (commit)
-  uint64_t* v_free = qk_free + 1;               // O = P V retired (commit)
-  uint64_t* s_full = v_free + 1;                // S complete in TMEM (commit)
-  uint64_t* p_full = s_full + 1;                // P written back by all 256 workers
-  uint64_t* o_full = p_full + 1;                // [2] O_h complete in TMEM (commit)
-  uint64_t* o_free = o_full + 2;                // [2] O_h buffer read by all 256 workers
-  uint64_t* scr_qk = o_free + 2;                // Q / K images of the tile are in the scratch buffer (V^T: scr_full)
-  uint32_t* tmem_slot = (uint32_t*)(scr_qk + 1);
+  uint64_t* full = (uint64_t*)(smem + TrSmem::bars());
   float* sb1 = (float*)(smem + TrSmem::bias());
   float* sb2 = sb1 + 256;
+  float* kst = (float*)(smem + TrSmem::wring(0));  // attention: K_h [128][64] fp32
+  float* vst = (float*)(smem + TrSmem::wring(1));  //            V_h [128][64] fp32
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x;
   const int N = p.N, NP = p.NP, L = p.L;
+  const int lnp = 31 - __clz(NP);                // NP is a power of two
   const int G = 128 / NP;                        // walker slots per tile
   const int MT = (p.walkers + G - 1) / G;
-  unsigned char* scratch = p.scratch + (size_t)blockIdx.x * kTrScratchPerCta;
+  float* qkv = (float*)(p.scratch + (size_t)blockIdx.x * kTrScratchPerCta);  // [128][768]
+  float* resid = qkv + 128 * 768;                                            // [128][256]
 
-  if (threadIdx.x == 0) {
-    for (int k = 0; k < 4; ++k) { mbar_init(&afull[k], 128); mbar_init(&ofull[k], 256); }
-    for (int s = 0; s < kTrSlots; ++s) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], 1); }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&accfull[b], 1); mbar_init(&accfree[b], 256);
-      mbar_init(&o_full[b], 1); mbar_init(&o_free[b], 256);
-    }
-    mbar_init(scr_full, 1); mbar_init(scr_qk, 1); mbar_init(qk_full, 1); mbar_init(v_full, 1); mbar_init(qk_free, 1); mbar_init(v_free, 1);
-    mbar_init(s_full, 1); mbar_init(p_full, 256);
+  if (tid == 0) {
+    for (int i = 0; i < kMlpSlots; ++i) mbar_init(&full[i], 1);
     fence_barrier_init();
-  }
-  if (warp == 9) tmem_alloc(tmem_slot, 512);
-  if (warp == 8 && lane == 0)
     for (int i = 0; i < 8 * L; ++i) tma_prefetch_desc(p.maps + i);
-  tc_fence_before();
+  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 8) {
-    // ===================== weight slots in issue order + the attention operand images ===========================
-    if (elect_one()) {
-      uint32_t it = 0, n_scr = 0, n_qkf = 0, n_vf = 0;
-      auto weight_slot = [&](const CUtensorMap* map, int x, int y) {
-        const int s = it % kTrSlots;
-        mbar_wait(&wempty[s & ~1], ((it / kTrSlots) & 1) ^ 1, p.err_flag);  // one release barrier per k-block (slot pair)
-        if (p.ablate & 1) {
-          mbar_arrive(&wfull[s]);
-        } else {
-          mbar_expect_tx(&wfull[s], 16384u);
-          tma_load_2d(map, &wfull[s], smem + TrSmem::wring(s), x, y);
-        }
-        ++it;
-      };
-      for (int tile = blockIdx.x; tile < MT; tile += gridDim.x)
-        for (int l = 0; l < L; ++l) {
-          const CUtensorMap* lm = p.maps + 8 * l;
-          for (int j = 0; j < 6; ++j)  // QKV: six 128-row sub-chunks of Wqkv^T
-            for (int kb = 0; kb < 4; ++kb)
-              for (int plane = 0; plane < 2; ++plane) weight_slot(lm + plane, kb * 64, 128 * j);
-          // the ring is handed to the attention: every weight slot issued so far has been consumed, the images are written
-          for (uint32_t k = it - kTrSlots; k != it; k += 2) mbar_wait(&wempty[k % kTrSlots], (k / kTrSlots) & 1, p.err_flag);
-          // Q / K images first (drains of sub-chunks 0-3); the V^T drains (4, 5) still run while head 0's Q / K load, S and
-          // softmax proceed
-          mbar_wait(scr_qk, n_scr & 1, p.err_flag);
-          for (int h = 0; h < 4; ++h) {
-            const unsigned char* img = scratch + (size_t)h * kTrHeadImage;
-            if (h > 0) { mbar_wait(qk_free, n_qkf & 1, p.err_flag); ++n_qkf; }
-            if (p.ablate & 8) {
-              mbar_arrive(qk_full);
-            } else {
-              mbar_expect_tx(qk_full, 65536u);
-              bulk_load(smem + TrSmem::wring(0), img, 65536u, qk_full);
-            }
-            if (h > 0) { mbar_wait(v_free, n_vf & 1, p.err_flag); ++n_vf; }
-            else { mbar_wait(scr_full, n_scr & 1, p.err_flag); ++n_scr; }
-            if (p.ablate & 8) {
-              mbar_arrive(v_full);
-            } else {
-              mbar_expect_tx(v_full, 32768u);
-              bulk_load(smem + TrSmem::wring(4), img + 65536, 32768u, v_full);
-            }
-          }
-          // ... and back: slots 0-3 once the last S is done, slots 4-5 once the last P V is done (ring position is 0 here).
-          // Wo, W1, W2: output halves [0, 128) and [128, 256) one after the other (the epilogue of a half overlaps the MMAs
-          // of the next half / GEMM)
-          for (int g = 1; g < 4; ++g)
-            for (int hb = 0; hb < 2; ++hb)
-              for (int kb = 0; kb < 4; ++kb)
-                for (int plane = 0; plane < 2; ++plane) {
-                  if (g == 1 && hb == 0 && kb == 0 && plane == 0) { mbar_wait(qk_free, n_qkf & 1, p.err_flag); ++n_qkf; }
-                  if (g == 1 && hb == 0 && kb == 2 && plane == 0) { mbar_wait(v_free, n_vf & 1, p.err_flag); ++n_vf; }
-                  weight_slot(lm + 2 * g + plane, kb * 64, 128 * hb);
-                }
-        }
-    }
-  } else if (warp == 9) {
-    // ===================== MMA issuer: ONE elected thread runs the whole loop (waits included) =====================
-    if (elect_one()) {
-    const uint32_t idesc64 = make_idesc_f16(128, 64), idesc128 = make_idesc_f16(128, 128);
-    const bool mma_on = !(p.ablate & 2);
-    // one k-block (64 K values) of a dense GEMM: ring slots it (hi plane of W^T) and it + 1 (lo plane) -> 12 instructions
-    // (A_lo W_hi + A_hi W_hi + A_hi W_lo per 16-wide k-step) issued after ONE pair of waits; the last k-block also commits the
-    // accumulator barrier
-    // tcgen05.commit costs ~150 clocks of tensor-pipe idle time per commit EVENT (tools/microbench/umma_rate.cu: 74.8 clocks per
-    // instruction without commits, 87.4 with one every 12 instructions, 99 with one every 6): one event per k-block (both ring
-    // slots + the accumulator barrier back to back).  Releasing the slots one k-block late (commit behind the NEXT k-block's
-    // instructions) was measured slower: the 3-k-block ring then starves the weight stream.
-    auto dense_kblock = [&](int kb, uint32_t d_tmem, uint32_t it0, uint64_t* accbar) {
-      const int s0 = it0 % kTrSlots, s1 = (it0 + 1) % kTrSlots;
-      mbar_wait(&wfull[s0], (it0 / kTrSlots) & 1, p.err_flag);
-      mbar_wait(&wfull[s1], ((it0 + 1) / kTrSlots) & 1, p.err_flag);
-      tc_fence_after();
-      {
-        const uint64_t whd = make_desc(smem_u32(smem + TrSmem::wring(s0))), wld = make_desc(smem_u32(smem + TrSmem::wring(s1)));
-        if (mma_on) {
-          if constexpr (TS) {
-            const uint32_t ta = tmem_base + (uint32_t)(kb * 32);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {  // a k-step = 32 bytes of the 128-byte swizzle row = +2 in the descriptor's address field
-              umma_f16_ts(d_tmem, ta + 128u + 8u * k, whd + 2u * k, idesc128, (kb | k) ? 1u : 0u);
-              umma_f16_ts(d_tmem, ta + 8u * k, whd + 2u * k, idesc128, 1u);
-              umma_f16_ts(d_tmem, ta + 8u * k, wld + 2u * k, idesc128, 1u);
-            }
-          } else {
-            const uint64_t ahd = make_desc(smem_u32(smem + TrSmem::abuf(kb, 0))), ald = make_desc(smem_u32(smem + TrSmem::abuf(kb, 1)));
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              umma_f16(d_tmem, ald + 2u * k, whd + 2u * k, idesc128, (kb | k) ? 1u : 0u);
-              umma_f16(d_tmem, ahd + 2u * k, whd + 2u * k, idesc128, 1u);
-              umma_f16(d_tmem, ahd + 2u * k, wld + 2u * k, idesc128, 1u);
-            }
-          }
-        }
-        umma_commit(&wempty[s0]);  // s0 is even: the barrier of the slot pair (s0, s0 + 1)
-        if (kb == 3) umma_commit(accbar);
-      }
+  const Frag f;
+  uint32_t nslot = 0;
+  float acc[128];
+  // attention task of this thread: tile row ar, head columns 32 ah .. +31
+  const int ar = tid >> 1, ah = tid & 1;
+  const int a_slot = ar >> lnp;
+  for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
+    // global row of tile row r (-1: padding row or walker past the end)
+    auto grow_of = [&](int r) -> long long {
+      const int walker = tile * G + (r >> lnp), el = r & (NP - 1);
+      return (el < N && walker < p.walkers) ? (long long)walker * N + el : -1;
     };
-    uint32_t it = 0, n_af = 0, n_of = 0, n_free0 = 0, n_free1 = 0, n_qk = 0, n_v = 0, n_p = 0, n_ofr0 = 0, n_ofr1 = 0;
-    for (int tile = blockIdx.x; tile < MT; tile += gridDim.x)
-      for (int l = 0; l < L; ++l) {
-        // ---- QKV: sub-chunk j -> accumulator half j & 1
-        for (int j = 0; j < 6; ++j) {
-          const int b = j & 1;
-          if (j == 0) {  // the operand comes from an epilogue that also read accumulator half 0 (its k-blocks 0, 1)
-            mbar_wait(&afull[0], n_af & 1, p.err_flag);
-            mbar_wait(&afull[1], n_af & 1, p.err_flag);
+    // ---- tile load: embedding rows -> residual stream and the operand buffer (loads in batches of 8 ahead of the stores)
+    for (int i0 = 0; i0 < 128 * 64 / kTrThreads; i0 += 8) {
+      float4 x[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int idx = tid + kTrThreads * (i0 + i), r = idx >> 6, c = 4 * (idx & 63);
+        const long long row = grow_of(r);
+        x[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (row >= 0) {
+          const float* xrow = p.X0 + (size_t)row * p.ldx;
+          if (p.vper > 0) {
+            const int walker = (int)(row / N), el = (int)(row % N);
+            const long long v = p.v0 + walker;
+            xrow = el == (int)((v / 12) % N) ? p.X0 + (size_t)walker * p.ldx : p.Xbase + ((size_t)(v / p.vper) * N + el) * p.ldx;
           }
-          if (j >= 2) {
-            if (b == 0) { mbar_wait(&accfree[0], n_free0 & 1, p.err_flag); ++n_free0; }
-            else { mbar_wait(&accfree[1], n_free1 & 1, p.err_flag); ++n_free1; }
+          x[i] = __ldg((const float4*)(xrow + c));
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int idx = tid + kTrThreads * (i0 + i), r = idx >> 6, c = 4 * (idx & 63);
+        *(float4*)(resid + r * 256 + c) = x[i];
+        const float sc = p.a_scale;
+        store_operand_quad(smem, r, c, make_float4(x[i].x * sc, x[i].y * sc, x[i].z * sc, x[i].w * sc));
+      }
+    }
+    fence_proxy_async();
+    __syncthreads();
+    for (int l = 0; l < L; ++l) {
+      const bool last = l == L - 1;
+      const CUtensorMap* lm = p.maps + 8 * l;
+      // ---- Q | K | V = X Wqkv, 256 columns at a time -> scratch (true values)
+      for (int j = 0; j < 3; ++j) {
+        gemm_abuf<256>(acc, smem, full, nslot, lm, lm + 1, 256 * j, p.err_flag);
+        const float us = p.us[l][0];
+#pragma unroll
+        for (int jj = 0; jj < 32; ++jj)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            *(float2*)(qkv + (f.fr + 8 * h) * 768 + 256 * j + 8 * jj + f.fc) =
+                make_float2(acc[4 * jj + 2 * h] * us, acc[4 * jj + 2 * h + 1] * us);
+      }
+      sb1[tid] = __ldg(p.b1[l] + tid);
+      sb2[tid] = __ldg(p.b2[l] + tid);
+      __syncthreads();  // Q / K / V rows of the whole tile are in the scratch buffer
+      // ---- attention, head by head
+      for (int h = 0; h < 4; ++h) {
+        {
+          float4 kv[2 * 128 * 16 / kTrThreads];  // all loads of this thread first, then the stores
+#pragma unroll
+          for (int i = 0; i < 128 * 16 / kTrThreads; ++i) {
+            const int idx = tid + kTrThreads * i, r = idx >> 4, c = 4 * (idx & 15);
+            kv[2 * i] = *(const float4*)(qkv + r * 768 + 256 + 64 * h + c);
+            kv[2 * i + 1] = *(const float4*)(qkv + r * 768 + 512 + 64 * h + c);
           }
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + 256u + 128u * (uint32_t)b;
-          for (int kb = 0; kb < 4; ++kb) {
-            if (j == 0 && kb >= 2) {  // k-blocks 2, 3 of the operand (written by the other column half of the workers)
-              mbar_wait(&afull[kb], n_af & 1, p.err_flag);
-              if (kb == 3) ++n_af;
-              tc_fence_after();
-            }
-            dense_kblock(kb, d_tmem, it, &accfull[b]);
-            it += 2;
+#pragma unroll
+          for (int i = 0; i < 128 * 16 / kTrThreads; ++i) {
+            const int idx = tid + kTrThreads * i, r = idx >> 4, c = 4 * (idx & 15);
+            *(float4*)(kst + r * 64 + c) = kv[2 * i];
+            *(float4*)(vst + r * 64 + c) = kv[2 * i + 1];
           }
         }
-        // the last two drains (sub-chunks 4, 5) free both halves of the accumulator: it now hosts S / P / O
-        mbar_wait(&accfree[0], n_free0 & 1, p.err_flag); ++n_free0;
-        mbar_wait(&accfree[1], n_free1 & 1, p.err_flag); ++n_free1;
-        // ---- attention, head by head
-        for (int h = 0; h < 4; ++h) {
-          const int ob = h & 1;
-          mbar_wait(qk_full, n_qk & 1, p.err_flag); ++n_qk;
-          tc_fence_after();
-          {  // S = Q K^T -> TMEM [256, 384)
-            const uint32_t qh = smem_u32(smem + TrSmem::wring(0)), ql = smem_u32(smem + TrSmem::wring(1));
-            const uint32_t kh = smem_u32(smem + TrSmem::wring(2)), kl = smem_u32(smem + TrSmem::wring(3));
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint32_t ko = k * 256;  // unswizzled images: a k-step of 16 halves = 2 chunks of 128 bytes
-              if (!mma_on) continue;
-              umma_f16(tmem_base + 256u, make_desc_ns(ql + ko), make_desc_ns(kh + ko), idesc128, k ? 1u : 0u);
-              umma_f16(tmem_base + 256u, make_desc_ns(qh + ko), make_desc_ns(kh + ko), idesc128, 1u);
-              umma_f16(tmem_base + 256u, make_desc_ns(qh + ko), make_desc_ns(kl + ko), idesc128, 1u);
-            }
-            umma_commit(s_full);
-            umma_commit(qk_free);
-          }
-          mbar_wait(p_full, n_p & 1, p.err_flag); ++n_p;
-          mbar_wait(v_full, n_v & 1, p.err_flag); ++n_v;
-          if (h >= 2) {  // the O buffer of head h - 2 has been read
-            if (ob == 0) { mbar_wait(&o_free[0], n_ofr0 & 1, p.err_flag); ++n_ofr0; }
-            else { mbar_wait(&o_free[1], n_ofr1 & 1, p.err_flag); ++n_ofr1; }
-          }
-          tc_fence_after();
-          {  // O_h = P V_h: A = P from TMEM (hi columns [256, 320), lo [320, 384)), B = V_h^T image
-            const uint32_t d_o = tmem_base + 384u + 64u * (uint32_t)ob;
-            const uint32_t vh = smem_u32(smem + TrSmem::wring(4)), vl = smem_u32(smem + TrSmem::wring(5));
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {  // 16 keys per step; k-block of 64 keys = 8 KB of the image plane
-              const uint32_t bo = (uint32_t)(k >> 2) * 8192u + (uint32_t)(k & 3) * 32u;
-              const uint32_t a_hi = tmem_base + 256u + 8u * (uint32_t)k, a_lo = a_hi + 64u;
-              if (!mma_on) continue;
-              umma_f16_ts(d_o, a_lo, make_desc(vh + bo), idesc64, k ? 1u : 0u);
-              umma_f16_ts(d_o, a_hi, make_desc(vh + bo), idesc64, 1u);
-              umma_f16_ts(d_o, a_hi, make_desc(vl + bo), idesc64, 1u);
-            }
-            umma_commit(&o_full[ob]);
-            umma_commit(v_free);
-          }
-        }
-        // ---- Wo (operand = attention output), W1, W2: two N = 128 halves each -> accumulator halves 0, 1.  The workers of a
-        // column half run its epilogue as soon as that half is complete, i.e. under the MMAs of the other half / next GEMM.
-        mbar_wait(&o_free[0], n_ofr0 & 1, p.err_flag); ++n_ofr0;  // heads 2, 3: buffers read (every completion is consumed)
-        mbar_wait(&o_free[1], n_ofr1 & 1, p.err_flag); ++n_ofr1;
-        for (int g = 0; g < 3; ++g)
-          for (int hb = 0; hb < 2; ++hb) {
-            const uint32_t d_tmem = tmem_base + 256u + 128u * (uint32_t)hb;
-            if (hb == 0 && g > 0) {  // accumulator half 0 has been read once operand k-blocks 0 AND 1 are written
-              mbar_wait(&afull[0], n_af & 1, p.err_flag);
-              mbar_wait(&afull[1], n_af & 1, p.err_flag);
-            }
-            tc_fence_after();
-            for (int kb = 0; kb < 4; ++kb) {
-              if (hb == 0) {
-                if (g == 0) {
-                  mbar_wait(&ofull[kb], n_of & 1, p.err_flag);
-                  if (kb == 3) ++n_of;
-                } else if (kb >= 2) {
-                  mbar_wait(&afull[kb], n_af & 1, p.err_flag);
-                  if (kb == 3) ++n_af;
-                }
-                tc_fence_after();
-              }
-              dense_kblock(kb, d_tmem, it, &accfull[hb]);
-              it += 2;
-            }
-          }
-      }
-    }  // elected thread
-  } else {
-    // ===================== workers: warps 0-7 ======================================================================
-    const int q4 = warp & 3, half = warp >> 2;
-    const int trow = 32 * q4 + lane;
-    const uint32_t tlane = (uint32_t)(32 * q4) << 16;
-    const int c_lo = 4 * half, c_hi = 4 * half + 4;  // this thread's 32-column chunks
-    const int lnp = 31 - __clz(NP);                      // NP is a power of two
-    const int slot = trow >> lnp, el = trow & (NP - 1);  // walker slot of the tile, electron
-    uint32_t n_acc0 = 0, n_acc1 = 0, n_s = 0, n_o0 = 0, n_o1 = 0;
-    for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
-      const bool tr_on = p.trace && blockIdx.x == 0 && tile == (int)(2 * gridDim.x) && threadIdx.x == 0;
-#define TR_STAMP(i) do { if (tr_on && l == 1) p.trace[i] = clock64(); } while (0)
-      const int walker = tile * G + slot;
-      const bool valid = el < N && walker < p.walkers;
-      const size_t row = (size_t)walker * N + el;  // global row (valid rows only)
-      const float* xrow = p.X0 + row * p.ldx;
-      if (p.vper > 0 && valid) {
-        const long long v = p.v0 + walker;
-        xrow = el == (int)((v / 12) % N) ? p.X0 + (size_t)walker * p.ldx : p.Xbase + ((size_t)(v / p.vper) * N + el) * p.ldx;
-      }
-      // ---- tile load: embedding rows -> residual stream in TMEM [0, 256) and the operand buffer
-      for (int c = c_lo; c < c_hi; ++c) {
-        float a[32];
+        __syncthreads();
+        float q[32], o[32];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const float4 x = valid ? __ldg((const float4*)(xrow + c * 32 + 4 * i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          a[4 * i] = x.x; a[4 * i + 1] = x.y; a[4 * i + 2] = x.z; a[4 * i + 3] = x.w;
+          const float4 v = *(const float4*)(qkv + ar * 768 + 64 * h + 32 * ah + 4 * i);
+          q[4 * i] = v.x; q[4 * i + 1] = v.y; q[4 * i + 2] = v.z; q[4 * i + 3] = v.w;
         }
-        uint32_t v[32];
-        if constexpr (TS) {
-          resid_store32(smem, trow, c * 32, a);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) a[i] *= p.a_scale;
-          pack_operand32(a, v);
-          store_operand_tmem(tmem_base + tlane, c * 32, v);
-          if (c & 1) {
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&afull[c >> 1]);
+        for (int i = 0; i < 32; ++i) o[i] = 0.f;
+        float mx = -3.0e38f, sum = 0.f;
+        for (int e = 0; e < N; ++e) {  // keys of this row's walker
+          const int kr = (a_slot << lnp) + e;
+          const float* kp = kst + kr * 64 + 32 * ah;
+          float sp[4] = {0.f, 0.f, 0.f, 0.f};  // four independent partial sums: the dot product is not one dependent chain
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float4 k4 = *(const float4*)(kp + 4 * i);
+            sp[i & 3] += q[4 * i] * k4.x + q[4 * i + 1] * k4.y + q[4 * i + 2] * k4.z + q[4 * i + 3] * k4.w;
           }
-        } else {
+          float s = (sp[0] + sp[1]) + (sp[2] + sp[3]);
+          s = (s + __shfl_xor_sync(0xffffffffu, s, 1)) * p.attn_scale;
+          const float mnew = fmaxf(mx, s);
+          const float corr = __expf(mx - mnew), pe = __expf(s - mnew);
+          sum = sum * corr + pe;
+          mx = mnew;
+          const float* vp = vst + kr * 64 + 32 * ah;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(a[i]);
-          tmem_st32(tmem_base + tlane + (uint32_t)(c * 32), v);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) a[i] *= p.a_scale;
-          store_operand_chunk(smem, trow, c * 32, a);
-          if (c & 1) {
-            tmem_st_wait();
-            fence_proxy_async();
-            mbar_arrive(&afull[c >> 1]);
+          for (int i = 0; i < 8; ++i) {
+            const float4 v4 = *(const float4*)(vp + 4 * i);
+            o[4 * i] = o[4 * i] * corr + pe * v4.x;
+            o[4 * i + 1] = o[4 * i + 1] * corr + pe * v4.y;
+            o[4 * i + 2] = o[4 * i + 2] * corr + pe * v4.z;
+            o[4 * i + 3] = o[4 * i + 3] * corr + pe * v4.w;
           }
         }
+        const float un = p.a_scale / sum;
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          store_operand_quad(smem, ar, 64 * h + 32 * ah + 4 * i,
+                             make_float4(o[4 * i] * un, o[4 * i + 1] * un, o[4 * i + 2] * un, o[4 * i + 3] * un));
+        __syncthreads();  // K_h / V_h staging is re-used by the next head (and the ring by the next GEMM)
       }
-      for (int l = 0; l < L; ++l) {
-        const bool last = l == L - 1;
-        // ---- QKV drain: sub-chunk j (W^T rows 128 j ..) -> matrix j / 2, heads 2 (j % 2) + {0, 1}; this thread: head .. + half
-        TR_STAMP(0);
-        for (int j = 0; j < 6; ++j) {
-          const int b = j & 1;
-          if (b == 0) { mbar_wait(&accfull[0], n_acc0 & 1, p.err_flag); ++n_acc0; }
-          else { mbar_wait(&accfull[1], n_acc1 & 1, p.err_flag); ++n_acc1; }
-          tc_fence_after();
-          TR_STAMP(1 + 2 * j);
-          uint32_t v0[32], v1[32];
-          tmem_ld32(tmem_base + tlane + (uint32_t)(256 + 128 * b + 64 * half), v0);
-          tmem_ld32(tmem_base + tlane + (uint32_t)(256 + 128 * b + 64 * half + 32), v1);
-          tmem_ld_wait();
-          tc_fence_before();
-          mbar_arrive(&accfree[b]);
-          const float sc = p.us[l][0] * 16.f;  // true value x 2^4 (operand scale of the attention products)
-          unsigned char* img = scratch + (size_t)(2 * b + half) * kTrHeadImage + (j >> 1) * 32768;  // Q | K | V^T of the head
-          float x[32];
+      fence_proxy_async();
+      __syncthreads();
+      // ---- A = X + O Wo, M1 = tanh(A W1 + b1), X = A + tanh(M1 W2 + b2)
+      const float* xin[2];
+      float* aout[2];
+      float* xout[2];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v0[i]) * sc;
-          const bool img_on = !(p.ablate & 4);
-          if (!img_on) {} else
-          if (j < 4) image_store32(img, trow, 0, x); else image_store_vt32(img, trow, 0, x);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v1[i]) * sc;
-          if (!img_on) {} else
-          if (j < 4) image_store32(img, trow, 32, x); else image_store_vt32(img, trow, 32, x);
-          TR_STAMP(2 + 2 * j);
-          if (j == 3) {  // Q and K images complete
-            fence_proxy_async_all();
-            __threadfence_block();
-            named_bar_sync(1, 256);
-            if (threadIdx.x == 0) mbar_arrive(scr_qk);
-          }
-        }
-        fence_proxy_async_all();  // the images are read back through the async proxy (bulk copies)
-        __threadfence_block();
-        named_bar_sync(1, 256);   // images complete; everybody is past the previous layer's last epilogue
-        if (threadIdx.x == 0) mbar_arrive(scr_full);
-        TR_STAMP(13);
-        if (threadIdx.x < 256) {
-          sb1[threadIdx.x] = __ldg(p.b1[l] + threadIdx.x);
-          sb2[threadIdx.x] = __ldg(p.b2[l] + threadIdx.x);
-        }
-        // ---- attention: softmax of head h, then the output rows of head h - 1 (overlaps P V of head h)
-        float inv_prev = 0.f, inv_cur = 0.f;  // 1 / row sum of head h - 1, h
-        for (int h = 0; h <= 4; ++h) {
-          inv_prev = inv_cur;
-          if (h < 4) {
-            mbar_wait(s_full, n_s & 1, p.err_flag); ++n_s;
-            tc_fence_after();
-            TR_STAMP(14 + 4 * h);
-            uint32_t sv[32];
-            tmem_ld32(tmem_base + tlane + (uint32_t)(256 + 32 * q4), sv);  // keys = tile rows 32 q4 .. +31
-            tmem_ld_wait();
-            named_bar_sync(2 + q4, 64);  // P overwrites S in place: the other warp of these rows has read its copy as well
-            const float cs = p.attn_scale * (1.f / 256.f) * 1.4426950408889634f;  // scores in units of log2 e
-            float mx = -3.0e38f;
-            float e[32];
-#pragma unroll
-            for (int c = 0; c < 32; ++c) {
-              const int key = 32 * q4 + c;
-              const bool on = (key >> lnp) == slot && (key & (NP - 1)) < N;  // keys of this row's walker
-              e[c] = on ? __uint_as_float(sv[c]) * cs : -3.0e38f;
-              mx = fmaxf(mx, e[c]);
-            }
-            float sum = 0.f;
-#pragma unroll
-            for (int c = 0; c < 32; ++c) {
-              e[c] = e[c] > -1.0e38f ? ex2_approx(e[c] - mx) : 0.f;
-              sum += e[c];
-            }
-            inv_cur = 1.f / sum;  // padding rows (el >= N) still see the walker's keys: finite, never written out
-            // P x 2^10 as packed halves: this warp writes the hi plane (half 0) or the lo plane (half 1) of its rows:
-            // 16 columns of the window, explicit zeros in the other 48 (S covered all 128 keys)
-            uint32_t pw[16], zero[16];
-#pragma unroll
-            for (int c = 0; c < 16; ++c) {
-              uint32_t hi, lo;
-              tr_split2(e[2 * c] * 1024.f, e[2 * c + 1] * 1024.f, hi, lo);
-              pw[c] = half ? lo : hi;
-              zero[c] = 0u;
-            }
-            const uint32_t pbase = tmem_base + tlane + 256u + 64u * (uint32_t)half;
-#pragma unroll
-            for (int gq = 0; gq < 4; ++gq) {
-              if (gq == q4) tmem_st16(pbase + 16u * (uint32_t)gq, pw);
-              else tmem_st16(pbase + 16u * (uint32_t)gq, zero);
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(p_full);
-            TR_STAMP(15 + 4 * h);
-          }
-          if (h > 0) {
-            const int ho = h - 1, ob = ho & 1;
-            if (ob == 0) { mbar_wait(&o_full[0], n_o0 & 1, p.err_flag); ++n_o0; }
-            else { mbar_wait(&o_full[1], n_o1 & 1, p.err_flag); ++n_o1; }
-            tc_fence_after();
-            TR_STAMP(16 + 4 * ho);
-            uint32_t ov[32];
-            tmem_ld32(tmem_base + tlane + (uint32_t)(384 + 64 * ob + 32 * half), ov);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(&o_free[ob]);
-            const float uo = p.a_scale * inv_prev * (1.f / (1024.f * 16.f));
-            float a[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) a[i] = __uint_as_float(ov[i]) * uo;
-            if constexpr (TS) {
-              uint32_t pv[32];
-              pack_operand32(a, pv);
-              store_operand_tmem(tmem_base + tlane, 64 * ho + 32 * half, pv);
-              tmem_st_wait();
-              tc_fence_before();
-            } else {
-              store_operand_chunk(smem, trow, 64 * ho + 32 * half, a);
-              fence_proxy_async();
-            }
-            mbar_arrive(&ofull[ho]);
-            TR_STAMP(17 + 4 * ho);
-          }
-        }
-        named_bar_sync(1, 256);  // biases of this layer are in shared memory
-#ifdef DQMC_EMU_DEBUG_TRUNK
-        if (!TS && threadIdx.x == 0 && tile == 0 && l == 0) {  // development aid: attention output operand of the first tile / layer
-          FILE* f = std::fopen("/tmp/trunk_dbg_O.bin", "wb");
-          for (int r = 0; r < 128; ++r)
-            for (int c = 0; c < 256; ++c) {
-              const int kb = c >> 6, cc = c & 63;
-              const int off = (r >> 3) * 1024 + (r & 7) * 128 + (((cc >> 3) ^ (r & 7)) << 4) + (cc & 7) * 2;
-              uint16_t hh, ll;
-              std::memcpy(&hh, smem + TrSmem::abuf(kb, 0) + off, 2);
-              std::memcpy(&ll, smem + TrSmem::abuf(kb, 1) + off, 2);
-              const float v = (half_bits_to_float(hh) + half_bits_to_float(ll)) / p.a_scale;
-              std::fwrite(&v, 4, 1, f);
-            }
-          std::fclose(f);
-        }
-#endif
-        // The three GEMMs run as two output halves each.  Column half 0 finishes first and its workers start at once, but the
-        // operand buffer still feeds the MMAs of half 1: they PARK their result (already scaled / split / packed) in place of
-        // the accumulator columns they have just read and move it to shared memory when half 1 is complete.  Half 1 writes
-        // directly.  Either way the epilogue of one half runs under the MMAs of the other.
-        auto emit = [&](int c, const float* a) {  // a: 32 scaled operand values of chunk c
-          uint32_t v[32];
-          pack_operand32(a, v);
-          if (half == 0) {
-            tmem_st32(tmem_base + tlane + (uint32_t)(256 + c * 32), v);
-          } else {
-            if constexpr (TS) store_operand_tmem(tmem_base + tlane, c * 32, v);
-            else store_operand_packed(smem, trow, c * 32, v);
-            if (c & 1) {
-              tmem_st_wait();
-              if constexpr (!TS) fence_proxy_async();
-              tc_fence_before();
-              mbar_arrive(&afull[c >> 1]);
-            }
-          }
-        };
-        auto unpark = [&]() {  // half 0: the whole GEMM has read the operand buffer -> move the parked chunks over
-          tmem_st_wait();
-          mbar_wait(&accfull[1], n_acc1 & 1, p.err_flag); ++n_acc1;
-          tc_fence_after();
-          for (int c = c_lo; c < c_hi; ++c) {
-            uint32_t v[32];
-            tmem_ld32(tmem_base + tlane + (uint32_t)(256 + c * 32), v);
-            tmem_ld_wait();
-            if constexpr (TS) store_operand_tmem(tmem_base + tlane, c * 32, v);
-            else store_operand_packed(smem, trow, c * 32, v);
-            if (c & 1) {
-              if constexpr (TS) tmem_st_wait();
-              else fence_proxy_async();
-              tc_fence_before();
-              mbar_arrive(&afull[c >> 1]);
-            }
-          }
-        };
-        // ---- epilogue 1: A = X + O Wo -> TMEM [0, 256) and the operand buffer
-        TR_STAMP(30);
-        if (half == 0) { mbar_wait(&accfull[0], n_acc0 & 1, p.err_flag); ++n_acc0; }
-        else { mbar_wait(&accfull[1], n_acc1 & 1, p.err_flag); ++n_acc1; ++n_acc0; }
-        tc_fence_after();
-        TR_STAMP(31);
-        for (int c = c_lo; c < c_hi; ++c) {
-          uint32_t v[32];
-          float a[32];
-          tmem_ld32(tmem_base + tlane + (uint32_t)(256 + c * 32), v);
-          if constexpr (TS) {
-            resid_load32(smem, trow, c * 32, a);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) a[i] += __uint_as_float(v[i]) * p.us[l][1];
-            resid_store32(smem, trow, c * 32, a);
-          } else {
-            uint32_t r[32];
-            tmem_ld32(tmem_base + tlane + (uint32_t)(c * 32), r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) a[i] = __uint_as_float(r[i]) + __uint_as_float(v[i]) * p.us[l][1];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(a[i]);
-            tmem_st32(tmem_base + tlane + (uint32_t)(c * 32), v);
-          }
-#pragma unroll
-          for (int i = 0; i < 32; ++i) a[i] *= p.a_scale;
-          emit(c, a);
-        }
-        if (half == 0) unpark();
-        // ---- epilogue 2: M1 = tanh(A W1 + b1) -> operand buffer
-        TR_STAMP(32);
-        if (half == 0) { mbar_wait(&accfull[0], n_acc0 & 1, p.err_flag); ++n_acc0; }
-        else { mbar_wait(&accfull[1], n_acc1 & 1, p.err_flag); ++n_acc1; ++n_acc0; }
-        tc_fence_after();
-        TR_STAMP(33);
-        for (int c = c_lo; c < c_hi; ++c) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + tlane + (uint32_t)(256 + c * 32), v);
-          tmem_ld_wait();
-          float a[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) a[i] = mlp_tanh(__uint_as_float(v[i]) * p.us[l][2] + sb1[c * 32 + i]) * p.a_scale;
-          emit(c, a);
-        }
-        if (half == 0) unpark();
-        // ---- epilogue 3: X' = A + tanh(M1 W2 + b2) -> next layer's residual stream + operand, or the output rows
-        TR_STAMP(34);
-        if (half == 0) { mbar_wait(&accfull[0], n_acc0 & 1, p.err_flag); ++n_acc0; }
-        else { mbar_wait(&accfull[1], n_acc1 & 1, p.err_flag); ++n_acc1; ++n_acc0; }
-        tc_fence_after();
-        TR_STAMP(35);
-        for (int c = c_lo; c < c_hi; ++c) {
-          uint32_t v[32];
-          float a[32];
-          tmem_ld32(tmem_base + tlane + (uint32_t)(256 + c * 32), v);
-          if constexpr (TS) {
-            resid_load32(smem, trow, c * 32, a);
-            tmem_ld_wait();
-          } else {
-            uint32_t r[32];
-            tmem_ld32(tmem_base + tlane + (uint32_t)(c * 32), r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) a[i] = __uint_as_float(r[i]);
-          }
-#pragma unroll
-          for (int i = 0; i < 32; ++i) a[i] += mlp_tanh(__uint_as_float(v[i]) * p.us[l][3] + sb2[c * 32 + i]);
-          if (last) {
-            if (valid) {
-              float* op = p.Out + row * p.ldout + c * 32;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) *(float4*)(op + 4 * i) = make_float4(a[4 * i], a[4 * i + 1], a[4 * i + 2], a[4 * i + 3]);
-            }
-          } else {
-            if constexpr (TS) {
-              resid_store32(smem, trow, c * 32, a);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(a[i]);
-              tmem_st32(tmem_base + tlane + (uint32_t)(c * 32), v);
-            }
-#pragma unroll
-            for (int i = 0; i < 32; ++i) a[i] *= p.a_scale;
-            emit(c, a);
-          }
-        }
-        if (half == 0) {
-          if (last) {  // nothing parked, but the next tile's load must not touch the operand buffer before W2 has read all of it
-            mbar_wait(&accfull[1], n_acc1 & 1, p.err_flag); ++n_acc1;
-          } else {
-            unpark();
-          }
-        }
-        TR_STAMP(36);
-        if (last) tc_fence_before();  // the next tile's load overwrites TMEM [0, 256) / the operand buffer from the same threads
+      for (int h = 0; h < 2; ++h) {
+        const int r = f.fr + 8 * h;
+        xin[h] = resid + r * 256;
+        aout[h] = resid + r * 256;
+        const long long row = grow_of(r);
+        xout[h] = !last ? resid + r * 256 : (row >= 0 ? p.Out + (size_t)row * p.ldout : nullptr);
       }
-#undef TR_STAMP
+      mlp3<256>(acc, smem, full, nslot, lm + 2, lm + 3, lm + 4, lm + 5, lm + 6, lm + 7, p.us[l][1], p.us[l][2], p.us[l][3],
+                p.a_scale, sb1, sb2, xin, aout, xout, !last, p.err_flag);
+      fence_proxy_async();
+      __syncthreads();  // next layer's operand complete / next tile's load may overwrite the residual rows
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -311,7 +311,7 @@ class Engine:
         self.lib = _lib.load(_lib_path)
         self.plan_only = plan_only
         if not self._host and not plan_only and not torch.cuda.is_available():
-            raise RuntimeError('deepqmc_b200 needs a CUDA device (B200, sm_100a); there is no CPU path')
+            raise RuntimeError('deepqmc_b200 needs a CUDA device (H100, sm_90a); there is no CPU path')
         self.spec, self.hamil = spec, hamil
         self.dtype_code = {'float64': 0, 'float32': 1}[dtype]
         self.dtype = _TORCH_DTYPE[self.dtype_code]

@@ -1,4 +1,4 @@
-/* dqmc_b200.h -- C ABI of the B200-native local-energy engine (libdqmc_b200.so).
+/* dqmc_b200.h -- C ABI of the H100-native local-energy engine (libdqmc_b200.so).
  *
  * Drop-in boundary for the per-walker local-energy hot path of deepqmc/deepqmc.  The
  * reference has no FFI of its own (pure JAX); each entry point below names the reference
@@ -222,7 +222,7 @@ int64_t dqmc_launch_count(dqmc_handle h);
  * with the named weight of the handle's parameter table, on the requested backend
  * (DQMC_GEMM_SIMT | DQMC_GEMM_TCGEN05).  A[rows][K], Res/C[rows][N] device arrays in the compute
  * dtype; sliced = 1 exercises the per-spin backflow mapping (weight "bf.up"/"bf.dn", rows = B*S).
- * Used by tests to validate the tcgen05 3xTF32 kernel against the CUDA-core kernel and fp64.
+ * Used by tests to validate the wgmma 3xTF32 kernel against the CUDA-core kernel and fp64.
  * No reference analogue (the reference's dense layers are hk.Linear -> XLA dot). */
 int dqmc_debug_gemm(dqmc_handle h, const char* weight, const char* bias, const void* A, const void* Res, void* C,
                     int32_t rows, int32_t S, int32_t sliced, int32_t backend, void* stream);
@@ -234,7 +234,7 @@ int dqmc_debug_gemm(dqmc_handle h, const char* weight, const char* bias, const v
 int dqmc_debug_mlp_block(dqmc_handle h, int32_t layer, const void* O, const void* X, void* Out, int32_t rows, void* stream);
 
 /* Self-test hook: ONE launch of the whole-trunk kernel of a plain forward (deepqmc_b200/csrc/trunk_tc.cuh; fp32 engines with the
- * tcgen05 backend and the shipped Psiformer shape: embedding_dim 256, 4 heads of 64, N <= 32 electrons): every attention layer
+ * tensor-core backend and the shipped Psiformer shape: embedding_dim 256, 4 heads of 64, N <= 32 electrons): every attention layer
  * (QKV projection, softmax attention, output projection + residual, tanh-MLP + residual) applied to the embedding rows
  * X0 [rows][256] (rows = walkers x electrons, walker-major), result Out [rows][256].  Status 2 if the configuration has none.
  * reference: gnn/electron_gnn.py:403-432 (layer loop), gnn/update_features.py:241-286, hkext.py:22-137, :215-253. */

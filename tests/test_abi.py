@@ -22,16 +22,16 @@ def test_header_symbols_exported(built_lib):
     from deepqmc_b200 import _lib
 
     assert sorted(_lib.SYMBOLS) == syms
-    assert b'sm_100a' in built_lib.dqmc_version()
+    assert b'sm_90a' in built_lib.dqmc_version()
 
 
-def test_sass_is_sm100a(built_lib):
+def test_sass_is_sm90a(built_lib):
     import subprocess
 
     from deepqmc_b200 import _lib
 
     out = subprocess.run(['cuobjdump', '-lelf', _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert 'sm_100a' in out
+    assert 'sm_90a' in out
 
 
 def test_no_cpu_fallback(monkeypatch, tmp_path):

@@ -270,7 +270,7 @@ def test_benzene_full_size_one_walker_vs_oracle():
     """BASELINE configs[3] at FULL size (benzene, ccECP, Psiformer d = 256, L = 4, H = 4, K = 16): ONE walker against the
     ORACLE (autograd Hessian over the 90 coordinates, all 2160 quadrature forwards; about a minute of host time):
       * fp64 engine: log|psi| to 1e-10, E_loc and all six statistics to 1e-8 (relative to max(1, |value|));
-      * fp32 production engine (tcgen05 backend: whole-trunk kernel for the quadrature forwards, 3xTF32 forward-Laplacian
+      * fp32 production engine (tensor-core backend: whole-trunk kernel for the quadrature forwards, 3xTF32 forward-Laplacian
         rows): E_loc to 2e-4 of its natural scale max(1, |E|, |lap| / 2, |grad|^2 / 2) -- E_kin = -(lap + |grad|^2) / 2 is a
         difference of those two terms, fp32 round-off is relative to them, not to their difference -- and V_nl to 2e-4 of
         max(1, |V_nl|)."""
@@ -558,7 +558,7 @@ def test_parameter_vjp_matches_autograd_fp64():
 
 def test_energy_gradient_fp32_close_to_fp64():
     """Energy gradient = one local-energy pass + one reverse pass with cotangent (E_loc - <E>) / B
-    (reference loss/energy.py:77-102): the fp32 engine (tcgen05 forward GEMMs) agrees with the fp64 engine."""
+    (reference loss/energy.py:77-102): the fp32 engine (tensor-core forward GEMMs) agrees with the fp64 engine."""
     from deepqmc_b200.energy import compute_mean_energy_tangent, median_clip_and_mask
 
     mol = Molecule.from_name('LiH')

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 3xTF32 dense-layer GEMM (gemm_tcgen05.cuh) against fp64 matmul and the
+"""GPU: the wgmma 3xTF32 dense-layer GEMM (gemm_wgmma.cuh) against fp64 matmul and the
 CUDA-core kernel, then the whole fp32 engine with the tensor-core backend against the oracle."""
 import numpy as np
 import pytest
@@ -103,39 +103,10 @@ def test_engine_tcgen05_backend_parity():
         assert abs(E1[b].item() - eo.item()) <= 2e-4 * scale_b
 
 
-def test_cta_pair_variant_matches_single_cta(monkeypatch):
-    """The cta_group::2 variant of the kernel (clusters of 2 CTAs, 256-row pair tiles, half weight tile per CTA,
-    multicast commits; engine switch DQMC_GEMM_2CTA read at handle creation) gives the same result as the
-    single-CTA kernel: dense GEMM incl. ragged row count and residual, sliced backflow heads, and one fp32
-    local-energy evaluation."""
-    hamil, a1, params, eng1 = _engine(1)
-    monkeypatch.setenv('DQMC_GEMM_2CTA', '1')
-    hamil2, a2, _, eng2 = _engine(1)
-    g = torch.Generator(device='cpu').manual_seed(5)
-    for rows, S, weight, bias in [(56 * 300 + 5, 14, 'L0.wqkv', None), (1000, 14, 'L1.w1', 'L1.b1'), (77, 1, 'L2.wo', None)]:
-        A = torch.randn(rows, 256, generator=g).to(DEV)
-        Res = torch.randn(rows, 256, generator=g).to(DEV) if weight.endswith('wo') else None
-        C1 = eng1.debug_gemm(weight, A, bias=bias, Res=Res, S=S, backend=1)
-        C2 = eng2.debug_gemm(weight, A, bias=bias, Res=Res, S=S, backend=1)
-        torch.cuda.synchronize()
-        assert torch.allclose(C1, C2, rtol=1e-6, atol=1e-5), (weight, (C1 - C2).abs().max().item())
-    A = torch.randn(37 * 4 * 14, 256, device=DEV)
-    assert torch.allclose(eng1.debug_gemm('bf.up', A, S=14, sliced=True, backend=1),
-                          eng2.debug_gemm('bf.up', A, S=14, sliced=True, backend=1), rtol=1e-6, atol=1e-5)
-    rng = np.random.default_rng(0)
-    mol = hamil.mol
-    r = torch.as_tensor(mol.coords[rng.integers(0, 2, size=(64, 4))] + rng.normal(size=(64, 4, 3)), device=DEV, dtype=torch.float32)
-    R = torch.as_tensor(mol.coords, device=DEV, dtype=torch.float32)
-    pc = PhysicalConfiguration(R, r, torch.zeros(64, device=DEV))
-    E1, _ = hamil.local_energy(a1.apply)(None, params, pc)
-    E2, _ = hamil2.local_energy(a2.apply)(None, params, pc)
-    assert torch.allclose(E1, E2, rtol=1e-5, atol=1e-4)
-
-
 @pytest.mark.parametrize('rows', [5, 128, 1000, 148 * 128 * 2 + 77])
 def test_fused_mlp_block_matches_fp64(rows):
     """One launch of the fused plain-forward MLP block (fused_tc.cuh: A = X + O Wo, M1 = tanh(A W1 + b1), X' = A + tanh(M1 W2 + b2),
-    half hi / lo operands on kind::f16, intermediates in TMEM / shared memory) against fp64; several tiles per CTA for the
+    half hi / lo operands on f16 wgmma, intermediates in registers / shared memory) against fp64; several tiles per CTA for the
     largest row count (barrier phases wrap), a ragged last tile, and in-place use (Out aliases O) as the engine calls it."""
     hamil, a, params, eng = _engine(1)
     g = torch.Generator(device='cpu').manual_seed(rows)
@@ -227,7 +198,7 @@ def _trunk_ref(eng, X0, N, L, H=4, dtype=torch.float64):
 @pytest.mark.parametrize('mol,walkers', [('LiH', 3), ('LiH', 32 * 148 * 2 + 5), ('benzene', 9), ('benzene', 4 * 148 * 3 + 1)])
 def test_fused_trunk_matches_fp64(mol, walkers):
     """ONE launch of the whole-trunk kernel (trunk_tc.cuh: all four attention layers of a plain forward, residual stream in
-    TMEM, operands in shared memory, Q / K / V through the per-CTA scratch planes, attention on mma.sync) against an fp64
+    per-CTA scratch, operands in shared memory, Q / K / V through the per-CTA scratch, fp32 attention) against an fp64
     restatement of the layers and against the same restatement in plain fp32: partial tiles, padding rows (benzene: 120 of
     128 tile rows), several tiles per CTA (barrier phases wrap)."""
     hamil = MolecularHamiltonian(mol=Molecule.from_name(mol), ecp_type='ccECP' if mol == 'benzene' else None)
@@ -244,7 +215,7 @@ def test_fused_trunk_matches_fp64(mol, walkers):
     err, err32 = (out.double() - ref).abs().max().item(), (ref32.double() - ref).abs().max().item()
     rms, rms32 = (out.double() - ref).pow(2).mean().sqrt().item(), (ref32.double() - ref).pow(2).mean().sqrt().item()
     assert torch.isfinite(out).all()
-    # fp32 class.  On the hardware the kind::f16 pipe sums the 16 products of an instruction with less than fp32 carry
+    # fp32 class.  On the hardware the f16 tensor-core pipe sums the 16 products of an instruction with less than fp32 carry
     # precision, so the result is a few ulp (measured: ~7x the plain-fp32 restatement in rms) off instead of the fraction of an
     # ulp an exact-product model gives; log|psi| and E_loc are not affected at their fp32 noise level (tools/acc_study.py).
     assert rms < 12 * rms32 + 1e-6 and err < 25 * err32 + 1e-5, (err, err32, rms, rms32)

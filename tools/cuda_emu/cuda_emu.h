@@ -131,7 +131,7 @@ inline T shfl_idx(T v, int src_lane) {
   std::memcpy(&out, &got, sizeof(T));
   return out;
 }
-// Launch limits of sm_100 that a CPU run would otherwise never notice: 1024 threads per block, grid.y/z <= 65535,
+// Launch limits of sm_90 that a CPU run would otherwise never notice: 1024 threads per block, grid.y/z <= 65535,
 // dynamic shared memory <= 48 KiB unless the kernel opted in (<= 227 KiB), and no write past the requested bytes.
 inline void check_limits(dim3 grid, dim3 block, size_t smem, const void* fn, const char* name) {
   State& s = S();

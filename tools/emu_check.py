@@ -15,7 +15,7 @@ import torch
 
 
 def build_emu(out='/tmp/libdqmc_emu.so'):
-    cmd = ['g++', '-std=c++17', '-O1', '-g', '-DDQMC_EMU', '-x', 'c++', f'-I{ROOT}/tools/cuda_emu',
+    cmd = ['g++', '-std=c++17', '-O1', '-g', '-DDQMC_EMU', '-DDQMC_NO_TCGEN05', '-x', 'c++', f'-I{ROOT}/tools/cuda_emu',
            f'-I{ROOT}/include', f'-I{ROOT}/deepqmc_b200/csrc', '-fPIC', '-shared',
            f'{ROOT}/deepqmc_b200/csrc/engine.cu', '-o', out]
     subprocess.check_call(cmd)

@@ -3,14 +3,14 @@
 NOT part of the product and not a parity claim -- the container this was written in has no GPU, so everything added after the
 round's GPU minutes ran out was first checked here (DESIGN.md section 8).  What a run checks beyond the test's own assertions:
   * the engine workspace, every cudaMalloc and every torch.empty of the host mirrors start poisoned (0xFF bytes: NaN / -1),
-  * launch limits of sm_100 (block size, grid dims, dynamic shared memory vs the opt-in) and a canary behind the dynamic
+  * launch limits of sm_90 (block size, grid dims, dynamic shared memory vs the opt-in) and a canary behind the dynamic
     shared memory of every block (tools/cuda_emu/cuda_emu.h),
   * DQMC_EMU_REVERSE=1: the threads of a block run from the highest index down (a missing barrier passes in one order at most),
   * DQMC_EMU_REVERSE_BLOCKS=1: the grid is walked backwards (blocks of one launch that depend on each other),
   * guard zones behind every buffer carved from the engine workspace (engine.cu DQ_TAKE_GUARD), verified after each chunk,
   * --asan: the kernels are compiled with AddressSanitizer (out-of-bounds global accesses; run with
     LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0:detect_stack_use_after_return=0).
-The tcgen05 / TMA GEMM cannot be emulated: engines are created with gemm_backend = 0.
+The wgmma / TMA kernels are not emulated (the build sets DQMC_NO_TCGEN05): engines are created with gemm_backend = 0.
 
 Usage:  python tools/emu_run_tests.py [--lib PATH] [--nobuild] [--asan] test_name [test_name ...]
         python tools/emu_run_tests.py --all-small          (every test small enough for the emulator, both files)
@@ -33,7 +33,7 @@ TOO_BIG = {'test_full_size_properties_4096_walkers', 'test_benzene_full_psiforme
 
 
 def build(out, asan=False):
-    cmd = ['g++', '-std=c++17', '-O1', '-g', '-DDQMC_EMU', '-x', 'c++', f'-I{ROOT}/tools/cuda_emu', f'-I{ROOT}/include',
+    cmd = ['g++', '-std=c++17', '-O1', '-g', '-DDQMC_EMU', '-DDQMC_NO_TCGEN05', '-x', 'c++', f'-I{ROOT}/tools/cuda_emu', f'-I{ROOT}/include',
            f'-I{ROOT}/deepqmc_b200/csrc', '-fPIC', '-shared', f'{ROOT}/deepqmc_b200/csrc/engine.cu', '-o', out]
     if asan:
         cmd[1:1] = ['-fsanitize=address', '-fno-omit-frame-pointer']

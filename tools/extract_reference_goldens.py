@@ -1,7 +1,7 @@
 """Extract the PARAM-FREE goldens of the reference's own test-suite into a small JSON fixture.
 
-Run in the build container (reads /root/reference/tests/**/*.npz, which do not travel to the
-GPU box):   python tools/extract_reference_goldens.py
+Run against a checkout of the reference (reads <reference>/tests/**/*.npz):
+    python tools/extract_reference_goldens.py <reference>/tests
 Only numbers are extracted (regression *data*), no reference source.  The parameter-dependent
 goldens (psi, its parameter gradient, Laplacian, E_loc of the Haiku-initialised test ansatz) are
 reproduced in tests/test_oracle_goldens.py by regenerating the Haiku / jax.random initialisation
@@ -9,10 +9,11 @@ in numpy (oracle/jaxrand.py); the walker is recovered from the edge-builder gold
 """
 import json
 import os
+import sys
 
 import numpy as np
 
-REF = '/root/reference/tests'
+REF = sys.argv[1] if len(sys.argv) > 1 else 'tests'
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests', 'golden', 'reference_goldens.json')
 
 
