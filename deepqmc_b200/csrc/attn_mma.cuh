@@ -79,17 +79,130 @@ __device__ __forceinline__ void am_split2(float x0, float x1, uint32_t& hi, uint
   lo = am_pack_half2(x0 - am_half_to_float(hi & 0xFFFFu), x1 - am_half_to_float(hi >> 16));
 }
 
+template <bool kCoherent>
+__device__ __forceinline__ float2 am_ld2(const float* p) {
+  if constexpr (kCoherent) return *(const float2*)p;
+  else return __ldg((const float2*)p);
+}
+template <bool kCoherent>
+__device__ __forceinline__ float am_ld1(const float* p) {
+  if constexpr (kCoherent) return *p;
+  else return __ldg(p);
+}
+
+// One warp task: 16 query rows of one head against 8 NK8 keys (dh = 64).  The caller supplies the rows and the mask; lane
+// (g = lane / 4, t = lane % 4) holds query rows g (i = 0) and g + 8 (i = 1):
+//   qrow(i)            query row i (64 fp32)
+//   krow(j), vrow(j)   key / value row j < 8 NK8 (padded keys must point at readable rows: their scores are masked)
+//   valid(i, j)        key j takes part in the softmax of query row i (every row needs at least one)
+//   store(i, c, o0, o1) normalised output of query row i, head columns c, c + 1
+// kCoherent: plain global loads (rows written earlier by the same kernel) instead of the read-only path.
+template <int NK8, bool kCoherent, class QRow, class KRow, class VRow, class Valid, class Store>
+__device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow, VRow vrow, Valid valid, Store store) {
+  constexpr int NK16 = (NK8 + 1) / 2;
+  constexpr float kQS = 16.f, kPS = 1024.f;  // operand scales: q, k, v by 2^4, probabilities by 2^10
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  // ---- Q fragments of this query tile (rows g, g + 8), hi / lo, 4 k-tiles of 16
+  const float* qp0 = qrow(0);
+  const float* qp1 = qrow(1);
+  uint32_t qh[4][4], ql[4][4];
+#pragma unroll
+  for (int kt = 0; kt < 4; ++kt) {
+    const float2 a0 = am_ld2<kCoherent>(qp0 + kt * 16 + 2 * t), a1 = am_ld2<kCoherent>(qp1 + kt * 16 + 2 * t);
+    const float2 a2 = am_ld2<kCoherent>(qp0 + kt * 16 + 8 + 2 * t), a3 = am_ld2<kCoherent>(qp1 + kt * 16 + 8 + 2 * t);
+    am_split2(a0.x * kQS, a0.y * kQS, qh[kt][0], ql[kt][0]);
+    am_split2(a1.x * kQS, a1.y * kQS, qh[kt][1], ql[kt][1]);
+    am_split2(a2.x * kQS, a2.y * kQS, qh[kt][2], ql[kt][2]);
+    am_split2(a3.x * kQS, a3.y * kQS, qh[kt][3], ql[kt][3]);
+  }
+  // ---- scores: S[16 x 8 NK8] = Q K^T; B fragment of key tile nt: (k = dh index, n = key nt * 8 + g)
+  float s[NK8][4];
+#pragma unroll
+  for (int nt = 0; nt < NK8; ++nt) {
+    s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+    const float* kp = krow(nt * 8 + g);
+#pragma unroll
+    for (int kt = 0; kt < 4; ++kt) {
+      const float2 b0 = am_ld2<kCoherent>(kp + kt * 16 + 2 * t), b1 = am_ld2<kCoherent>(kp + kt * 16 + 8 + 2 * t);
+      uint32_t kh[2], kl[2];
+      am_split2(b0.x * kQS, b0.y * kQS, kh[0], kl[0]);
+      am_split2(b1.x * kQS, b1.y * kQS, kh[1], kl[1]);
+      mma16816(s[nt], qh[kt], kl);
+      mma16816(s[nt], ql[kt], kh);
+      mma16816(s[nt], qh[kt], kh);
+    }
+  }
+  // ---- softmax over the keys of rows g (c0, c1) and g + 8 (c2, c3); a lane holds keys nt * 8 + 2 t, + 1
+  const float us = scale / (kQS * kQS);
+  float m0 = -3.0e38f, m1 = -3.0e38f;
+#pragma unroll
+  for (int nt = 0; nt < NK8; ++nt) {
+    const int j0 = nt * 8 + 2 * t;
+    s[nt][0] = valid(0, j0) ? s[nt][0] * us : -3.0e38f;
+    s[nt][1] = valid(0, j0 + 1) ? s[nt][1] * us : -3.0e38f;
+    s[nt][2] = valid(1, j0) ? s[nt][2] * us : -3.0e38f;
+    s[nt][3] = valid(1, j0 + 1) ? s[nt][3] * us : -3.0e38f;
+    m0 = fmaxf(m0, fmaxf(s[nt][0], s[nt][1]));
+    m1 = fmaxf(m1, fmaxf(s[nt][2], s[nt][3]));
+  }
+  m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1)); m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+  m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+  float l0 = 0.f, l1 = 0.f;
+#pragma unroll
+  for (int nt = 0; nt < NK8; ++nt) {
+    s[nt][0] = m_exp(s[nt][0] - m0); s[nt][1] = m_exp(s[nt][1] - m0);
+    s[nt][2] = m_exp(s[nt][2] - m1); s[nt][3] = m_exp(s[nt][3] - m1);
+    l0 += s[nt][0] + s[nt][1];
+    l1 += s[nt][2] + s[nt][3];
+  }
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  // ---- probabilities as A fragments of P V: key tile pair (2 kk, 2 kk + 1) = one 16-key k-tile
+  uint32_t ph[NK16][4], pl[NK16][4];
+#pragma unroll
+  for (int kk = 0; kk < NK16; ++kk) {
+    const int n0 = 2 * kk, n1 = 2 * kk + 1;
+    am_split2(s[n0][0] * kPS, s[n0][1] * kPS, ph[kk][0], pl[kk][0]);
+    am_split2(s[n0][2] * kPS, s[n0][3] * kPS, ph[kk][1], pl[kk][1]);
+    if (n1 < NK8) {
+      am_split2(s[n1 < NK8 ? n1 : n0][0] * kPS, s[n1 < NK8 ? n1 : n0][1] * kPS, ph[kk][2], pl[kk][2]);
+      am_split2(s[n1 < NK8 ? n1 : n0][2] * kPS, s[n1 < NK8 ? n1 : n0][3] * kPS, ph[kk][3], pl[kk][3]);
+    } else {
+      ph[kk][2] = ph[kk][3] = pl[kk][2] = pl[kk][3] = 0u;
+    }
+  }
+  // ---- O[16 x 64] = P V: B fragment of dh tile nt: (k = key 16 kk + 2 t (+1, +8, +9), n = dh nt * 8 + g)
+  const float uo0 = 1.f / (l0 * kPS * kQS), uo1 = 1.f / (l1 * kPS * kQS);
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) {
+    float o[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < NK16; ++kk) {
+      const int j = kk * 16 + 2 * t;
+      const float v00 = am_ld1<kCoherent>(vrow(j) + nt * 8 + g), v01 = am_ld1<kCoherent>(vrow(j + 1) + nt * 8 + g);
+      const float v10 = am_ld1<kCoherent>(vrow(j + 8) + nt * 8 + g), v11 = am_ld1<kCoherent>(vrow(j + 9) + nt * 8 + g);
+      uint32_t vh[2], vl[2];
+      am_split2(v00 * kQS, v01 * kQS, vh[0], vl[0]);
+      am_split2(v10 * kQS, v11 * kQS, vh[1], vl[1]);
+      mma16816(o, ph[kk], vl);
+      mma16816(o, pl[kk], vh);
+      mma16816(o, ph[kk], vh);
+    }
+    store(0, nt * 8 + 2 * t, o[0] * uo0, o[1] * uo0);
+    store(1, nt * 8 + 2 * t, o[2] * uo1, o[3] * uo1);
+  }
+}
+
 // NK8 = number of 8-key tiles (keys padded to 8 NK8 <= 48); block = 4 warps, each warp walks over (pair, query tile) tasks.
 template <int NK8>
 __global__ void __launch_bounds__(128)
 attn_fwd_mma_kernel(const float* __restrict__ QKV, int ldq, float* __restrict__ O, int ldo, int N, int H, int dmodel, float scale,
                     int n_pairs, const float* __restrict__ Kn, const float* __restrict__ Vn, int Mn) {
-  constexpr int DH = 64, NK16 = (NK8 + 1) / 2;
-  constexpr float kQS = 16.f, kPS = 1024.f;  // operand scales: q, k, v by 2^4, probabilities by 2^10
-  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  constexpr int DH = 64;
   const int NKEY = N + Mn;
   const int MT = (N + 15) / 16;  // query tiles per pair
   const int n_tasks = n_pairs * MT;
+  const int g = (threadIdx.x & 31) >> 2;
   const int wglobal = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), wtotal = gridDim.x * (blockDim.x >> 5);
   for (int task = wglobal; task < n_tasks; task += wtotal) {
     const int pair = task / MT, mt = task - pair * MT;
@@ -104,98 +217,17 @@ attn_fwd_mma_kernel(const float* __restrict__ QKV, int ldq, float* __restrict__ 
       j = j < NKEY ? j : NKEY - 1;
       return j < N ? base + (size_t)j * ldq + 2 * dmodel : Vn + (size_t)(j - N) * dmodel + h * DH;
     };
-    // ---- Q fragments of this query tile (rows g, g + 8), hi / lo, 4 k-tiles of 16
     const int q0 = mt * 16 + g, q1 = q0 + 8;
-    const float* qp0 = base + (size_t)(q0 < N ? q0 : N - 1) * ldq;
-    const float* qp1 = base + (size_t)(q1 < N ? q1 : N - 1) * ldq;
-    uint32_t qh[4][4], ql[4][4];
-#pragma unroll
-    for (int kt = 0; kt < 4; ++kt) {
-      const float2 a0 = __ldg((const float2*)(qp0 + kt * 16 + 2 * t)), a1 = __ldg((const float2*)(qp1 + kt * 16 + 2 * t));
-      const float2 a2 = __ldg((const float2*)(qp0 + kt * 16 + 8 + 2 * t)), a3 = __ldg((const float2*)(qp1 + kt * 16 + 8 + 2 * t));
-      am_split2(a0.x * kQS, a0.y * kQS, qh[kt][0], ql[kt][0]);
-      am_split2(a1.x * kQS, a1.y * kQS, qh[kt][1], ql[kt][1]);
-      am_split2(a2.x * kQS, a2.y * kQS, qh[kt][2], ql[kt][2]);
-      am_split2(a3.x * kQS, a3.y * kQS, qh[kt][3], ql[kt][3]);
-    }
-    // ---- scores: S[16 x 8 NK8] = Q K^T; B fragment of key tile nt: (k = dh index, n = key nt * 8 + g)
-    float s[NK8][4];
-#pragma unroll
-    for (int nt = 0; nt < NK8; ++nt) {
-      s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-      const float* kp = krow(nt * 8 + g);
-#pragma unroll
-      for (int kt = 0; kt < 4; ++kt) {
-        const float2 b0 = __ldg((const float2*)(kp + kt * 16 + 2 * t)), b1 = __ldg((const float2*)(kp + kt * 16 + 8 + 2 * t));
-        uint32_t kh[2], kl[2];
-        am_split2(b0.x * kQS, b0.y * kQS, kh[0], kl[0]);
-        am_split2(b1.x * kQS, b1.y * kQS, kh[1], kl[1]);
-        mma16816(s[nt], qh[kt], kl);
-        mma16816(s[nt], ql[kt], kh);
-        mma16816(s[nt], qh[kt], kh);
-      }
-    }
-    // ---- softmax over the keys of rows g (c0, c1) and g + 8 (c2, c3); a lane holds keys nt * 8 + 2 t, + 1
-    const float us = scale / (kQS * kQS);
-    float m0 = -3.0e38f, m1 = -3.0e38f;
-#pragma unroll
-    for (int nt = 0; nt < NK8; ++nt) {
-      const int j0 = nt * 8 + 2 * t;
-      s[nt][0] = j0 < NKEY ? s[nt][0] * us : -3.0e38f;
-      s[nt][1] = j0 + 1 < NKEY ? s[nt][1] * us : -3.0e38f;
-      s[nt][2] = j0 < NKEY ? s[nt][2] * us : -3.0e38f;
-      s[nt][3] = j0 + 1 < NKEY ? s[nt][3] * us : -3.0e38f;
-      m0 = fmaxf(m0, fmaxf(s[nt][0], s[nt][1]));
-      m1 = fmaxf(m1, fmaxf(s[nt][2], s[nt][3]));
-    }
-    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1)); m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-    float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-    for (int nt = 0; nt < NK8; ++nt) {
-      s[nt][0] = m_exp(s[nt][0] - m0); s[nt][1] = m_exp(s[nt][1] - m0);
-      s[nt][2] = m_exp(s[nt][2] - m1); s[nt][3] = m_exp(s[nt][3] - m1);
-      l0 += s[nt][0] + s[nt][1];
-      l1 += s[nt][2] + s[nt][3];
-    }
-    l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    // ---- probabilities as A fragments of P V: key tile pair (2 kk, 2 kk + 1) = one 16-key k-tile
-    uint32_t ph[NK16][4], pl[NK16][4];
-#pragma unroll
-    for (int kk = 0; kk < NK16; ++kk) {
-      const int n0 = 2 * kk, n1 = 2 * kk + 1;
-      am_split2(s[n0][0] * kPS, s[n0][1] * kPS, ph[kk][0], pl[kk][0]);
-      am_split2(s[n0][2] * kPS, s[n0][3] * kPS, ph[kk][1], pl[kk][1]);
-      if (n1 < NK8) {
-        am_split2(s[n1 < NK8 ? n1 : n0][0] * kPS, s[n1 < NK8 ? n1 : n0][1] * kPS, ph[kk][2], pl[kk][2]);
-        am_split2(s[n1 < NK8 ? n1 : n0][2] * kPS, s[n1 < NK8 ? n1 : n0][3] * kPS, ph[kk][3], pl[kk][3]);
-      } else {
-        ph[kk][2] = ph[kk][3] = pl[kk][2] = pl[kk][3] = 0u;
-      }
-    }
-    // ---- O[16 x 64] = P V: B fragment of dh tile nt: (k = key 16 kk + 2 t (+1, +8, +9), n = dh nt * 8 + g)
-    const float uo0 = 1.f / (l0 * kPS * kQS), uo1 = 1.f / (l1 * kPS * kQS);
-    float* op0 = O + ((size_t)b * N + q0) * ldo + h * DH;
-    float* op1 = O + ((size_t)b * N + q1) * ldo + h * DH;
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-      float o[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int kk = 0; kk < NK16; ++kk) {
-        const int j = kk * 16 + 2 * t;
-        const float v00 = __ldg(vrow(j) + nt * 8 + g), v01 = __ldg(vrow(j + 1) + nt * 8 + g);
-        const float v10 = __ldg(vrow(j + 8) + nt * 8 + g), v11 = __ldg(vrow(j + 9) + nt * 8 + g);
-        uint32_t vh[2], vl[2];
-        am_split2(v00 * kQS, v01 * kQS, vh[0], vl[0]);
-        am_split2(v10 * kQS, v11 * kQS, vh[1], vl[1]);
-        mma16816(o, ph[kk], vl);
-        mma16816(o, pl[kk], vh);
-        mma16816(o, ph[kk], vh);
-      }
-      if (q0 < N) *(float2*)(op0 + nt * 8 + 2 * t) = make_float2(o[0] * uo0, o[1] * uo0);
-      if (q1 < N) *(float2*)(op1 + nt * 8 + 2 * t) = make_float2(o[2] * uo1, o[3] * uo1);
-    }
+    auto qrow = [&](int i) -> const float* {
+      const int q = i ? q1 : q0;
+      return base + (size_t)(q < N ? q : N - 1) * ldq;
+    };
+    auto valid = [&](int, int j) { return j < NKEY; };
+    auto store = [&](int i, int c, float o0, float o1) {
+      const int q = i ? q1 : q0;
+      if (q < N) *(float2*)(O + ((size_t)b * N + q) * ldo + h * DH + c) = make_float2(o0, o1);
+    };
+    attn_task_mma<NK8, false>(scale, qrow, krow, vrow, valid, store);
   }
 }
 

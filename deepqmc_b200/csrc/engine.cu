@@ -74,6 +74,7 @@ struct EngineBase {
   virtual int stats_pack(const void* E, const void* stats, int B, double* out, cudaStream_t st) = 0;
   virtual int debug_mlp_block(int layer, const void* O, const void* X, void* Out, int rows, cudaStream_t st) = 0;
   virtual int debug_trunk(const void* X0, void* Out, int rows, cudaStream_t st) = 0;
+  virtual int debug_trunk_phases(uint64_t* out, int n) = 0;
   virtual int forward(const void* r, const void* R, int Rb, int B, void* sign, void* logp, void* ws, int64_t wsb,
                       cudaStream_t st) = 0;
   virtual int local_energy(const void* r, const void* R, int Rb, int B, uint64_t seed, const void* twist, void* E,
@@ -358,6 +359,7 @@ struct Engine : EngineBase {
   bool fuse_trunk = true;  // all layers of a plain forward in one persistent launch (trunk_tc.cuh); DQMC_TC_TRUNK=0 disables
   CUtensorMap* d_trunk_maps = nullptr;       // [L][4][2]
   unsigned char* d_trunk_scratch = nullptr;  // n_sms x 512 KB: Q / K / V and residual rows of a tile
+  unsigned long long* d_trunk_phase = nullptr;  // DQMC_TRUNK_PHASES=1: the whole-trunk kernel's phase timers (tc::kPhases)
   bool f16_on = true;      // plain forwards (S = 1) on f16 wgmma with hi / lo half operands; DQMC_TC_F16=0: stay on 3xTF32
   bool fuse_mlp = true;    // W_o + residual -> W1 + tanh -> W2 + tanh + residual in one launch (S = 1); DQMC_TC_FUSE_MLP=0 disables
   static constexpr float kActScale = 16.f;  // 2^4: |activation| < 4094 representable, absolute floor 2^-29
@@ -576,6 +578,10 @@ struct Engine : EngineBase {
       if (psif && !trans && d == 256 && H == 4 && N <= 32 && cfg.n_layers <= tc::kTrMaxLayers) {
         DQ_CHECK(cudaMalloc((void**)&d_trunk_maps, sizeof(CUtensorMap) * 8 * cfg.n_layers));
         DQ_CHECK(cudaMalloc((void**)&d_trunk_scratch, (size_t)n_sms * tc::kTrScratchPerCta));
+        if (const char* ev = std::getenv("DQMC_TRUNK_PHASES"); ev && std::atoi(ev) != 0) {
+          DQ_CHECK(cudaMalloc((void**)&d_trunk_phase, sizeof(unsigned long long) * tc::kPhases));
+          DQ_CHECK(cudaMemset(d_trunk_phase, 0, sizeof(unsigned long long) * tc::kPhases));
+        }
       }
 #else
       err = "this build has no tensor-core backend"; return 2;
@@ -599,6 +605,7 @@ struct Engine : EngineBase {
     }
     if (d_trunk_maps) cudaFree(d_trunk_maps);
     if (d_trunk_scratch) cudaFree(d_trunk_scratch);
+    if (d_trunk_phase) cudaFree(d_trunk_phase);
 #endif
   }
   const T* P(const std::string& n) const { return d_params + off(n); }
@@ -1026,7 +1033,7 @@ struct Engine : EngineBase {
       int np2 = 1;
       while (np2 < N) np2 *= 2;  // walker slot of the tile: electrons rounded up to a power of two (<= 32)
       p.walkers = rows / N; p.N = N; p.NP = np2; p.L = cfg.n_layers; p.a_scale = kActScale;
-      p.attn_scale = (float)(1.0 / std::sqrt((double)dh)); p.err_flag = nullptr;
+      p.attn_scale = (float)(1.0 / std::sqrt((double)dh)); p.err_flag = nullptr; p.phase = d_trunk_phase;
       for (int l = 0; l < cfg.n_layers; ++l) {
         const std::string pfx = "L" + std::to_string(l) + ".";
         p.b1[l] = P(pfx + "b1"); p.b2[l] = P(pfx + "b2");
@@ -1052,6 +1059,17 @@ struct Engine : EngineBase {
 #endif
     err = "internal: fused trunk without the tensor-core backend";
     return 5;
+  }
+  int debug_trunk_phases(uint64_t* out, int n) override {
+#if !defined(DQMC_NO_TCGEN05)
+    if (!d_trunk_phase) { err = "trunk phase timers are off (set DQMC_TRUNK_PHASES=1 before creating the engine)"; return 2; }
+    if (n < tc::kPhases) { err = "dqmc_debug_trunk_phases: the output holds fewer than the kernel's counters"; return 2; }
+    DQ_CHECK(cudaMemcpy(out, d_trunk_phase, sizeof(unsigned long long) * tc::kPhases, cudaMemcpyDeviceToHost));
+    DQ_CHECK(cudaMemset(d_trunk_phase, 0, sizeof(unsigned long long) * tc::kPhases));
+    return 0;
+#else
+    err = "this build has no tensor-core backend"; return 2;
+#endif
   }
   int debug_trunk(const void* X0, void* Out, int rows, cudaStream_t st) override {
     if (!can_trunk(1)) { err = "fused trunk not available for this configuration"; return 2; }
@@ -2512,6 +2530,12 @@ int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, voi
   if (!h) return 2;
   DQ_NEED_DEVICE(h);
   return h->e->debug_trunk(X0, Out, rows, (cudaStream_t)stream);
+}
+int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!out) { h->e->err = "dqmc_debug_trunk_phases: null output"; return 2; }
+  return h->e->debug_trunk_phases(out, n);
 }
 
 int dqmc_profile_begin(dqmc_handle h) {

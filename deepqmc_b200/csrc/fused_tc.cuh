@@ -43,7 +43,34 @@ struct MlpSmem {
   static __host__ __device__ int wring(int s) { return 131072 + s * 32768; }                      // [<= 256 rows][128 B]
   static __host__ __device__ int bias() { return 131072 + kMlpSlots * 32768; }                    // b1[256], b2[256]
   static __host__ __device__ int bars() { return bias() + 2048; }
-  static __host__ __device__ int total() { return bars() + 64; }
+  static __host__ __device__ int phases() { return bars() + 64; }                                 // [2][kPhases] u64
+  static __host__ __device__ int total() { return phases() + 2 * 8 * 16; }
+};
+
+// Phase timers of the whole-trunk kernel (TrunkParams::phase): clock64() cycles summed over the consumer warpgroups of all
+// CTAs, in this order; kPhWait is the time spent waiting for weight slots to land and is not part of the mainloop phases.
+enum Phase { kPhLoad, kPhQkv, kPhQkvEpi, kPhAttn, kPhWo, kPhW1, kPhW2, kPhMlpEpi, kPhWait, kPhPairs, kPhases };
+static_assert(kPhases <= 16, "MlpSmem::phases() holds 16 counters per warpgroup");
+struct PhaseClock {
+  unsigned long long* acc;  // this warpgroup's shared-memory counters on its timing thread, nullptr: not timing
+  long long t;
+  __device__ __forceinline__ explicit PhaseClock(unsigned long long* a) : acc(a), t(0) {
+    if (a) t = clock64();
+  }
+  // the time since the last mark goes to phase k
+  __device__ __forceinline__ void mark(int k) {
+    if (acc) {
+      const long long n = clock64();
+      acc[k] += (unsigned long long)(n - t);
+      t = n;
+    }
+  }
+  __device__ __forceinline__ void count(int k) { if (acc) acc[k] += 1; }
+  // w cycles of weight wait inside the current phase: booked to kPhWait instead
+  __device__ __forceinline__ void waited(long long w) {
+    acc[kPhWait] += (unsigned long long)w;
+    t += w;
+  }
 };
 
 // tanh of the plain-forward epilogues (same as gemm_wgmma.cuh tanh_fwd): absolute error <= ~3e-7
@@ -94,7 +121,7 @@ __device__ __forceinline__ void store_operand_quad(unsigned char* smem, int row,
 // `nslot` counts the ring slots used so far: slot g lives in ring stage g % 3 and completes phase (g / 3) & 1 of its barrier.
 template <int D>
 __device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* smem, uint64_t* full, uint32_t& nslot,
-                                          const CUtensorMap* mh, const CUtensorMap* ml, int y0, int* err) {
+                                          const CUtensorMap* mh, const CUtensorMap* ml, int y0, int* err, PhaseClock& pc) {
   constexpr int KB = D / 64;
   constexpr int NS = 2 * KB;  // slots of this GEMM: slot i = plane i % 2 (hi, lo) of k-block i / 2
   static_assert(NS >= kMlpSlots, "the ring is filled at the start of a GEMM");
@@ -113,7 +140,9 @@ __device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* sm
   // waits for slot i and returns its shared-memory address
   auto acquire = [&](int i) {
     const int st = stage(i);
+    const long long t0 = pc.acc ? clock64() : 0;
     mbar_wait(&full[st], ((nslot + (uint32_t)i) / (uint32_t)kMlpSlots) & 1u, err);
+    if (pc.acc) pc.waited(clock64() - t0);
     return smem_u32(smem + MlpSmem::wring(st));
   };
   // slot i retired by both warpgroups -> its stage takes slot i + 3
@@ -172,13 +201,14 @@ __device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, u
                                      const CUtensorMap* w1_lo, const CUtensorMap* w2_hi, const CUtensorMap* w2_lo, float us0,
                                      float us1, float us2, float a_scale, const float* sb1, const float* sb2,
                                      const float* const (&xin)[2], float* const (&aout)[2], float* const (&xout)[2],
-                                     bool operand_out, int* err) {
+                                     bool operand_out, int* err, PhaseClock& pc) {
   const Frag f;
   // Row loads are issued in batches of kJ fragment columns ahead of the stores: xin / aout / xout may alias, so the compiler
   // would otherwise wait for every load behind the previous store.
   constexpr int kJ = 4;
   // ---- A = X + O Wo -> parked rows and the operand buffer
-  gemm_abuf<D>(acc, smem, full, nslot, wo_hi, wo_lo, 0, err);
+  gemm_abuf<D>(acc, smem, full, nslot, wo_hi, wo_lo, 0, err, pc);
+  pc.mark(kPhWo);
 #pragma unroll
   for (int jb = 0; jb < D / 8; jb += kJ) {
     float2 x[kJ][2];
@@ -198,8 +228,10 @@ __device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, u
   }
   fence_proxy_async();
   __syncthreads();
+  pc.mark(kPhMlpEpi);
   // ---- M1 = tanh(A W1 + b1) -> operand buffer
-  gemm_abuf<D>(acc, smem, full, nslot, w1_hi, w1_lo, 0, err);
+  gemm_abuf<D>(acc, smem, full, nslot, w1_hi, w1_lo, 0, err, pc);
+  pc.mark(kPhW1);
 #pragma unroll
   for (int j = 0; j < D / 8; ++j)
 #pragma unroll
@@ -210,8 +242,10 @@ __device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, u
     }
   fence_proxy_async();
   __syncthreads();
+  pc.mark(kPhMlpEpi);
   // ---- X' = A + tanh(M1 W2 + b2)
-  gemm_abuf<D>(acc, smem, full, nslot, w2_hi, w2_lo, 0, err);
+  gemm_abuf<D>(acc, smem, full, nslot, w2_hi, w2_lo, 0, err, pc);
+  pc.mark(kPhW2);
 #pragma unroll
   for (int jb = 0; jb < D / 8; jb += kJ) {
     float2 a[kJ][2];
@@ -231,6 +265,7 @@ __device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, u
         if (operand_out) store_operand_pair(smem, f.fr + 8 * h, c, x0 * a_scale, x1 * a_scale);
       }
   }
+  pc.mark(kPhMlpEpi);
 }
 
 template <int D>
@@ -260,6 +295,7 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
   const Frag f;
   uint32_t nslot = 0;
   float acc[D / 2];
+  PhaseClock pc(nullptr);
   for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
     // ---- stage the O tile: coalesced float4 loads, hi / lo split
     for (int idx = tid; idx < 128 * (D / 4); idx += kMlpThreads) {
@@ -282,7 +318,7 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
       aout[h] = valid ? p.Out + (size_t)grow * p.ldout : nullptr;
     }
     mlp3<D>(acc, smem, full, nslot, &wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo, p.us0, p.us1, p.us2, p.a_scale, sb1, sb2,
-            xin, aout, aout, false, p.err_flag);
+            xin, aout, aout, false, p.err_flag, pc);
   }
 }
 

@@ -14,12 +14,16 @@
 // tile and layer, i.e. L2 resident): the register file holds one accumulator, and shared memory (operand buffer + ring)
 // cannot park them.
 //
-// Attention, one head at a time for the whole tile: K_h and V_h of the tile are staged in the (then idle) weight ring as
-// fp32; two threads per tile row (32 head columns each) run an online softmax over the keys of the row's own walker and write
-// O_h straight into k-block h of the Wo operand.
+// Attention on the tensor cores: warp w takes tile rows r0 = 16 w .. +15 and runs the 3xFP16 mma.sync task of attn_mma.cuh
+// (shared with attn_fwd_mma_kernel) for each head, with Q, K and V read straight from the scratch (plain, coherent loads: the
+// rows were written by this kernel) and O_h written, scaled and split, into k-block h of the operand buffer (dead once the
+// QKV GEMMs have retired).  The keys of a task are its walker slot (NP = 32: 4 key tiles of 8) or, for slots of at most 16
+// rows, the task's own 16 rows masked to the query's slot (2 key tiles).  Padding rows (electron >= N) get no attention
+// output: their operand rows keep the finite previous operand and are never stored.
 #pragma once
 #include <cstdint>
 
+#include "attn_mma.cuh"
 #include "common.cuh"
 #include "fused_tc.cuh"
 #include "tc_ptx.cuh"
@@ -48,6 +52,7 @@ struct TrunkParams {
   float a_scale;                 // power of two applied to activations before the hi / lo split
   float attn_scale;              // 1 / sqrt(dh)
   int* err_flag;
+  unsigned long long* phase;     // kPhases cycle / pair counters (fused_tc.cuh Phase), accumulated; nullptr: timers off
 };
 
 __global__ void __launch_bounds__(kTrThreads, 1)
@@ -57,8 +62,6 @@ trunk_f16_kernel(TrunkParams p) {
   uint64_t* full = (uint64_t*)(smem + TrSmem::bars());
   float* sb1 = (float*)(smem + TrSmem::bias());
   float* sb2 = sb1 + 256;
-  float* kst = (float*)(smem + TrSmem::wring(0));  // attention: K_h [128][64] fp32
-  float* vst = (float*)(smem + TrSmem::wring(1));  //            V_h [128][64] fp32
 
   const int tid = threadIdx.x;
   const int N = p.N, NP = p.NP, L = p.L;
@@ -73,13 +76,16 @@ trunk_f16_kernel(TrunkParams p) {
     fence_barrier_init();
     for (int i = 0; i < 8 * L; ++i) tma_prefetch_desc(p.maps + i);
   }
+  unsigned long long* ph = (unsigned long long*)(smem + TrSmem::phases());
+  if (tid < 32) ph[tid] = 0ull;
   __syncthreads();
+  PhaseClock pc(p.phase && (tid & 127) == 0 ? ph + 16 * (tid >> 7) : nullptr);
   const Frag f;
   uint32_t nslot = 0;
   float acc[128];
-  // attention task of this thread: tile row ar, head columns 32 ah .. +31
-  const int ar = tid >> 1, ah = tid & 1;
-  const int a_slot = ar >> lnp;
+  // attention task of this warp: tile rows r0 .. r0 + 15 (lane: rows r0 + ag, r0 + ag + 8), keys from tile row k0
+  const int r0 = 16 * (tid >> 5), ag = (tid & 31) >> 2;
+  const int k0 = r0 & ~((NP > 16 ? NP : 16) - 1);
   for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
     // global row of tile row r (-1: padding row or walker past the end)
     auto grow_of = [&](int r) -> long long {
@@ -114,12 +120,14 @@ trunk_f16_kernel(TrunkParams p) {
     }
     fence_proxy_async();
     __syncthreads();
+    pc.mark(kPhLoad);
     for (int l = 0; l < L; ++l) {
       const bool last = l == L - 1;
       const CUtensorMap* lm = p.maps + 8 * l;
       // ---- Q | K | V = X Wqkv, 256 columns at a time -> scratch (true values)
       for (int j = 0; j < 3; ++j) {
-        gemm_abuf<256>(acc, smem, full, nslot, lm, lm + 1, 256 * j, p.err_flag);
+        gemm_abuf<256>(acc, smem, full, nslot, lm, lm + 1, 256 * j, p.err_flag, pc);
+        pc.mark(kPhQkv);
         const float us = p.us[l][0];
 #pragma unroll
         for (int jj = 0; jj < 32; ++jj)
@@ -127,71 +135,31 @@ trunk_f16_kernel(TrunkParams p) {
           for (int h = 0; h < 2; ++h)
             *(float2*)(qkv + (f.fr + 8 * h) * 768 + 256 * j + 8 * jj + f.fc) =
                 make_float2(acc[4 * jj + 2 * h] * us, acc[4 * jj + 2 * h + 1] * us);
+        pc.mark(kPhQkvEpi);
       }
       sb1[tid] = __ldg(p.b1[l] + tid);
       sb2[tid] = __ldg(p.b2[l] + tid);
       __syncthreads();  // Q / K / V rows of the whole tile are in the scratch buffer
-      // ---- attention, head by head
+      // ---- attention on the tensor cores, head by head -> k-block h of the operand buffer
       for (int h = 0; h < 4; ++h) {
-        {
-          float4 kv[2 * 128 * 16 / kTrThreads];  // all loads of this thread first, then the stores
-#pragma unroll
-          for (int i = 0; i < 128 * 16 / kTrThreads; ++i) {
-            const int idx = tid + kTrThreads * i, r = idx >> 4, c = 4 * (idx & 15);
-            kv[2 * i] = *(const float4*)(qkv + r * 768 + 256 + 64 * h + c);
-            kv[2 * i + 1] = *(const float4*)(qkv + r * 768 + 512 + 64 * h + c);
-          }
-#pragma unroll
-          for (int i = 0; i < 128 * 16 / kTrThreads; ++i) {
-            const int idx = tid + kTrThreads * i, r = idx >> 4, c = 4 * (idx & 15);
-            *(float4*)(kst + r * 64 + c) = kv[2 * i];
-            *(float4*)(vst + r * 64 + c) = kv[2 * i + 1];
-          }
-        }
-        __syncthreads();
-        float q[32], o[32];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 v = *(const float4*)(qkv + ar * 768 + 64 * h + 32 * ah + 4 * i);
-          q[4 * i] = v.x; q[4 * i + 1] = v.y; q[4 * i + 2] = v.z; q[4 * i + 3] = v.w;
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = 0.f;
-        float mx = -3.0e38f, sum = 0.f;
-        for (int e = 0; e < N; ++e) {  // keys of this row's walker
-          const int kr = (a_slot << lnp) + e;
-          const float* kp = kst + kr * 64 + 32 * ah;
-          float sp[4] = {0.f, 0.f, 0.f, 0.f};  // four independent partial sums: the dot product is not one dependent chain
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 k4 = *(const float4*)(kp + 4 * i);
-            sp[i & 3] += q[4 * i] * k4.x + q[4 * i + 1] * k4.y + q[4 * i + 2] * k4.z + q[4 * i + 3] * k4.w;
-          }
-          float s = (sp[0] + sp[1]) + (sp[2] + sp[3]);
-          s = (s + __shfl_xor_sync(0xffffffffu, s, 1)) * p.attn_scale;
-          const float mnew = fmaxf(mx, s);
-          const float corr = __expf(mx - mnew), pe = __expf(s - mnew);
-          sum = sum * corr + pe;
-          mx = mnew;
-          const float* vp = vst + kr * 64 + 32 * ah;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 v4 = *(const float4*)(vp + 4 * i);
-            o[4 * i] = o[4 * i] * corr + pe * v4.x;
-            o[4 * i + 1] = o[4 * i + 1] * corr + pe * v4.y;
-            o[4 * i + 2] = o[4 * i + 2] * corr + pe * v4.z;
-            o[4 * i + 3] = o[4 * i + 3] * corr + pe * v4.w;
-          }
-        }
-        const float un = p.a_scale / sum;
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          store_operand_quad(smem, ar, 64 * h + 32 * ah + 4 * i,
-                             make_float4(o[4 * i] * un, o[4 * i + 1] * un, o[4 * i + 2] * un, o[4 * i + 3] * un));
-        __syncthreads();  // K_h / V_h staging is re-used by the next head (and the ring by the next GEMM)
+        const float* qb = qkv + 64 * h;
+        auto qrow = [&](int i) -> const float* { return qb + (r0 + ag + 8 * i) * 768; };
+        auto krow = [&](int j) -> const float* { return qb + (k0 + j) * 768 + 256; };
+        auto vrow = [&](int j) -> const float* { return qb + (k0 + j) * 768 + 512; };
+        auto valid = [&](int i, int j) {
+          const int r = r0 + ag + 8 * i, k = k0 + j;
+          return (k >> lnp) == (r >> lnp) && (k & (NP - 1)) < N;
+        };
+        auto store = [&](int i, int c, float o0, float o1) {
+          const int r = r0 + ag + 8 * i;
+          if ((r & (NP - 1)) < N) store_operand_pair(smem, r, 64 * h + c, o0 * p.a_scale, o1 * p.a_scale);
+        };
+        if (NP > 16) attn_task_mma<4, true>(p.attn_scale, qrow, krow, vrow, valid, store);
+        else attn_task_mma<2, true>(p.attn_scale, qrow, krow, vrow, valid, store);
       }
       fence_proxy_async();
       __syncthreads();
+      pc.mark(kPhAttn);
       // ---- A = X + O Wo, M1 = tanh(A W1 + b1), X = A + tanh(M1 W2 + b2)
       const float* xin[2];
       float* aout[2];
@@ -205,11 +173,15 @@ trunk_f16_kernel(TrunkParams p) {
         xout[h] = !last ? resid + r * 256 : (row >= 0 ? p.Out + (size_t)row * p.ldout : nullptr);
       }
       mlp3<256>(acc, smem, full, nslot, lm + 2, lm + 3, lm + 4, lm + 5, lm + 6, lm + 7, p.us[l][1], p.us[l][2], p.us[l][3],
-                p.a_scale, sb1, sb2, xin, aout, xout, !last, p.err_flag);
+                p.a_scale, sb1, sb2, xin, aout, xout, !last, p.err_flag, pc);
       fence_proxy_async();
       __syncthreads();  // next layer's operand complete / next tile's load may overwrite the residual rows
+      pc.mark(kPhMlpEpi);
+      if (tid < 128) pc.count(kPhPairs);
     }
   }
+  if (pc.acc)
+    for (int k = 0; k < kPhases; ++k) atomicAdd(p.phase + k, pc.acc[k]);
 }
 
 }  // namespace tc

@@ -694,6 +694,17 @@ class Engine:
         self._check(rc, 'dqmc_debug_trunk')
         return out
 
+    TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'w1_mainloop', 'w2_mainloop',
+                    'mlp_epilogues', 'weight_wait', 'tile_layer_pairs')
+
+    def debug_trunk_phases(self):
+        """{phase: cycles} of the whole-trunk kernel's timers (engine created with DQMC_TRUNK_PHASES=1) since the last call;
+        'tile_layer_pairs' is a count.  Resets the counters."""
+        out = (C.c_uint64 * len(self.TRUNK_PHASES))()
+        rc = self.lib.dqmc_debug_trunk_phases(self.h, out, len(out))
+        self._check(rc, 'dqmc_debug_trunk_phases')
+        return dict(zip(self.TRUNK_PHASES, out))
+
     def profile_begin(self):
         self.lib.dqmc_profile_begin(self.h)
 

@@ -240,6 +240,12 @@ int dqmc_debug_mlp_block(dqmc_handle h, int32_t layer, const void* O, const void
  * reference: gnn/electron_gnn.py:403-432 (layer loop), gnn/update_features.py:241-286, hkext.py:22-137, :215-253. */
 int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, void* stream);
 
+/* Measurement aid: the phase timers of the whole-trunk kernel, summed over every launch since the last call, then reset.  On
+ * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 10.  out[0..9]: clock64()
+ * cycles of the consumer warpgroups in tile load, QKV mainloop, QKV epilogue, attention, Wo / W1 / W2 mainloops, MLP
+ * epilogues, waiting for weight slots (not part of the mainloops), then the number of (tile, layer) pairs processed. */
+int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n);
+
 /* Measurement aid (bench.py roofline): between begin/end every dense-layer GEMM launch is
  * bracketed by CUDA events on the caller's stream; end() returns their summed duration [ms],
  * the algorithmic flops they performed (2*M*N*K each) and their count.  No reference analogue
