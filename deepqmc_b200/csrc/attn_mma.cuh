@@ -97,8 +97,14 @@ __device__ __forceinline__ float am_ld1(const float* p) {
 //   valid(i, j)        key j takes part in the softmax of query row i (every row needs at least one)
 //   store(i, c, o0, o1) normalised output of query row i, head columns c, c + 1
 // kCoherent: plain global loads (rows written earlier by the same kernel) instead of the read-only path.
+// slot > 0 (NK8 = 2, keys = the task's own 16 rows, every key masked to the query rows of its own slot of `slot` rows): a masked
+// key's probability is an exact zero, but its V row still enters P V, and 0 x Inf = NaN, so one slot with a non-finite V row
+// (or one past the range of the scaled half split, |v| >= 65504 / 16) would make the outputs of every slot in the 16-row window
+// non-finite.  If any output of the task is non-finite, P V is therefore recomputed slot by slot with the V rows of the other
+// slots read as zeros: the other slots' outputs come out exactly as without the bad slot, the bad slot's stay non-finite.
 template <int NK8, bool kCoherent, class QRow, class KRow, class VRow, class Valid, class Store>
-__device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow, VRow vrow, Valid valid, Store store) {
+__device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow, VRow vrow, Valid valid, Store store,
+                                              int slot = 0) {
   constexpr int NK16 = (NK8 + 1) / 2;
   constexpr float kQS = 16.f, kPS = 1024.f;  // operand scales: q, k, v by 2^4, probabilities by 2^10
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
@@ -173,14 +179,16 @@ __device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow,
   }
   // ---- O[16 x 64] = P V: B fragment of dh tile nt: (k = key 16 kk + 2 t (+1, +8, +9), n = dh nt * 8 + g)
   const float uo0 = 1.f / (l0 * kPS * kQS), uo1 = 1.f / (l1 * kPS * kQS);
-#pragma unroll
-  for (int nt = 0; nt < 8; ++nt) {
-    float o[4] = {0.f, 0.f, 0.f, 0.f};
+  // dh tile nt of P V, V rows of the keys j with keep(j) (the others read as zeros)
+  auto pv = [&](int nt, float (&o)[4], auto keep) {
+    o[0] = o[1] = o[2] = o[3] = 0.f;
 #pragma unroll
     for (int kk = 0; kk < NK16; ++kk) {
       const int j = kk * 16 + 2 * t;
-      const float v00 = am_ld1<kCoherent>(vrow(j) + nt * 8 + g), v01 = am_ld1<kCoherent>(vrow(j + 1) + nt * 8 + g);
-      const float v10 = am_ld1<kCoherent>(vrow(j + 8) + nt * 8 + g), v11 = am_ld1<kCoherent>(vrow(j + 9) + nt * 8 + g);
+      const float v00 = keep(j) ? am_ld1<kCoherent>(vrow(j) + nt * 8 + g) : 0.f;
+      const float v01 = keep(j + 1) ? am_ld1<kCoherent>(vrow(j + 1) + nt * 8 + g) : 0.f;
+      const float v10 = keep(j + 8) ? am_ld1<kCoherent>(vrow(j + 8) + nt * 8 + g) : 0.f;
+      const float v11 = keep(j + 9) ? am_ld1<kCoherent>(vrow(j + 9) + nt * 8 + g) : 0.f;
       uint32_t vh[2], vl[2];
       am_split2(v00 * kQS, v01 * kQS, vh[0], vl[0]);
       am_split2(v10 * kQS, v11 * kQS, vh[1], vl[1]);
@@ -188,8 +196,34 @@ __device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow,
       mma16816(o, pl[kk], vh);
       mma16816(o, ph[kk], vh);
     }
-    store(0, nt * 8 + 2 * t, o[0] * uo0, o[1] * uo0);
-    store(1, nt * 8 + 2 * t, o[2] * uo1, o[3] * uo1);
+  };
+  int bad = 0;  // this lane stored a non-finite output (NaN fails the comparison)
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt) {
+    float o[4];
+    pv(nt, o, [](int) { return true; });
+    o[0] *= uo0; o[1] *= uo0; o[2] *= uo1; o[3] *= uo1;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) bad |= !(fabsf(o[e]) <= 3.4e38f);
+    store(0, nt * 8 + 2 * t, o[0], o[1]);
+    store(1, nt * 8 + 2 * t, o[2], o[3]);
+  }
+  if (slot > 0) {
+#pragma unroll
+    for (int m = 1; m < 32; m *= 2) bad |= __shfl_xor_sync(0xffffffffu, bad, m);
+  }
+  if (slot > 0 && bad) {
+    const int sm = ~(slot - 1);
+    for (int s0 = 0; s0 < 16; s0 += slot) {
+      const bool mine0 = (g & sm) == s0, mine1 = ((g + 8) & sm) == s0;
+#pragma unroll 1
+      for (int nt = 0; nt < 8; ++nt) {
+        float o[4];
+        pv(nt, o, [&](int j) { return (j & sm) == s0; });
+        if (mine0) store(0, nt * 8 + 2 * t, o[0] * uo0, o[1] * uo0);
+        if (mine1) store(1, nt * 8 + 2 * t, o[2] * uo1, o[3] * uo1);
+      }
+    }
   }
 }
 

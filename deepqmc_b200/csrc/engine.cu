@@ -74,6 +74,7 @@ struct EngineBase {
   virtual int stats_pack(const void* E, const void* stats, int B, double* out, cudaStream_t st) = 0;
   virtual int debug_mlp_block(int layer, const void* O, const void* X, void* Out, int rows, cudaStream_t st) = 0;
   virtual int debug_trunk(const void* X0, void* Out, int rows, cudaStream_t st) = 0;
+  virtual int debug_attention(int layer, const void* QKV, void* O, int rows, int32_t* kernel, cudaStream_t st) = 0;
   virtual int debug_trunk_phases(uint64_t* out, int n) = 0;
   virtual int forward(const void* r, const void* R, int Rb, int B, void* sign, void* logp, void* ws, int64_t wsb,
                       cudaStream_t st) = 0;
@@ -1080,6 +1081,16 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  int debug_attention(int layer, const void* QKV, void* O, int rows, int32_t* kernel, cudaStream_t st) override {
+    if (!(cfg.kind == DQMC_PSIFORMER || trans)) { err = "debug_attention: the configuration has no softmax attention layers"; return 2; }
+    if (layer < 0 || layer >= cfg.n_layers) { err = "debug_attention: layer out of range"; return 2; }
+    if (rows < 1 || rows % N != 0) { err = "debug_attention: rows must be a positive multiple of the electron count"; return 2; }
+    int rc = attention((const T*)QKV, (T*)O, rows / N, 1, layer, st, kernel);
+    if (rc) return rc;
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
   int debug_gemm(const char* wname, const char* bname, const void* A, const void* Res, void* C, int Mr, int S,
                  int sliced, int backend, cudaStream_t st) override {
     int64_t o = off(wname);
@@ -1314,6 +1325,89 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  // softmax attention of layer l on the Q | K | V rows [Bc N S][3d] -> O [Bc N S][d], with the kernel the configuration picks
+  // (TransPsiformer: plus the layer's nuclear key / value tokens); *kernel (if given) = that kernel, DQMC_ATTN_KERNEL_*
+  int attention(const T* QKV, T* O, int Bc, int S, int l, cudaStream_t st, int32_t* kernel = nullptr) {
+    int32_t which = DQMC_ATTN_KERNEL_GENERIC;
+    const std::string p = "L" + std::to_string(l) + ".";
+    const T scale = (T)(1.0 / std::sqrt((double)dh));
+    const int tb = S > 1 ? attn_tb : 1;
+    const T* kn = Mn > 0 ? P(p + "kn") : nullptr;
+    const T* vn = Mn > 0 ? P(p + "vn") : nullptr;
+    if constexpr (std::is_same<T, float>::value) {
+      if (S == 1 && attn_mma_ok) {
+        which = DQMC_ATTN_KERNEL_MMA;
+        // tensor-core attention: a warp per (walker, head, 16-query tile), fragments straight from global memory
+        const int n_pairs = Bc * H, tasks = n_pairs * ((N + 15) / 16);
+        int nblk = (tasks + 3) / 4;
+        if (nblk > n_sms * 8) nblk = n_sms * 8;
+        const dim3 grid(nblk), block(128);
+#define DQ_ATTN_MMA(NK_)                                                                                                     \
+  DQ_LAUNCH(attn_fwd_mma_kernel<NK_>, grid, block, 0, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d, (float)scale, \
+        n_pairs, (const float*)kn, (const float*)vn, Mn)
+        switch ((N + Mn + 7) / 8) {
+          case 1: DQ_ATTN_MMA(1); break;
+          case 2: DQ_ATTN_MMA(2); break;
+          case 3: DQ_ATTN_MMA(3); break;
+          case 4: DQ_ATTN_MMA(4); break;
+          case 5: DQ_ATTN_MMA(5); break;
+          default: DQ_ATTN_MMA(6); break;
+        }
+#undef DQ_ATTN_MMA
+      } else if (S == 1 && attn_fwd_ok && attn_fwd_pipelined) {
+        which = DQMC_ATTN_KERNEL_FWD2;
+        // persistent blocks (one per SM), 6 warps each, K / V of the next pair prefetched by cp.async
+        const int n_pairs = Bc * H, wpb = 6;
+        const int smem = wpb * 4 * N * 64 * (int)sizeof(float);
+        const int nblk = (n_pairs + wpb - 1) / wpb;
+        const dim3 grid(nblk < n_sms ? nblk : n_sms), block(32 * wpb);
+        if (N <= 8)
+          DQ_LAUNCH(attn_fwd2_f32_kernel<8>, grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d,
+                    (float)scale, n_pairs);
+        else if (N <= 16)
+          DQ_LAUNCH(attn_fwd2_f32_kernel<16>, grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d,
+                    (float)scale, n_pairs);
+        else
+          DQ_LAUNCH(attn_fwd2_f32_kernel<32>, grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d,
+                    (float)scale, n_pairs);
+      } else if (S == 1 && attn_fwd_ok) {
+        which = DQMC_ATTN_KERNEL_FWD;
+        const int n_pairs = Bc * H;
+        const int smem = 4 * 2 * (N + Mn) * 64 * (int)sizeof(float);
+        const dim3 grid((n_pairs + 3) / 4), block(128);
+#define DQ_ATTN_FWD(NM_, EX_)                                                                                          \
+  DQ_LAUNCH((attn_fwd_f32_kernel<NM_, EX_>), grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d, \
+        (float)scale, n_pairs, (const float*)kn, (const float*)vn, Mn)
+        switch (Mn > 0 ? -1 : N) {  // exact-size instances for the benchmark molecules, padded generic ones otherwise
+          case 4: DQ_ATTN_FWD(4, true); break;
+          case 10: DQ_ATTN_FWD(10, true); break;
+          case 14: DQ_ATTN_FWD(14, true); break;
+          case 28: DQ_ATTN_FWD(28, true); break;
+          case 30: DQ_ATTN_FWD(30, true); break;
+          default:
+            if (N + Mn <= 8) DQ_ATTN_FWD(8, false);
+            else if (N + Mn <= 16) DQ_ATTN_FWD(16, false);
+            else if (N + Mn <= 32) DQ_ATTN_FWD(32, false);
+            else DQ_ATTN_FWD(48, false);
+        }
+#undef DQ_ATTN_FWD
+      } else if (attn_f32) {
+        which = DQMC_ATTN_KERNEL_FL_F32;
+        if (launch_attn_f32((const float*)QKV, (float*)O, Bc, S, tb, (float)scale, 0,
+                            (int)attn_f32_smem_bytes(N, dh, tb), st, false))
+          return 1;
+      } else {
+        int rc = launch_attn_generic((const T*)QKV, O, Bc, S, tb, scale, kn, vn, st);
+        if (rc) return rc;
+      }
+    } else {
+      int rc = launch_attn_generic((const T*)QKV, O, Bc, S, tb, scale, kn, vn, st);
+      if (rc) return rc;
+    }
+    if (kernel) *kernel = which;
+    return 0;
+  }
+
   int run_chunk(const T* r, const T* R, int Rb, int Bc, int S, int Bstat, T* sign, T* logp, T* E, T* stats, T* grad,
                 void* wsbase, cudaStream_t st) {
     Ws w = carve(wsbase, Bc, S);
@@ -1360,7 +1454,6 @@ struct Engine : EngineBase {
     }
     T* X = w.X;
     T* O = w.O;
-    const T scale = (T)(1.0 / std::sqrt((double)dh));
     if (can_trunk(S)) {  // plain forward: every layer in one persistent tensor-core launch
       int rc = trunk_block(X, O, rows, st, compact ? ecp_emb : nullptr);
       if (rc) return rc;
@@ -1369,77 +1462,8 @@ struct Engine : EngineBase {
     for (int l = 0; l < cfg.n_layers; ++l) {
       std::string p = "L" + std::to_string(l) + ".";
       gemm(X, d, (p + "wqkv").c_str(), nullptr, 0, 3 * d, nullptr, nullptr, 0, w.QKV, 3 * d, rows, 3 * d, d, S, 0, N, st);
-      {
-        const int tb = S > 1 ? attn_tb : 1;
-        const T* kn = Mn > 0 ? P(p + "kn") : nullptr;
-        const T* vn = Mn > 0 ? P(p + "vn") : nullptr;
-        if constexpr (std::is_same<T, float>::value) {
-          if (S == 1 && attn_mma_ok) {
-            // tensor-core attention: a warp per (walker, head, 16-query tile), fragments straight from global memory
-            const int n_pairs = Bc * H, tasks = n_pairs * ((N + 15) / 16);
-            int nblk = (tasks + 3) / 4;
-            if (nblk > n_sms * 8) nblk = n_sms * 8;
-            const dim3 grid(nblk), block(128);
-#define DQ_ATTN_MMA(NK_)                                                                                                     \
-  DQ_LAUNCH(attn_fwd_mma_kernel<NK_>, grid, block, 0, st, (const float*)w.QKV, 3 * d, (float*)O, d, N, H, d, (float)scale, \
-            n_pairs, (const float*)kn, (const float*)vn, Mn)
-            switch ((N + Mn + 7) / 8) {
-              case 1: DQ_ATTN_MMA(1); break;
-              case 2: DQ_ATTN_MMA(2); break;
-              case 3: DQ_ATTN_MMA(3); break;
-              case 4: DQ_ATTN_MMA(4); break;
-              case 5: DQ_ATTN_MMA(5); break;
-              default: DQ_ATTN_MMA(6); break;
-            }
-#undef DQ_ATTN_MMA
-          } else if (S == 1 && attn_fwd_ok && attn_fwd_pipelined) {
-            // persistent blocks (one per SM), 6 warps each, K / V of the next pair prefetched by cp.async
-            const int n_pairs = Bc * H, wpb = 6;
-            const int smem = wpb * 4 * N * 64 * (int)sizeof(float);
-            const int nblk = (n_pairs + wpb - 1) / wpb;
-            const dim3 grid(nblk < n_sms ? nblk : n_sms), block(32 * wpb);
-            if (N <= 8)
-              DQ_LAUNCH(attn_fwd2_f32_kernel<8>, grid, block, smem, st, (const float*)w.QKV, 3 * d, (float*)O, d, N, H, d,
-                        (float)scale, n_pairs);
-            else if (N <= 16)
-              DQ_LAUNCH(attn_fwd2_f32_kernel<16>, grid, block, smem, st, (const float*)w.QKV, 3 * d, (float*)O, d, N, H, d,
-                        (float)scale, n_pairs);
-            else
-              DQ_LAUNCH(attn_fwd2_f32_kernel<32>, grid, block, smem, st, (const float*)w.QKV, 3 * d, (float*)O, d, N, H, d,
-                        (float)scale, n_pairs);
-          } else if (S == 1 && attn_fwd_ok) {
-            const int n_pairs = Bc * H;
-            const int smem = 4 * 2 * (N + Mn) * 64 * (int)sizeof(float);
-            const dim3 grid((n_pairs + 3) / 4), block(128);
-#define DQ_ATTN_FWD(NM_, EX_)                                                                                          \
-  DQ_LAUNCH((attn_fwd_f32_kernel<NM_, EX_>), grid, block, smem, st, (const float*)w.QKV, 3 * d, (float*)O, d, N, H, d, \
-            (float)scale, n_pairs, (const float*)kn, (const float*)vn, Mn)
-            switch (Mn > 0 ? -1 : N) {  // exact-size instances for the benchmark molecules, padded generic ones otherwise
-              case 4: DQ_ATTN_FWD(4, true); break;
-              case 10: DQ_ATTN_FWD(10, true); break;
-              case 14: DQ_ATTN_FWD(14, true); break;
-              case 28: DQ_ATTN_FWD(28, true); break;
-              case 30: DQ_ATTN_FWD(30, true); break;
-              default:
-                if (N + Mn <= 8) DQ_ATTN_FWD(8, false);
-                else if (N + Mn <= 16) DQ_ATTN_FWD(16, false);
-                else if (N + Mn <= 32) DQ_ATTN_FWD(32, false);
-                else DQ_ATTN_FWD(48, false);
-            }
-#undef DQ_ATTN_FWD
-          } else if (attn_f32) {
-            if (launch_attn_f32((const float*)w.QKV, (float*)O, Bc, S, tb, (float)scale, 0,
-                                (int)attn_f32_smem_bytes(N, dh, tb), st, false))
-              return 1;
-          } else {
-            int rc = launch_attn_generic((const T*)w.QKV, O, Bc, S, tb, scale, kn, vn, st);
-            if (rc) return rc;
-          }
-        } else {
-          int rc = launch_attn_generic((const T*)w.QKV, O, Bc, S, tb, scale, kn, vn, st);
-          if (rc) return rc;
-        }
-      }
+      int rc = attention(w.QKV, O, Bc, S, l, st);
+      if (rc) return rc;
       if (can_fuse_mlp(S, p)) {
         // plain forward: attention projection + residual and both MLP layers in ONE launch, result in place of O
         int rc = mlp_block(p, O, X, O, rows, st);
@@ -2530,6 +2554,12 @@ int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, voi
   if (!h) return 2;
   DQ_NEED_DEVICE(h);
   return h->e->debug_trunk(X0, Out, rows, (cudaStream_t)stream);
+}
+int dqmc_debug_attention(dqmc_handle h, int32_t layer, const void* QKV, void* O, int32_t rows, int32_t* kernel, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!QKV || !O) { h->e->err = "dqmc_debug_attention: null array"; return 2; }
+  return h->e->debug_attention(layer, QKV, O, rows, kernel, (cudaStream_t)stream);
 }
 int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n) {
   if (!h) return 2;

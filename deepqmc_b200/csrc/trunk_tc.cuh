@@ -18,7 +18,8 @@
 // (shared with attn_fwd_mma_kernel) for each head, with Q, K and V read straight from the scratch (plain, coherent loads: the
 // rows were written by this kernel) and O_h written, scaled and split, into k-block h of the operand buffer (dead once the
 // QKV GEMMs have retired).  The keys of a task are its walker slot (NP = 32: 4 key tiles of 8) or, for slots of at most 16
-// rows, the task's own 16 rows masked to the query's slot (2 key tiles).  Padding rows (electron >= N) get no attention
+// rows, the task's own 16 rows masked to the query's slot (2 key tiles; a walker whose V rows are non-finite cannot turn the
+// other walkers of the window non-finite, see attn_task_mma's slot argument).  Padding rows (electron >= N) get no attention
 // output: their operand rows keep the finite previous operand and are never stored.
 #pragma once
 #include <cstdint>
@@ -155,7 +156,7 @@ trunk_f16_kernel(TrunkParams p) {
           if ((r & (NP - 1)) < N) store_operand_pair(smem, r, 64 * h + c, o0 * p.a_scale, o1 * p.a_scale);
         };
         if (NP > 16) attn_task_mma<4, true>(p.attn_scale, qrow, krow, vrow, valid, store);
-        else attn_task_mma<2, true>(p.attn_scale, qrow, krow, vrow, valid, store);
+        else attn_task_mma<2, true>(p.attn_scale, qrow, krow, vrow, valid, store, NP < 16 ? NP : 0);
       }
       fence_proxy_async();
       __syncthreads();

@@ -410,7 +410,7 @@ class Engine:
             self.entries[name.value.decode()] = (off.value, rows.value, cols.value)
         self.n_packed = self.lib.dqmc_param_total(h)
         self._ws = None
-        self._ws_ok = set()  # (n_walkers, mode, cap) requests the current workspace is known to satisfy
+        self._ws_ok = {}  # (n_walkers, mode, cap) -> the workspace (view) that serves that request
         self._params_version = None
         self._nuc_R_dev = None
 
@@ -449,10 +449,12 @@ class Engine:
     def workspace(self, n_walkers: int, mode: int, max_bytes: int | None = None):
         """The engine's scratch buffer for one call of the entry point ``mode`` names: dqmc_workspace_bytes (a dry pass of the
         code that carves it), capped at ``max_bytes`` / 60 % of the free HBM -- the engine then chunks the walkers -- but
-        never below dqmc_workspace_bytes_min."""
+        never below dqmc_workspace_bytes_min.  An explicit ``max_bytes`` also caps the view handed to the call when a larger
+        buffer is already held, so the engine chunks exactly as that size makes it."""
         key = (n_walkers, mode, max_bytes)
         if self._ws is not None and key in self._ws_ok:  # hot path: no driver queries per call
-            return self._ws
+            return self._ws_ok[key]
+        explicit = max_bytes is not None
         need = self.lib.dqmc_workspace_bytes(self.h, n_walkers, mode)
         if max_bytes is None and not self._host:
             free = torch.cuda.mem_get_info(self.device)[0] + (self._ws.numel() if self._ws is not None else 0)
@@ -462,9 +464,9 @@ class Engine:
         if self._ws is None or self._ws.numel() < need:
             self._ws = None
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-            self._ws_ok = set()
-        self._ws_ok.add(key)
-        return self._ws
+            self._ws_ok = {}
+        self._ws_ok[key] = self._ws[:need] if explicit else self._ws
+        return self._ws_ok[key]
 
     def _prep(self, x):
         x = torch.as_tensor(x, dtype=self.dtype, device=self.device)
@@ -689,10 +691,27 @@ class Engine:
     def debug_trunk(self, X0):
         """One launch of the whole-trunk kernel: all attention layers applied to the embedding rows -> [rows, d] (self-test hook)."""
         X0 = self._prep(X0)
+        assert X0.dim() == 2 and X0.shape[1] == self.spec.embedding_dim and X0.shape[0] % self.spec.n_elec == 0, tuple(X0.shape)
         out = torch.empty_like(X0)
         rc = self.lib.dqmc_debug_trunk(self.h, X0.data_ptr(), out.data_ptr(), X0.shape[0], self._stream())
         self._check(rc, 'dqmc_debug_trunk')
         return out
+
+    ATTN_KERNELS = ('attn_fwd_mma_kernel', 'attn_fwd2_f32_kernel', 'attn_fwd_f32_kernel', 'attn_fl_f32_kernel', 'attn_fl_kernel')
+
+    def debug_attention(self, layer, QKV):
+        """The plain-forward softmax attention of `layer` (the kernel the engine picks) on Q | K | V rows [rows, 3d]
+        -> (O [rows, d], name of the kernel that ran); the TransPsiformer's nuclear tokens come from the parameter table
+        (self-test hook)."""
+        QKV = self._prep(QKV)
+        d = self.spec.embedding_dim
+        assert QKV.dim() == 2 and QKV.shape[1] == 3 * d and QKV.shape[0] % self.spec.n_elec == 0, tuple(QKV.shape)
+        out = torch.empty(QKV.shape[0], d, dtype=self.dtype, device=self.device)
+        kernel = C.c_int32(-1)
+        rc = self.lib.dqmc_debug_attention(self.h, layer, QKV.data_ptr(), out.data_ptr(), QKV.shape[0], C.byref(kernel),
+                                           self._stream())
+        self._check(rc, 'dqmc_debug_attention')
+        return out, self.ATTN_KERNELS[kernel.value]
 
     TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'w1_mainloop', 'w2_mainloop',
                     'mlp_epilogues', 'weight_wait', 'tile_layer_pairs')

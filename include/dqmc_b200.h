@@ -240,6 +240,22 @@ int dqmc_debug_mlp_block(dqmc_handle h, int32_t layer, const void* O, const void
  * reference: gnn/electron_gnn.py:403-432 (layer loop), gnn/update_features.py:241-286, hkext.py:22-137, :215-253. */
 int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, void* stream);
 
+/* Self-test hook: the softmax attention of layer `layer` in a plain forward (S = 1), run by the kernel the engine picks for it
+ * (fp32, dh = 64, N + nuclear tokens <= 48: the tensor-core attn_fwd_mma_kernel), on caller-supplied rows QKV [rows][3d]
+ * (Q | K | V, head h in columns h dh .. h dh + dh - 1 of each; rows = walkers x electrons, walker-major) -> O [rows][d].
+ * TransPsiformer: the keys and values also hold the layer's nuclear tokens from the parameter table (L<layer>.kn / .vn).
+ * *kernel (if not null) receives the kernel that ran, one of DQMC_ATTN_KERNEL_*.
+ * Status 2 for kinds without softmax attention, a layer out of range, or rows not a multiple of the electron count.
+ * reference: gnn/update_features.py:273-280 (hk.MultiHeadAttention), algebra hkext.py:215-253. */
+enum {
+  DQMC_ATTN_KERNEL_MMA = 0,     /* attn_fwd_mma_kernel: 3xFP16 mma.sync, fp32 dh = 64, N + nuclear tokens <= 48 */
+  DQMC_ATTN_KERNEL_FWD2 = 1,    /* attn_fwd2_f32_kernel: persistent SIMT plain forward (DQMC_ATTN_FWD2) */
+  DQMC_ATTN_KERNEL_FWD = 2,     /* attn_fwd_f32_kernel: SIMT plain forward, block per walker */
+  DQMC_ATTN_KERNEL_FL_F32 = 3,  /* attn_fl_f32_kernel: fp32 forward-Laplacian attention (plain forward: no tangents) */
+  DQMC_ATTN_KERNEL_GENERIC = 4  /* attn_fl_kernel: generic, any dtype */
+};
+int dqmc_debug_attention(dqmc_handle h, int32_t layer, const void* QKV, void* O, int32_t rows, int32_t* kernel, void* stream);
+
 /* Measurement aid: the phase timers of the whole-trunk kernel, summed over every launch since the last call, then reset.  On
  * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 10.  out[0..9]: clock64()
  * cycles of the consumer warpgroups in tile load, QKV mainloop, QKV epilogue, attention, Wo / W1 / W2 mainloops, MLP

@@ -11,6 +11,7 @@ from deepqmc_b200.ansatz import B200Ansatz
 from deepqmc_b200.hamil import MolecularHamiltonian
 from deepqmc_b200.molecule import Molecule
 from deepqmc_b200.types import PhysicalConfiguration
+from tc_reference import trunk_ref as _trunk_ref
 
 DEV = 'cuda:0'
 
@@ -173,32 +174,10 @@ def test_plain_forward_half_operands_vs_3xtf32(monkeypatch):
     ref = A.double() @ Wq
     assert ((C.double() - ref).abs() / (A.double().abs() @ Wq.abs())).max().item() < 2e-6
 
-def _trunk_ref(eng, X0, N, L, H=4, dtype=torch.float64):
-    """The layers of gnn/update_features.py:241-286 (hk.MultiHeadAttention + hkext.py MLP / residuals) in torch."""
-    flat = torch.as_tensor(eng._flat, device=DEV)
-
-    def W(name):
-        off, K, Nc = eng.entries[name]
-        return flat[off:off + K * Nc].reshape(K, Nc).float().to(dtype)
-
-    X = X0.to(dtype)
-    rows, d = X.shape
-    B, dh = rows // N, d // H
-    for l in range(L):
-        p = f'L{l}.'
-        q, k, v = ((t.reshape(B, N, H, dh).permute(0, 2, 1, 3)) for t in (X @ W(p + 'wqkv')).split(d, dim=1))
-        att = torch.softmax(q @ k.transpose(-1, -2) / dh ** 0.5, dim=-1)
-        O = (att @ v).permute(0, 2, 1, 3).reshape(rows, d)
-        A = X + O @ W(p + 'wo')
-        M1 = torch.tanh(A @ W(p + 'w1') + W(p + 'b1')[0])
-        X = A + torch.tanh(M1 @ W(p + 'w2') + W(p + 'b2')[0])
-    return X
-
-
 @pytest.mark.parametrize('mol,walkers', [('LiH', 3), ('LiH', 32 * 148 * 2 + 5), ('benzene', 9), ('benzene', 4 * 148 * 3 + 1)])
 def test_fused_trunk_matches_fp64(mol, walkers):
     """ONE launch of the whole-trunk kernel (trunk_tc.cuh: all four attention layers of a plain forward, residual stream in
-    per-CTA scratch, operands in shared memory, Q / K / V through the per-CTA scratch, fp32 attention) against an fp64
+    per-CTA scratch, operands in shared memory, Q / K / V through the per-CTA scratch, 3xFP16 tensor-core attention) against an fp64
     restatement of the layers and against the same restatement in plain fp32: partial tiles, padding rows (benzene: 120 of
     128 tile rows), several tiles per CTA (barrier phases wrap)."""
     hamil = MolecularHamiltonian(mol=Molecule.from_name(mol), ecp_type='ccECP' if mol == 'benzene' else None)

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """Where the whole-trunk kernel's time goes: phase timers of `tc::trunk_f16_kernel` at the production tile shape.
 
-  python tools/trunk_phases.py OUT_DIR [--walkers 16384] [--launches 20]
+  python tools/trunk_phases.py OUT_DIR [--mol benzene|LiH] [--walkers 16384] [--launches 20]
 
 Builds the benzene / ccECP Psiformer engine (fp32, tensor-core backend; N = 30 electrons, walker slot 32, 4 walkers per
-128-row tile) and runs the trunk alone (dqmc_debug_trunk) on random embedding rows.  Two engines: one without timers for the
+128-row tile) or the LiH one (N = 4, walker slot 4, 32 walkers per tile) and runs the trunk alone (dqmc_debug_trunk) on random embedding rows.  Two engines: one without timers for the
 kernel time (CUDA events over --launches launches after a warm-up), one created with DQMC_TRUNK_PHASES=1 for the phase shares.
-Prints and writes OUT_DIR/trunk_phases.json: us per (tile, layer) per SM, algorithmic TFLOP/s (counted as the engine's
+Prints and writes OUT_DIR/trunk_phases_<mol>.json: us per (tile, layer) per SM, algorithmic TFLOP/s (counted as the engine's
 profiler counts the trunk class: 2 rows (6 d^2 + 2 N d) per layer), each phase's share of the consumer warpgroups' cycles,
 and the card's name, power limit and SM clocks (read-only nvidia-smi query).
 """
@@ -47,6 +47,7 @@ def engine(hamil, params, phases):
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument('out_dir')
+    ap.add_argument('--mol', choices=('benzene', 'LiH'), default='benzene')
     ap.add_argument('--walkers', type=int, default=16384)
     ap.add_argument('--launches', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=3)
@@ -54,7 +55,7 @@ def main():
     assert a.walkers >= 16384 and a.launches >= 20, 'production shape: >= 16384 walkers, >= 20 timed launches'
     assert torch.cuda.is_available(), 'the trunk phase timers need a GPU'
     torch.cuda.set_device(0)
-    hamil = MolecularHamiltonian(mol=Molecule.from_name('benzene'), ecp_type='ccECP')
+    hamil = MolecularHamiltonian(mol=Molecule.from_name(a.mol), ecp_type='ccECP' if a.mol == 'benzene' else None)
     params = PN.perturb_params(B200Ansatz(hamil, 'psiformer', dtype='float32', gemm_backend=1).init(0))
     N, d, L = hamil.n_up + hamil.n_down, 256, 4
     g = torch.Generator(device='cpu').manual_seed(0)
@@ -89,12 +90,12 @@ def main():
     flops = L * 2.0 * a.walkers * N * (6 * d * d + 2 * N * d)
     total = sum(ph.values())
     res = dict(
-        kernel='tc::trunk_f16_kernel', mol='benzene', ecp='ccECP', walkers=a.walkers, N=N, slot=np2, walkers_per_tile=128 // np2,
+        kernel='tc::trunk_f16_kernel', mol=a.mol, ecp=hamil.ecp_type, walkers=a.walkers, N=N, slot=np2, walkers_per_tile=128 // np2,
         launches=a.launches, grid=grid, ms_per_launch=ms, us_per_tile_layer=ms * 1e3 * grid / pairs,
         algorithmic_tflops=flops / (ms * 1e-3) / 1e12, phase_share={k: v / total for k, v in ph.items()},
         phase_cycles={k: int(v) for k, v in ph.items()}, card=card())
     os.makedirs(a.out_dir, exist_ok=True)
-    with open(os.path.join(a.out_dir, 'trunk_phases.json'), 'w') as f:
+    with open(os.path.join(a.out_dir, f'trunk_phases_{a.mol}.json'), 'w') as f:
         json.dump(res, f, indent=1)
     print(f"{res['card']['name']}, power limit {res['card']['power.limit']}, SM clock {res['card']['clocks.sm']} "
           f"(max {res['card']['clocks.max.sm']})")
