@@ -74,7 +74,9 @@ struct EngineBase {
   virtual int stats_pack(const void* E, const void* stats, int B, double* out, cudaStream_t st) = 0;
   virtual int debug_mlp_block(int layer, const void* O, const void* X, void* Out, int rows, cudaStream_t st) = 0;
   virtual int debug_trunk(const void* X0, void* Out, int rows, cudaStream_t st) = 0;
-  virtual int debug_attention(int layer, const void* QKV, void* O, int rows, int32_t* kernel, cudaStream_t st) = 0;
+  virtual int debug_attention(int layer, const void* QKV, void* O, int rows, int S, int32_t* kernel, cudaStream_t st) = 0;
+  virtual int debug_mlp(int layer, int S, const void* O, const void* X, void* Out, void* scratch, int rows, int32_t* path,
+                        cudaStream_t st) = 0;
   virtual int debug_trunk_phases(uint64_t* out, int n) = 0;
   virtual int forward(const void* r, const void* R, int Rb, int B, void* sign, void* logp, void* ws, int64_t wsb,
                       cudaStream_t st) = 0;
@@ -329,6 +331,7 @@ struct Engine : EngineBase {
   bool attn_fl_mma = false;   // fp32 forward-Laplacian attention: tangent chunks as warp-level 3xTF32 mma.sync products
   int attn_fl_threads = 128;  // block size of the fp32 forward-Laplacian attention (large molecules: one block per SM fits -> more warps)
   bool attn_f32 = false;
+  bool gemm_ran_tc = false;   // the last gemm() call ran the tensor-core kernel (not the CUDA-core gemm_kernel)
   bool embed_fwd_ok = false;
   bool attn_fwd_ok = false;
   bool attn_fwd_pipelined = false;
@@ -888,9 +891,11 @@ struct Engine : EngineBase {
     if (dry) return 0;  // planning pass
     const T* W0 = P(w0);
     const T* W1 = w1 ? P(w1) : nullptr;
+    gemm_ran_tc = false;
 #if !defined(DQMC_NO_TCGEN05)
     if constexpr (std::is_same<T, float>::value) {
       if (use_tc() && !bias1 && Kc % 32 == 0 && lda % 4 == 0 && ldc % 4 == 0 && tcw.count(w0) && (!w1 || tcw.count(w1))) {
+        gemm_ran_tc = true;
         const TcWeight& t0 = tcw.at(w0);
         const TcWeight& t1 = w1 ? tcw.at(w1) : t0;
         tc::Params p;
@@ -1081,11 +1086,27 @@ struct Engine : EngineBase {
     return 0;
   }
 
-  int debug_attention(int layer, const void* QKV, void* O, int rows, int32_t* kernel, cudaStream_t st) override {
+  int debug_attention(int layer, const void* QKV, void* O, int rows, int S, int32_t* kernel, cudaStream_t st) override {
     if (!(cfg.kind == DQMC_PSIFORMER || trans)) { err = "debug_attention: the configuration has no softmax attention layers"; return 2; }
     if (layer < 0 || layer >= cfg.n_layers) { err = "debug_attention: layer out of range"; return 2; }
-    if (rows < 1 || rows % N != 0) { err = "debug_attention: rows must be a positive multiple of the electron count"; return 2; }
-    int rc = attention((const T*)QKV, (T*)O, rows / N, 1, layer, st, kernel);
+    // the tangent chunk and the shared memory of the forward-Laplacian kernels were sized for T3 = 3N at creation
+    if (S != 1 && S != T3 + 2) { err = "debug_attention: S must be 1 or 3N + 2"; return 2; }
+    if (rows < 1 || rows % (N * S) != 0) { err = "debug_attention: rows must be a positive multiple of N S"; return 2; }
+    int rc = attention((const T*)QKV, (T*)O, rows / (N * S), S, layer, st, kernel);
+    if (rc) return rc;
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
+  int debug_mlp(int layer, int S, const void* O, const void* X, void* Out, void* scratch, int rows, int32_t* path,
+                cudaStream_t st) override {
+    if (!(cfg.kind == DQMC_PSIFORMER || trans)) { err = "debug_mlp: the configuration has no attention layers"; return 2; }
+    if (layer < 0 || layer >= cfg.n_layers) { err = "debug_mlp: layer out of range"; return 2; }
+    if (S != 1 && S != T3 + 2) { err = "debug_mlp: S must be 1 or 3N + 2"; return 2; }
+    if (rows < 1 || rows % (N * S) != 0) { err = "debug_mlp: rows must be a positive multiple of N S"; return 2; }
+    T* A = (T*)scratch;
+    int rc = mlp("L" + std::to_string(layer) + ".", (const T*)O, (const T*)X, (T*)Out, A, A + (size_t)rows * d, rows / (N * S), S,
+                 st, path);
     if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
     return 0;
@@ -1392,11 +1413,12 @@ struct Engine : EngineBase {
         }
 #undef DQ_ATTN_FWD
       } else if (attn_f32) {
-        which = DQMC_ATTN_KERNEL_FL_F32;
+        which = attn_fl_mma && S > 1 ? DQMC_ATTN_KERNEL_FL_F32_MMA : DQMC_ATTN_KERNEL_FL_F32;
         if (launch_attn_f32((const float*)QKV, (float*)O, Bc, S, tb, (float)scale, 0,
                             (int)attn_f32_smem_bytes(N, dh, tb), st, false))
           return 1;
       } else {
+        if (attn_gen_mma && S > 1) which = DQMC_ATTN_KERNEL_GENERIC_MMA;
         int rc = launch_attn_generic((const T*)QKV, O, Bc, S, tb, scale, kn, vn, st);
         if (rc) return rc;
       }
@@ -1405,6 +1427,37 @@ struct Engine : EngineBase {
       if (rc) return rc;
     }
     if (kernel) *kernel = which;
+    return 0;
+  }
+
+  // what follows the attention of a layer, on [Bc N S] slot rows: A = X + O Wo; M1 = tanh(A W1 + b1); Out = A + tanh(M1 W2 + b2),
+  // with the forward-Laplacian propagation of the tanh for S > 1.  A / M1: [Bc N S][d] scratch (unused by the fused block);
+  // Out may alias O.  *path (if given) = the path that ran, DQMC_MLP_PATH_*
+  int mlp(const std::string& p, const T* O, const T* X, T* Out, T* A, T* M1, int Bc, int S, cudaStream_t st,
+          int32_t* path = nullptr) {
+    const int rows = Bc * N * S;
+    int32_t which;
+    if (can_fuse_mlp(S, p)) {
+      // plain forward: attention projection + residual and both MLP layers in ONE launch
+      which = DQMC_MLP_PATH_BLOCK;
+      int rc = mlp_block(p, O, X, Out, rows, st);
+      if (rc) return rc;
+    } else {
+      gemm(O, d, (p + "wo").c_str(), nullptr, 0, d, nullptr, X, d, A, d, rows, d, d, S, 0, N, st);
+      if (can_fuse_act(S)) {
+        // MLP with the tanh (and its Jacobian/Laplacian propagation) inside the GEMM epilogues
+        which = DQMC_MLP_PATH_GEMM_ACT;
+        gemm(A, d, (p + "w1").c_str(), nullptr, 0, d, P(p + "b1"), nullptr, 0, M1, d, rows, d, d, S, 0, N, st, 1);
+        gemm(M1, d, (p + "w2").c_str(), nullptr, 0, d, P(p + "b2"), A, d, Out, d, rows, d, d, S, 0, N, st, 1);
+      } else {
+        gemm(A, d, (p + "w1").c_str(), nullptr, 0, d, P(p + "b1"), nullptr, 0, M1, d, rows, d, d, S, 0, N, st);
+        which = gemm_ran_tc ? DQMC_MLP_PATH_GEMM_TANH : DQMC_MLP_PATH_SIMT_TANH;
+        DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, (d + 127) / 128), dim3(128), 0, st, M1, d, (const T*)nullptr, 0, S, d, T(1));
+        gemm(M1, d, (p + "w2").c_str(), nullptr, 0, d, P(p + "b2"), nullptr, 0, Out, d, rows, d, d, S, 0, N, st);
+        DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, (d + 127) / 128), dim3(128), 0, st, Out, d, (const T*)A, d, S, d, T(1));
+      }
+    }
+    if (path) *path = which;
     return 0;
   }
 
@@ -1464,25 +1517,8 @@ struct Engine : EngineBase {
       gemm(X, d, (p + "wqkv").c_str(), nullptr, 0, 3 * d, nullptr, nullptr, 0, w.QKV, 3 * d, rows, 3 * d, d, S, 0, N, st);
       int rc = attention(w.QKV, O, Bc, S, l, st);
       if (rc) return rc;
-      if (can_fuse_mlp(S, p)) {
-        // plain forward: attention projection + residual and both MLP layers in ONE launch, result in place of O
-        int rc = mlp_block(p, O, X, O, rows, st);
-        if (rc) return rc;
-        T* tmp = X; X = O; O = tmp;
-        continue;
-      }
-      gemm(O, d, (p + "wo").c_str(), nullptr, 0, d, nullptr, X, d, w.A, d, rows, d, d, S, 0, N, st);
-      if (can_fuse_act(S)) {
-        // MLP with the tanh (and its Jacobian/Laplacian propagation) inside the GEMM epilogues
-        gemm(w.A, d, (p + "w1").c_str(), nullptr, 0, d, P(p + "b1"), nullptr, 0, w.M1, d, rows, d, d, S, 0, N, st, 1);
-        gemm(w.M1, d, (p + "w2").c_str(), nullptr, 0, d, P(p + "b2"), w.A, d, O, d, rows, d, d, S, 0, N, st, 1);
-      } else {
-        gemm(w.A, d, (p + "w1").c_str(), nullptr, 0, d, P(p + "b1"), nullptr, 0, w.M1, d, rows, d, d, S, 0, N, st);
-        DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, (d + 127) / 128), dim3(128), 0, st, w.M1, d, (const T*)nullptr, 0, S, d,
-                  T(1));
-        gemm(w.M1, d, (p + "w2").c_str(), nullptr, 0, d, P(p + "b2"), nullptr, 0, O, d, rows, d, d, S, 0, N, st);
-        DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, (d + 127) / 128), dim3(128), 0, st, O, d, (const T*)w.A, d, S, d, T(1));
-      }
+      rc = mlp(p, O, X, O, w.A, w.M1, Bc, S, st);
+      if (rc) return rc;
       T* tmp = X; X = O; O = tmp;
     }
     return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, X, st, nullptr, qa);
@@ -2555,11 +2591,19 @@ int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, voi
   DQ_NEED_DEVICE(h);
   return h->e->debug_trunk(X0, Out, rows, (cudaStream_t)stream);
 }
-int dqmc_debug_attention(dqmc_handle h, int32_t layer, const void* QKV, void* O, int32_t rows, int32_t* kernel, void* stream) {
+int dqmc_debug_attention(dqmc_handle h, int32_t layer, const void* QKV, void* O, int32_t rows, int32_t S, int32_t* kernel,
+                         void* stream) {
   if (!h) return 2;
   DQ_NEED_DEVICE(h);
   if (!QKV || !O) { h->e->err = "dqmc_debug_attention: null array"; return 2; }
-  return h->e->debug_attention(layer, QKV, O, rows, kernel, (cudaStream_t)stream);
+  return h->e->debug_attention(layer, QKV, O, rows, S, kernel, (cudaStream_t)stream);
+}
+int dqmc_debug_mlp(dqmc_handle h, int32_t layer, int32_t S, const void* O, const void* X, void* Out, void* scratch, int32_t rows,
+                   int32_t* path, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!O || !X || !Out || !scratch) { h->e->err = "dqmc_debug_mlp: null array"; return 2; }
+  return h->e->debug_mlp(layer, S, O, X, Out, scratch, rows, path, (cudaStream_t)stream);
 }
 int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n) {
   if (!h) return 2;

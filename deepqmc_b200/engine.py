@@ -697,21 +697,39 @@ class Engine:
         self._check(rc, 'dqmc_debug_trunk')
         return out
 
-    ATTN_KERNELS = ('attn_fwd_mma_kernel', 'attn_fwd2_f32_kernel', 'attn_fwd_f32_kernel', 'attn_fl_f32_kernel', 'attn_fl_kernel')
+    ATTN_KERNELS = ('attn_fwd_mma_kernel', 'attn_fwd2_f32_kernel', 'attn_fwd_f32_kernel', 'attn_fl_f32_kernel', 'attn_fl_kernel',
+                    'attn_fl_f32_kernel_mma', 'attn_fl_kernel_mma')
 
-    def debug_attention(self, layer, QKV):
-        """The plain-forward softmax attention of `layer` (the kernel the engine picks) on Q | K | V rows [rows, 3d]
-        -> (O [rows, d], name of the kernel that ran); the TransPsiformer's nuclear tokens come from the parameter table
-        (self-test hook)."""
+    def debug_attention(self, layer, QKV, S=1):
+        """The softmax attention of `layer` (the kernel the engine picks) on Q | K | V rows [rows, 3d] with S slots per electron
+        (1: plain forward; 3N + 2: value, 3N tangents, Laplacian; row (b N + i) S + s) -> (O [rows, d], name of the kernel that
+        ran); the TransPsiformer's nuclear tokens come from the parameter table (self-test hook)."""
         QKV = self._prep(QKV)
         d = self.spec.embedding_dim
-        assert QKV.dim() == 2 and QKV.shape[1] == 3 * d and QKV.shape[0] % self.spec.n_elec == 0, tuple(QKV.shape)
+        assert QKV.dim() == 2 and QKV.shape[1] == 3 * d and QKV.shape[0] % (self.spec.n_elec * S) == 0, tuple(QKV.shape)
         out = torch.empty(QKV.shape[0], d, dtype=self.dtype, device=self.device)
         kernel = C.c_int32(-1)
-        rc = self.lib.dqmc_debug_attention(self.h, layer, QKV.data_ptr(), out.data_ptr(), QKV.shape[0], C.byref(kernel),
+        rc = self.lib.dqmc_debug_attention(self.h, layer, QKV.data_ptr(), out.data_ptr(), QKV.shape[0], S, C.byref(kernel),
                                            self._stream())
         self._check(rc, 'dqmc_debug_attention')
         return out, self.ATTN_KERNELS[kernel.value]
+
+    MLP_PATHS = ('mlp_block', 'gemm_fused_tanh', 'gemm_tanh_fl_kernel', 'simt_gemm_tanh_fl_kernel')
+
+    def debug_mlp(self, layer, O, X, S=1):
+        """What follows the attention of `layer` on slot rows O, X [rows, d] (layout of debug_attention):
+        Out = A + tanh(tanh(A W1 + b1) W2 + b2), A = X + O Wo, with forward-Laplacian propagation for S > 1
+        -> (Out [rows, d], name of the path that ran) (self-test hook)."""
+        O, X = self._prep(O), self._prep(X)
+        d = self.spec.embedding_dim
+        assert O.shape == X.shape and O.dim() == 2 and O.shape[1] == d and O.shape[0] % (self.spec.n_elec * S) == 0, tuple(O.shape)
+        out = torch.empty_like(O)
+        scratch = torch.empty(2 * O.shape[0], d, dtype=self.dtype, device=self.device)
+        path = C.c_int32(-1)
+        rc = self.lib.dqmc_debug_mlp(self.h, layer, S, O.data_ptr(), X.data_ptr(), out.data_ptr(), scratch.data_ptr(), O.shape[0],
+                                     C.byref(path), self._stream())
+        self._check(rc, 'dqmc_debug_mlp')
+        return out, self.MLP_PATHS[path.value]
 
     TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'w1_mainloop', 'w2_mainloop',
                     'mlp_epilogues', 'weight_wait', 'tile_layer_pairs')

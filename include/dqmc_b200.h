@@ -240,21 +240,44 @@ int dqmc_debug_mlp_block(dqmc_handle h, int32_t layer, const void* O, const void
  * reference: gnn/electron_gnn.py:403-432 (layer loop), gnn/update_features.py:241-286, hkext.py:22-137, :215-253. */
 int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, void* stream);
 
-/* Self-test hook: the softmax attention of layer `layer` in a plain forward (S = 1), run by the kernel the engine picks for it
- * (fp32, dh = 64, N + nuclear tokens <= 48: the tensor-core attn_fwd_mma_kernel), on caller-supplied rows QKV [rows][3d]
- * (Q | K | V, head h in columns h dh .. h dh + dh - 1 of each; rows = walkers x electrons, walker-major) -> O [rows][d].
+/* Self-test hook: the softmax attention of layer `layer` with S slots per electron, run by the kernel the engine picks for it
+ * (the same Engine::attention the forward calls), on caller-supplied rows QKV [rows][3d] (Q | K | V, head h in columns
+ * h dh .. h dh + dh - 1 of each) -> O [rows][d].  rows = walkers x electrons x S in the engine's slot layout: row
+ * (b N + i) S + s holds slot s of electron i of walker b.  S = 1: plain forward (fp32, dh = 64, N + nuclear tokens <= 48: the
+ * tensor-core attn_fwd_mma_kernel).  S = 3N + 2: forward-Laplacian pass, slot 0 the value, slots 1 .. 3N the tangents, slot
+ * 3N + 1 the Laplacian (the tangent chunk and the shared memory were sized for this S when the engine was created).
  * TransPsiformer: the keys and values also hold the layer's nuclear tokens from the parameter table (L<layer>.kn / .vn).
  * *kernel (if not null) receives the kernel that ran, one of DQMC_ATTN_KERNEL_*.
- * Status 2 for kinds without softmax attention, a layer out of range, or rows not a multiple of the electron count.
- * reference: gnn/update_features.py:273-280 (hk.MultiHeadAttention), algebra hkext.py:215-253. */
+ * Status 2 for kinds without softmax attention, a layer out of range, S other than 1 or 3N + 2, or rows not a multiple of N S.
+ * reference: gnn/update_features.py:273-280 (hk.MultiHeadAttention), algebra hkext.py:215-253; derivative rules
+ * folxext.py:70-171. */
 enum {
   DQMC_ATTN_KERNEL_MMA = 0,     /* attn_fwd_mma_kernel: 3xFP16 mma.sync, fp32 dh = 64, N + nuclear tokens <= 48 */
   DQMC_ATTN_KERNEL_FWD2 = 1,    /* attn_fwd2_f32_kernel: persistent SIMT plain forward (DQMC_ATTN_FWD2) */
   DQMC_ATTN_KERNEL_FWD = 2,     /* attn_fwd_f32_kernel: SIMT plain forward, block per walker */
-  DQMC_ATTN_KERNEL_FL_F32 = 3,  /* attn_fl_f32_kernel: fp32 forward-Laplacian attention (plain forward: no tangents) */
-  DQMC_ATTN_KERNEL_GENERIC = 4  /* attn_fl_kernel: generic, any dtype */
+  DQMC_ATTN_KERNEL_FL_F32 = 3,  /* attn_fl_f32_kernel<., ., false>: fp32 forward-Laplacian attention, SIMT tangent chunks */
+  DQMC_ATTN_KERNEL_GENERIC = 4, /* attn_fl_kernel<T, false>: generic, any dtype, SIMT */
+  DQMC_ATTN_KERNEL_FL_F32_MMA = 5,  /* attn_fl_f32_kernel<., ., true>: tangent chunks as 3xTF32 mma.sync products */
+  DQMC_ATTN_KERNEL_GENERIC_MMA = 6  /* attn_fl_kernel<float, true>: generic fp32 kernel, tangent chunks on the tensor cores */
 };
-int dqmc_debug_attention(dqmc_handle h, int32_t layer, const void* QKV, void* O, int32_t rows, int32_t* kernel, void* stream);
+int dqmc_debug_attention(dqmc_handle h, int32_t layer, const void* QKV, void* O, int32_t rows, int32_t S, int32_t* kernel,
+                         void* stream);
+
+/* Self-test hook: what follows the attention in layer `layer`, with S slots per electron (1 or 3N + 2, rows in the layout of
+ * dqmc_debug_attention), run by the same Engine::mlp the forward calls:  A = X + O Wo;  M1 = tanh(A W1 + b1);
+ * Out = A + tanh(M1 W2 + b2), the tanh with its forward-Laplacian propagation for S > 1 (y_t = y' z_t,
+ * y_L = y' z_L + y'' sum_t z_t^2).  O / X / Out [rows][d] device arrays; scratch: 2 rows d elements (A and M1).
+ * *path (if not null) receives the path that ran, one of DQMC_MLP_PATH_*.
+ * Status 2 for kinds without attention layers, a layer out of range, S other than 1 or 3N + 2, or rows not a multiple of N S.
+ * reference: gnn/update_features.py:241-286, hkext.py:22-137 (MLP), :104-113 (activation). */
+enum {
+  DQMC_MLP_PATH_BLOCK = 0,      /* plain forward: one fused MLP-block launch (fused_tc.cuh) */
+  DQMC_MLP_PATH_GEMM_ACT = 1,   /* 3xTF32 row GEMMs, tanh (+ forward-Laplacian rule) in the W1 / W2 epilogues */
+  DQMC_MLP_PATH_GEMM_TANH = 2,  /* 3xTF32 row GEMMs, tanh_fl_kernel after W1 and W2 */
+  DQMC_MLP_PATH_SIMT_TANH = 3   /* CUDA-core gemm_kernel, tanh_fl_kernel after W1 and W2 */
+};
+int dqmc_debug_mlp(dqmc_handle h, int32_t layer, int32_t S, const void* O, const void* X, void* Out, void* scratch, int32_t rows,
+                   int32_t* path, void* stream);
 
 /* Measurement aid: the phase timers of the whole-trunk kernel, summed over every launch since the last call, then reset.  On
  * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 10.  out[0..9]: clock64()
