@@ -356,9 +356,10 @@ struct Engine : EngineBase {
   struct TcWeight {
     float* hi = nullptr; float* lo = nullptr; CUtensorMap mh, ml; int N = 0, K = 0;
     // "3xFP16" operands of the plain-forward kernels: (W 2^e)^T as halves, hi / lo planes [N][K]; maps with BN-row boxes
-    // (row GEMM) and with all-N-row boxes (fused MLP block, N <= 256)
+    // (row GEMM) and with all-N-row boxes of 32 halves (64-byte swizzle: the per-warpgroup weight slots of the fused MLP
+    // block, N <= 256, fused_tc.cuh)
     uint16_t* h16 = nullptr; CUtensorMap m16h, m16l, m16h_all, m16l_all; float wscale = 1.f; bool f16 = false, f16_all = false;
-    CUtensorMap m16h_256, m16l_256; bool f16_256 = false;  // 256-row boxes: weight slots of the whole-trunk kernel (trunk_tc.cuh)
+    CUtensorMap m16h_256, m16l_256; bool f16_256 = false;  // 256-row boxes of 32 halves: weight slots of the whole-trunk kernel (trunk_tc.cuh)
   };
   bool fuse_trunk = true;  // all layers of a plain forward in one persistent launch (trunk_tc.cuh); DQMC_TC_TRUNK=0 disables
   CUtensorMap* d_trunk_maps = nullptr;       // [L][4][2]
@@ -388,14 +389,14 @@ struct Engine : EngineBase {
         }
         w.f16 = true;
         if (Nc <= 256 && Nc % 16 == 0) {
-          if (tc::make_kmajor_map(&w.m16h_all, w.h16, 2, Nc, Kc, 64, Nc) || tc::make_kmajor_map(&w.m16l_all, lo16, 2, Nc, Kc, 64, Nc)) {
+          if (tc::make_kmajor_map(&w.m16h_all, w.h16, 2, Nc, Kc, 32, Nc) || tc::make_kmajor_map(&w.m16l_all, lo16, 2, Nc, Kc, 32, Nc)) {
             err = "cuTensorMapEncodeTiled (whole-N half planes) failed for " + name;
             return 4;
           }
           w.f16_all = true;
         }
         if (Kc == 256 && Nc % 256 == 0 &&
-            !tc::make_kmajor_map(&w.m16h_256, w.h16, 2, Nc, Kc, 64, 256) && !tc::make_kmajor_map(&w.m16l_256, lo16, 2, Nc, Kc, 64, 256))
+            !tc::make_kmajor_map(&w.m16h_256, w.h16, 2, Nc, Kc, 32, 256) && !tc::make_kmajor_map(&w.m16l_256, lo16, 2, Nc, Kc, 32, 256))
           w.f16_256 = true;
       }
     }

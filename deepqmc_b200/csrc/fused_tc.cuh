@@ -13,9 +13,15 @@
 // (the accumulator of the next GEMM already fills the register file).
 //
 // 256 threads = two warpgroups; warpgroup w computes tile rows 64 w .. +63 over all d columns (wgmma m64 n = d, fp32
-// accumulators in registers).  Thread 0 streams the pre-split weight planes [d rows x 64 halves] (hi, lo per k-block) of
-// Wo, W1, W2 through a 3-slot ring (TMA): the planes of the next two k-steps land while the current one is multiplied.
-// shared memory: operand buffer 4 k-blocks x {hi, lo} x 16 KB = 128 KB, weight ring 3 x 32 KB, biases, barriers (226 KB).
+// accumulators in registers) and owns those rows from the tile load to the output: its half of the operand buffer, its
+// residual rows, its weight ring.  The two warpgroups never wait for each other except for the MMA token (ping-pong): each
+// runs its own copy of the layer, and one warpgroup's epilogues (and the trunk's attention) run while the other's MMAs
+// keep the tensor cores busy.  Thread 0 of a warpgroup streams the pre-split weight half-planes [d rows x 32 halves] (hi,
+// lo per k-block, two halves each) of the GEMM through the warpgroup's 3-slot ring (TMA, 64-byte swizzle): the slots of the
+// next two k-steps land while the current one is multiplied.  A warpgroup takes the token before the first MMA of a GEMM
+// (of the trunk's whole QKV projection: its three column blocks have epilogues much shorter than a GEMM) and hands it to
+// the other after issuing the last one, so the two warpgroups' GEMMs alternate on the tensor cores.
+// shared memory: operand buffer 4 k-blocks x {hi, lo} x 16 KB = 128 KB, weight rings 2 x 3 x 16 KB, barriers (224 KB).
 #pragma once
 #include <cstdint>
 
@@ -25,12 +31,12 @@ namespace dq {
 namespace tc {
 
 constexpr int kMlpThreads = 256;
-constexpr int kMlpSlots = 3;  // weight ring: a slot is refilled 3 slots ahead, i.e. under the MMAs of the next two
+constexpr int kMlpSlots = 3;  // weight ring of a warpgroup: a slot is refilled 3 slots ahead, i.e. under the MMAs of the next two
 
 struct MlpParams {
   const float* O; int ldo;     // attention output rows [M][d]
   const float* X; int ldx;     // residual stream rows [M][d]
-  float* Out; int ldout;       // X' rows [M][d]; may alias O (a tile reads its O rows before it writes them)
+  float* Out; int ldout;       // X' rows [M][d]; may alias O (a warpgroup reads its O rows before it writes them)
   const float* b1; const float* b2;
   int M, d;
   float a_scale;               // power of two applied to every activation operand before the hi / lo split
@@ -40,16 +46,32 @@ struct MlpParams {
 
 struct MlpSmem {
   static __host__ __device__ int abuf(int kb, int plane) { return (kb * 2 + plane) * 16384; }   // [128 rows][128 B]
-  static __host__ __device__ int wring(int s) { return 131072 + s * 32768; }                      // [<= 256 rows][128 B]
-  static __host__ __device__ int bias() { return 131072 + kMlpSlots * 32768; }                    // b1[256], b2[256]
-  static __host__ __device__ int bars() { return bias() + 2048; }
-  static __host__ __device__ int phases() { return bars() + 64; }                                 // [2][kPhases] u64
+  static __host__ __device__ int wring(int wg, int s) { return 131072 + (wg * kMlpSlots + s) * 16384; }  // [<= 256 rows][64 B]
+  static __host__ __device__ int bars() { return 131072 + 2 * kMlpSlots * 16384; }  // full [2][kMlpSlots], token [2]
+  static __host__ __device__ int phases() { return bars() + 64; }                                 // [2][16] u64
   static __host__ __device__ int total() { return phases() + 2 * 8 * 16; }
 };
+// mbarriers: slot s of warpgroup wg's ring landed (TMA tx); the MMA token of warpgroup wg (arrived by the other one)
+__device__ __forceinline__ uint64_t* ring_full(unsigned char* smem, int wg) {
+  return (uint64_t*)(smem + MlpSmem::bars()) + wg * kMlpSlots;
+}
+__device__ __forceinline__ uint64_t* mma_token(unsigned char* smem, int wg) {
+  return (uint64_t*)(smem + MlpSmem::bars()) + 2 * kMlpSlots + wg;
+}
+// Kernel prologue (thread 0 with the CTA barrier after it): the barriers of both rings and both tokens.
+__device__ __forceinline__ void init_rings(unsigned char* smem) {
+  for (int i = 0; i < 2 * kMlpSlots + 2; ++i) mbar_init((uint64_t*)(smem + MlpSmem::bars()) + i, 1);
+  fence_barrier_init();
+}
+// After that CTA barrier: warpgroup 0 holds the token for the first GEMM.
+__device__ __forceinline__ void start_pingpong(unsigned char* smem) {
+  if (threadIdx.x == 128) mbar_arrive(mma_token(smem, 0));
+}
 
 // Phase timers of the whole-trunk kernel (TrunkParams::phase): clock64() cycles summed over the consumer warpgroups of all
-// CTAs, in this order; kPhWait is the time spent waiting for weight slots to land and is not part of the mainloop phases.
-enum Phase { kPhLoad, kPhQkv, kPhQkvEpi, kPhAttn, kPhWo, kPhW1, kPhW2, kPhMlpEpi, kPhWait, kPhPairs, kPhases };
+// CTAs, in this order; kPhWait (waiting for weight slots to land) and kPhTurn (waiting for the other warpgroup to hand over
+// the MMA token) are not part of the mainloop phases.
+enum Phase { kPhLoad, kPhQkv, kPhQkvEpi, kPhAttn, kPhWo, kPhW1, kPhW2, kPhMlpEpi, kPhWait, kPhTurn, kPhPairs, kPhases };
 static_assert(kPhases <= 16, "MlpSmem::phases() holds 16 counters per warpgroup");
 struct PhaseClock {
   unsigned long long* acc;  // this warpgroup's shared-memory counters on its timing thread, nullptr: not timing
@@ -66,9 +88,9 @@ struct PhaseClock {
     }
   }
   __device__ __forceinline__ void count(int k) { if (acc) acc[k] += 1; }
-  // w cycles of weight wait inside the current phase: booked to kPhWait instead
-  __device__ __forceinline__ void waited(long long w) {
-    acc[kPhWait] += (unsigned long long)w;
+  // w cycles of waiting inside the current phase: booked to phase k (kPhWait, kPhTurn) instead
+  __device__ __forceinline__ void waited(long long w, int k) {
+    acc[k] += (unsigned long long)w;
     t += w;
   }
 };
@@ -116,69 +138,102 @@ __device__ __forceinline__ void store_operand_quad(unsigned char* smem, int row,
   *(uint2*)(smem + MlpSmem::abuf(kb, 1) + off) = make_uint2(l01, l23);
 }
 
-// acc = (operand buffer, K = D) x (rows y0 .. y0 + D - 1 of W^T), hi / lo planes through the 3-slot weight ring.  Called by all
-// 256 threads with the operand buffer complete (fenced + __syncthreads); returns with every MMA retired and the ring free.
-// `nslot` counts the ring slots used so far: slot g lives in ring stage g % 3 and completes phase (g / 3) & 1 of its barrier.
+// Per-warpgroup pipeline state: ring slots used so far (slot g lives in ring stage g % 3 and completes phase (g / 3) & 1 of
+// its barrier) and MMA tokens taken so far (token u completes phase u & 1 of the warpgroup's token barrier).
+struct Ring {
+  uint32_t nslot = 0, nturn = 0;
+};
+// What a GEMM does with the MMA token: take it before its first MMA, pass it to the other warpgroup after its last.  A run of
+// GEMMs with short epilogues in between (the three column blocks of the QKV projection) holds the token throughout.
+enum Turn { kTurnTake = 1, kTurnPass = 2, kTurnOwn = kTurnTake | kTurnPass, kTurnKeep = 0 };
+
+// acc = (this warpgroup's 64 operand rows, K = D) x (rows y0 .. y0 + D - 1 of W^T), hi / lo half-planes through the
+// warpgroup's 3-slot weight ring.  Called by the 128 threads of a warpgroup with its operand rows complete (fenced +
+// wg_sync); returns with every MMA retired and the ring free.
+//
+// The MMAs run in the same order as with whole 64-half planes (per k-block: lo A x hi W and hi A x hi W for k-steps 0 .. 3,
+// then hi A x lo W for k-steps 0 .. 3), so every output element sums the same products in the same order.
 template <int D>
-__device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* smem, uint64_t* full, uint32_t& nslot,
-                                          const CUtensorMap* mh, const CUtensorMap* ml, int y0, int* err, PhaseClock& pc) {
+__device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const CUtensorMap* mh,
+                                          const CUtensorMap* ml, int y0, int turn, int* err, PhaseClock& pc) {
+  uint32_t& nslot = ring.nslot;
   constexpr int KB = D / 64;
-  constexpr int NS = 2 * KB;  // slots of this GEMM: slot i = plane i % 2 (hi, lo) of k-block i / 2
+  constexpr int NS = 4 * KB;  // slots of this GEMM: slot i = k-steps 2 (i % 2) .. +1 of plane (i / 2) % 2 (hi, lo) of k-block i / 4
   static_assert(NS >= kMlpSlots, "the ring is filled at the start of a GEMM");
-  constexpr uint32_t kSlot = D * 128u;
-  const int tid = threadIdx.x, wg = tid >> 7;
+  constexpr uint32_t kSlot = D * 64u;
+  const int wg = threadIdx.x >> 7;
+  const bool leader = (threadIdx.x & 127) == 0;
+  uint64_t* full = ring_full(smem, wg);
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) acc[i] = 0.f;  // the previous contents are dead: registers free between GEMMs
   auto stage = [&](int i) { return (int)((nslot + (uint32_t)i) % (uint32_t)kMlpSlots); };
   auto load = [&](int i) {
     const int st = stage(i);
     mbar_expect_tx(&full[st], kSlot);
-    tma_load_2d((i & 1) ? ml : mh, &full[st], smem + MlpSmem::wring(st), (i >> 1) * 64, y0);
+    tma_load_2d(((i >> 1) & 1) ? ml : mh, &full[st], smem + MlpSmem::wring(wg, st), (i >> 2) * 64 + (i & 1) * 32, y0);
   };
-  if (tid == 0)
+  if (leader)
     for (int i = 0; i < kMlpSlots; ++i) load(i);
+  // the first slots land while this warpgroup waits for the token
+  if (turn & kTurnTake) {
+    const long long t0 = pc.acc ? clock64() : 0;
+    mbar_wait(mma_token(smem, wg), ring.nturn & 1u, err);
+    ++ring.nturn;
+    if (pc.acc) pc.waited(clock64() - t0, kPhTurn);
+  }
   // waits for slot i and returns its shared-memory address
   auto acquire = [&](int i) {
     const int st = stage(i);
     const long long t0 = pc.acc ? clock64() : 0;
     mbar_wait(&full[st], ((nslot + (uint32_t)i) / (uint32_t)kMlpSlots) & 1u, err);
-    if (pc.acc) pc.waited(clock64() - t0);
-    return smem_u32(smem + MlpSmem::wring(st));
+    if (pc.acc) pc.waited(clock64() - t0, kPhWait);
+    return smem_u32(smem + MlpSmem::wring(wg, st));
   };
-  // slot i retired by both warpgroups -> its stage takes slot i + 3
-  auto release = [&](int i) {
-    __syncthreads();
-    if (tid == 0 && i + kMlpSlots < NS) load(i + kMlpSlots);
+  // slot i's MMAs were just committed: once the previous slot's have retired in every warp of the warpgroup, its stage takes
+  // slot i + 2
+  auto retire = [&](int i) {
+    wgmma_wait1();
+    if (i == 0) return;
+    wg_sync(wg);
+    if (leader && i + kMlpSlots - 1 < NS) load(i + kMlpSlots - 1);
   };
   auto mma = [&](float (&d)[D / 2], uint32_t a, uint32_t w, int accumulate) {
-    if constexpr (D == 256) wgmma_f16_n256(d, make_desc(a), make_desc(w), accumulate);
-    else wgmma_f16_n128(d, make_desc(a), make_desc(w), accumulate);
+    if constexpr (D == 256) wgmma_f16_n256(d, make_desc(a), make_desc64(w), accumulate);
+    else wgmma_f16_n128(d, make_desc(a), make_desc64(w), accumulate);
   };
-  // The MMAs of one slot are straight-line code (no branch between them): control flow between wgmmas that share the
-  // accumulator makes the compiler fence every instruction.
+  // The MMAs of one slot are straight-line code; between slots nothing touches the accumulator, so the wgmmas of one GEMM
+  // stay in flight back to back.
 #pragma unroll 1
   for (int kb = 0; kb < KB; ++kb) {
     const uint32_t ah = smem_u32(smem + MlpSmem::abuf(kb, 0)) + wg * 8192, al = smem_u32(smem + MlpSmem::abuf(kb, 1)) + wg * 8192;
-    const uint32_t whi = acquire(2 * kb);
-    wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {  // 16 halves = 32 bytes per instruction
-      mma(acc, al + 32 * k, whi + 32 * k, (kb | k) ? 1 : 0);
-      mma(acc, ah + 32 * k, whi + 32 * k, 1);
+    for (int q = 0; q < 2; ++q) {  // hi plane, k-steps 2 q, 2 q + 1 (16 halves = 32 bytes per instruction)
+      const uint32_t w = acquire(4 * kb + q);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) {
+        const int k = 2 * q + kk;
+        mma(acc, al + 32 * k, w + 32 * kk, (kb | k) ? 1 : 0);
+        mma(acc, ah + 32 * k, w + 32 * kk, 1);
+      }
+      wgmma_commit();
+      retire(4 * kb + q);
     }
-    wgmma_commit();
-    wgmma_wait0();
-    fence_acc(acc);
-    release(2 * kb);
-    const uint32_t wlo = acquire(2 * kb + 1);
-    wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k) mma(acc, ah + 32 * k, wlo + 32 * k, 1);
-    wgmma_commit();
-    wgmma_wait0();
-    fence_acc(acc);
-    release(2 * kb + 1);
+    for (int q = 0; q < 2; ++q) {  // lo plane
+      const uint32_t w = acquire(4 * kb + 2 + q);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) mma(acc, ah + 32 * (2 * q + kk), w + 32 * kk, 1);
+      wgmma_commit();
+      retire(4 * kb + 2 + q);
+    }
   }
+  // every MMA of the GEMM is issued: the other warpgroup's GEMM queues behind them
+  if ((turn & kTurnPass) && leader) mbar_arrive(mma_token(smem, wg ^ 1));
+  wgmma_wait0();
+  fence_acc(acc);
+  wg_sync(wg);  // the last slots are retired in every warp: the next GEMM may refill their stages
   nslot += NS;
 }
 
@@ -192,22 +247,24 @@ struct Frag {
   }
 };
 
-// The three GEMMs of the MLP block with their epilogues, operand buffer holding O (scaled, split) on entry.  Per fragment row
-// h (tile rows fr, fr + 8): xin[h] residual X (nullptr: zero), aout[h] where A is parked (nullptr: row not stored), xout[h]
-// where X' goes (nullptr: not stored); operand_out: X' also becomes the operand buffer (next layer of the trunk).
+// The three GEMMs of the MLP block with their epilogues, run by one warpgroup on its 64 rows, its operand rows holding O
+// (scaled, split) on entry.  Per fragment row h (tile rows fr, fr + 8): xin[h] residual X (nullptr: zero), aout[h] where A is
+// parked (nullptr: row not stored), xout[h] where X' goes (nullptr: not stored); operand_out: X' also becomes the operand
+// rows (next layer of the trunk).  b1, b2: the biases in global memory (read through the read-only cache).
 template <int D>
-__device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, uint64_t* full, uint32_t& nslot,
-                                     const CUtensorMap* wo_hi, const CUtensorMap* wo_lo, const CUtensorMap* w1_hi,
-                                     const CUtensorMap* w1_lo, const CUtensorMap* w2_hi, const CUtensorMap* w2_lo, float us0,
-                                     float us1, float us2, float a_scale, const float* sb1, const float* sb2,
-                                     const float* const (&xin)[2], float* const (&aout)[2], float* const (&xout)[2],
-                                     bool operand_out, int* err, PhaseClock& pc) {
+__device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const CUtensorMap* wo_hi,
+                                     const CUtensorMap* wo_lo, const CUtensorMap* w1_hi, const CUtensorMap* w1_lo,
+                                     const CUtensorMap* w2_hi, const CUtensorMap* w2_lo, float us0, float us1, float us2,
+                                     float a_scale, const float* b1, const float* b2, const float* const (&xin)[2],
+                                     float* const (&aout)[2], float* const (&xout)[2], bool operand_out, int* err,
+                                     PhaseClock& pc) {
   const Frag f;
+  const int wg = threadIdx.x >> 7;
   // Row loads are issued in batches of kJ fragment columns ahead of the stores: xin / aout / xout may alias, so the compiler
   // would otherwise wait for every load behind the previous store.
   constexpr int kJ = 4;
   // ---- A = X + O Wo -> parked rows and the operand buffer
-  gemm_abuf<D>(acc, smem, full, nslot, wo_hi, wo_lo, 0, err, pc);
+  gemm_abuf<D>(acc, smem, ring, wo_hi, wo_lo, 0, kTurnOwn, err, pc);
   pc.mark(kPhWo);
 #pragma unroll
   for (int jb = 0; jb < D / 8; jb += kJ) {
@@ -227,24 +284,26 @@ __device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, u
       }
   }
   fence_proxy_async();
-  __syncthreads();
+  wg_sync(wg);
   pc.mark(kPhMlpEpi);
   // ---- M1 = tanh(A W1 + b1) -> operand buffer
-  gemm_abuf<D>(acc, smem, full, nslot, w1_hi, w1_lo, 0, err, pc);
+  gemm_abuf<D>(acc, smem, ring, w1_hi, w1_lo, 0, kTurnOwn, err, pc);
   pc.mark(kPhW1);
 #pragma unroll
-  for (int j = 0; j < D / 8; ++j)
+  for (int j = 0; j < D / 8; ++j) {
+    const int c = 8 * j + f.fc;
+    const float2 b = make_float2(__ldg(b1 + c), __ldg(b1 + c + 1));  // (the parameter table gives no 8-byte alignment)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int c = 8 * j + f.fc;
-      const float m0 = mlp_tanh(acc[4 * j + 2 * h] * us1 + sb1[c]), m1 = mlp_tanh(acc[4 * j + 2 * h + 1] * us1 + sb1[c + 1]);
+      const float m0 = mlp_tanh(acc[4 * j + 2 * h] * us1 + b.x), m1 = mlp_tanh(acc[4 * j + 2 * h + 1] * us1 + b.y);
       store_operand_pair(smem, f.fr + 8 * h, c, m0 * a_scale, m1 * a_scale);
     }
+  }
   fence_proxy_async();
-  __syncthreads();
+  wg_sync(wg);
   pc.mark(kPhMlpEpi);
   // ---- X' = A + tanh(M1 W2 + b2)
-  gemm_abuf<D>(acc, smem, full, nslot, w2_hi, w2_lo, 0, err, pc);
+  gemm_abuf<D>(acc, smem, ring, w2_hi, w2_lo, 0, kTurnOwn, err, pc);
   pc.mark(kPhW2);
 #pragma unroll
   for (int jb = 0; jb < D / 8; jb += kJ) {
@@ -259,8 +318,9 @@ __device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, u
       for (int h = 0; h < 2; ++h) {
         const int c = 8 * (jb + j) + f.fc;
         if (!aout[h]) continue;
-        const float x0 = a[j][h].x + mlp_tanh(acc[4 * (jb + j) + 2 * h] * us2 + sb2[c]);
-        const float x1 = a[j][h].y + mlp_tanh(acc[4 * (jb + j) + 2 * h + 1] * us2 + sb2[c + 1]);
+        const float2 b = make_float2(__ldg(b2 + c), __ldg(b2 + c + 1));
+        const float x0 = a[j][h].x + mlp_tanh(acc[4 * (jb + j) + 2 * h] * us2 + b.x);
+        const float x1 = a[j][h].y + mlp_tanh(acc[4 * (jb + j) + 2 * h + 1] * us2 + b.y);
         if (xout[h]) *(float2*)(xout[h] + c) = make_float2(x0, x1);
         if (operand_out) store_operand_pair(smem, f.fr + 8 * h, c, x0 * a_scale, x1 * a_scale);
       }
@@ -275,31 +335,26 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
                      const __grid_constant__ CUtensorMap w2_hi, const __grid_constant__ CUtensorMap w2_lo, MlpParams p) {
   DQMC_TC_SMEM(smem);
   if ((smem_u32(smem) & 1023u) != 0u) tc_trap();
-  uint64_t* full = (uint64_t*)(smem + MlpSmem::bars());  // [kMlpSlots] weight slot landed (TMA tx)
-  float* sb1 = (float*)(smem + MlpSmem::bias());
-  float* sb2 = sb1 + 256;
-  const int tid = threadIdx.x;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int MT = (p.M + 127) / 128;
 
   if (tid == 0) {
-    for (int i = 0; i < kMlpSlots; ++i) mbar_init(&full[i], 1);
-    fence_barrier_init();
+    init_rings(smem);
     tma_prefetch_desc(&wo_hi); tma_prefetch_desc(&wo_lo); tma_prefetch_desc(&w1_hi);
     tma_prefetch_desc(&w1_lo); tma_prefetch_desc(&w2_hi); tma_prefetch_desc(&w2_lo);
   }
-  for (int i = tid; i < D; i += blockDim.x) {
-    sb1[i] = p.b1[i];
-    sb2[i] = p.b2[i];
-  }
   __syncthreads();
+  start_pingpong(smem);
   const Frag f;
-  uint32_t nslot = 0;
+  Ring ring;
   float acc[D / 2];
   PhaseClock pc(nullptr);
+  // Both warpgroups run every tile of the CTA (a warpgroup without valid rows computes on zeros and stores nothing), so
+  // they take the MMA token equally often.
   for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
-    // ---- stage the O tile: coalesced float4 loads, hi / lo split
-    for (int idx = tid; idx < 128 * (D / 4); idx += kMlpThreads) {
-      const int r = idx / (D / 4), c = 4 * (idx % (D / 4));
+    // ---- stage this warpgroup's 64 rows of the O tile: coalesced float4 loads, hi / lo split
+    for (int idx = tid & 127; idx < 64 * (D / 4); idx += 128) {
+      const int r = 64 * wg + idx / (D / 4), c = 4 * (idx % (D / 4));
       const int grow = tile * 128 + r;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (grow < p.M) v = __ldg((const float4*)(p.O + (size_t)grow * p.ldo + c));
@@ -307,7 +362,7 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
       store_operand_quad(smem, r, c, make_float4(v.x * sc, v.y * sc, v.z * sc, v.w * sc));
     }
     fence_proxy_async();
-    __syncthreads();  // also: every O row of the tile has been read before A is parked in the (possibly aliasing) Out rows
+    wg_sync(wg);  // also: every O row of the warpgroup has been read before A is parked in the (possibly aliasing) Out rows
     const float* xin[2];
     float* aout[2];
 #pragma unroll
@@ -317,7 +372,7 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
       xin[h] = valid ? p.X + (size_t)grow * p.ldx : nullptr;
       aout[h] = valid ? p.Out + (size_t)grow * p.ldout : nullptr;
     }
-    mlp3<D>(acc, smem, full, nslot, &wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo, p.us0, p.us1, p.us2, p.a_scale, sb1, sb2,
+    mlp3<D>(acc, smem, ring, &wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo, p.us0, p.us1, p.us2, p.a_scale, p.b1, p.b2,
             xin, aout, aout, false, p.err_flag, pc);
   }
 }

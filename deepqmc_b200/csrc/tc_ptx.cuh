@@ -40,6 +40,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* e
     }
   }
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// barrier of the 128 threads of one warpgroup (named barrier id = 1 + warpgroup; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
@@ -64,6 +69,16 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   d |= (uint64_t)1 << 62;
   return d;
 }
+// The same for a SWIZZLE_64B operand (rows of 64 B = 32 halves): SBO = 512 B (8 rows of 64 B), layout SWIZZLE_64B (2).  A
+// k-step of 16 halves advances the start address by 32 B.
+__device__ __forceinline__ uint64_t make_desc64(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512 >> 4) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
 
 // Warpgroup MMA, both operands K-major in shared memory, fp32 accumulators in registers: d (+)= A B^T for a 64-row slice
 // (the warpgroup's) of A and N rows of B.  acc = 0 overwrites d.  Accumulator fragment of thread t of the warpgroup:
@@ -71,6 +86,7 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 // the accumulator registers are read only after the wait: keeps the compiler from moving their uses above it
 template <int R>
 __device__ __forceinline__ void fence_acc(float (&d)[R]) {
@@ -179,7 +195,7 @@ __device__ __forceinline__ float tf32_rna(float x) {
 }
 
 // ---- host side: tensor maps of K-major operand matrices [rows][K] (K contiguous), box = box_k x box_rows elements with the
-// inner extent box_k * elem_bytes = 128 bytes, 128-byte swizzle ---------------------------------------------------------
+// inner extent box_k * elem_bytes = 128 bytes (128-byte swizzle) or 64 bytes (64-byte swizzle) ----------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -197,13 +213,15 @@ inline EncodeTiledFn get_encode_fn() {
 inline int make_kmajor_map(CUtensorMap* map, const void* base, int elem_bytes, int rows, int K, int box_k, int box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return 1;
-  if (box_k * elem_bytes != 128 || (elem_bytes != 4 && elem_bytes != 2)) return 3;
+  const int inner = box_k * elem_bytes;
+  if ((inner != 128 && inner != 64) || (elem_bytes != 4 && elem_bytes != 2)) return 3;
   cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
   cuuint64_t gstr[1] = {(cuuint64_t)K * (cuuint64_t)elem_bytes};
   cuuint32_t box[2] = {(cuuint32_t)box_k, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, gdim,
-                  gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  inner == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : 2;
 }

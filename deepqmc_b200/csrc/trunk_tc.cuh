@@ -44,7 +44,7 @@ struct TrunkParams {
   long long v0; int vper;        //   [base][N][256]; walker w of this launch is virtual walker v0 + w = base (v0 + w) / vper
                                  //   with electron ((v0 + w) / 12) % N moved (ecp_points_kernel layout)
   float* Out; int ldout;         // trunk output rows [rows][256]
-  const CUtensorMap* maps;       // device array [L][4][2]: (Wqkv, Wo, W1, W2) x (hi, lo); boxes of 64 halves x 256 rows
+  const CUtensorMap* maps;       // device array [L][4][2]: (Wqkv, Wo, W1, W2) x (hi, lo); boxes of 32 halves x 256 rows
   const float* b1[kTrMaxLayers];
   const float* b2[kTrMaxLayers];
   float us[kTrMaxLayers][4];     // accumulator unscale of the four GEMMs of a layer: 1 / (a_scale * weight scale)
@@ -60,11 +60,8 @@ __global__ void __launch_bounds__(kTrThreads, 1)
 trunk_f16_kernel(TrunkParams p) {
   DQMC_TC_SMEM(smem);
   if ((smem_u32(smem) & 1023u) != 0u) tc_trap();
-  uint64_t* full = (uint64_t*)(smem + TrSmem::bars());
-  float* sb1 = (float*)(smem + TrSmem::bias());
-  float* sb2 = sb1 + 256;
 
-  const int tid = threadIdx.x;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int N = p.N, NP = p.NP, L = p.L;
   const int lnp = 31 - __clz(NP);                // NP is a power of two
   const int G = 128 / NP;                        // walker slots per tile
@@ -73,32 +70,37 @@ trunk_f16_kernel(TrunkParams p) {
   float* resid = qkv + 128 * 768;                                            // [128][256]
 
   if (tid == 0) {
-    for (int i = 0; i < kMlpSlots; ++i) mbar_init(&full[i], 1);
-    fence_barrier_init();
+    init_rings(smem);
     for (int i = 0; i < 8 * L; ++i) tma_prefetch_desc(p.maps + i);
   }
   unsigned long long* ph = (unsigned long long*)(smem + TrSmem::phases());
   if (tid < 32) ph[tid] = 0ull;
   __syncthreads();
-  PhaseClock pc(p.phase && (tid & 127) == 0 ? ph + 16 * (tid >> 7) : nullptr);
+  start_pingpong(smem);
+  PhaseClock pc(p.phase && (tid & 127) == 0 ? ph + 16 * wg : nullptr);
   const Frag f;
-  uint32_t nslot = 0;
+  Ring ring;
   float acc[128];
-  // attention task of this warp: tile rows r0 .. r0 + 15 (lane: rows r0 + ag, r0 + ag + 8), keys from tile row k0
+  // attention task of this warp: tile rows r0 .. r0 + 15 (lane: rows r0 + ag, r0 + ag + 8), keys from tile row k0 (inside
+  // the warpgroup's 64 rows: a walker slot is at most 32 rows and aligned)
   const int r0 = 16 * (tid >> 5), ag = (tid & 31) >> 2;
   const int k0 = r0 & ~((NP > 16 ? NP : 16) - 1);
+  // From here on the warpgroups only meet at the MMA token: warpgroup w owns tile rows 64 w .. +63 (operand rows, residual
+  // and Q / K / V scratch rows, attention keys) and synchronises its own 128 threads.  Both run every tile and layer of the
+  // CTA (a warpgroup without walkers computes on zero rows and stores nothing), so they take the token equally often.
   for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
     // global row of tile row r (-1: padding row or walker past the end)
     auto grow_of = [&](int r) -> long long {
       const int walker = tile * G + (r >> lnp), el = r & (NP - 1);
       return (el < N && walker < p.walkers) ? (long long)walker * N + el : -1;
     };
-    // ---- tile load: embedding rows -> residual stream and the operand buffer (loads in batches of 8 ahead of the stores)
-    for (int i0 = 0; i0 < 128 * 64 / kTrThreads; i0 += 8) {
+    // ---- tile load: the warpgroup's embedding rows -> residual stream and the operand buffer (loads in batches of 8 ahead
+    // of the stores)
+    for (int i0 = 0; i0 < 64 * 64 / 128; i0 += 8) {
       float4 x[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const int idx = tid + kTrThreads * (i0 + i), r = idx >> 6, c = 4 * (idx & 63);
+        const int idx = (tid & 127) + 128 * (i0 + i), r = 64 * wg + (idx >> 6), c = 4 * (idx & 63);
         const long long row = grow_of(r);
         x[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (row >= 0) {
@@ -113,21 +115,23 @@ trunk_f16_kernel(TrunkParams p) {
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const int idx = tid + kTrThreads * (i0 + i), r = idx >> 6, c = 4 * (idx & 63);
+        const int idx = (tid & 127) + 128 * (i0 + i), r = 64 * wg + (idx >> 6), c = 4 * (idx & 63);
         *(float4*)(resid + r * 256 + c) = x[i];
         const float sc = p.a_scale;
         store_operand_quad(smem, r, c, make_float4(x[i].x * sc, x[i].y * sc, x[i].z * sc, x[i].w * sc));
       }
     }
     fence_proxy_async();
-    __syncthreads();
+    wg_sync(wg);
     pc.mark(kPhLoad);
     for (int l = 0; l < L; ++l) {
       const bool last = l == L - 1;
       const CUtensorMap* lm = p.maps + 8 * l;
       // ---- Q | K | V = X Wqkv, 256 columns at a time -> scratch (true values)
       for (int j = 0; j < 3; ++j) {
-        gemm_abuf<256>(acc, smem, full, nslot, lm, lm + 1, 256 * j, p.err_flag, pc);
+        // one MMA token for the three column blocks: their epilogues are much shorter than a GEMM
+        const int turn = j == 0 ? kTurnTake : (j == 2 ? kTurnPass : kTurnKeep);
+        gemm_abuf<256>(acc, smem, ring, lm, lm + 1, 256 * j, turn, p.err_flag, pc);
         pc.mark(kPhQkv);
         const float us = p.us[l][0];
 #pragma unroll
@@ -138,9 +142,7 @@ trunk_f16_kernel(TrunkParams p) {
                 make_float2(acc[4 * jj + 2 * h] * us, acc[4 * jj + 2 * h + 1] * us);
         pc.mark(kPhQkvEpi);
       }
-      sb1[tid] = __ldg(p.b1[l] + tid);
-      sb2[tid] = __ldg(p.b2[l] + tid);
-      __syncthreads();  // Q / K / V rows of the whole tile are in the scratch buffer
+      wg_sync(wg);  // Q / K / V rows of the warpgroup are in the scratch buffer
       // ---- attention on the tensor cores, head by head -> k-block h of the operand buffer
       for (int h = 0; h < 4; ++h) {
         const float* qb = qkv + 64 * h;
@@ -159,7 +161,7 @@ trunk_f16_kernel(TrunkParams p) {
         else attn_task_mma<2, true>(p.attn_scale, qrow, krow, vrow, valid, store, NP < 16 ? NP : 0);
       }
       fence_proxy_async();
-      __syncthreads();
+      wg_sync(wg);
       pc.mark(kPhAttn);
       // ---- A = X + O Wo, M1 = tanh(A W1 + b1), X = A + tanh(M1 W2 + b2)
       const float* xin[2];
@@ -173,10 +175,10 @@ trunk_f16_kernel(TrunkParams p) {
         const long long row = grow_of(r);
         xout[h] = !last ? resid + r * 256 : (row >= 0 ? p.Out + (size_t)row * p.ldout : nullptr);
       }
-      mlp3<256>(acc, smem, full, nslot, lm + 2, lm + 3, lm + 4, lm + 5, lm + 6, lm + 7, p.us[l][1], p.us[l][2], p.us[l][3],
-                p.a_scale, sb1, sb2, xin, aout, xout, !last, p.err_flag, pc);
+      mlp3<256>(acc, smem, ring, lm + 2, lm + 3, lm + 4, lm + 5, lm + 6, lm + 7, p.us[l][1], p.us[l][2], p.us[l][3],
+                p.a_scale, p.b1[l], p.b2[l], xin, aout, xout, !last, p.err_flag, pc);
       fence_proxy_async();
-      __syncthreads();  // next layer's operand complete / next tile's load may overwrite the residual rows
+      wg_sync(wg);  // next layer's operand rows complete / next tile's load may overwrite the residual rows
       pc.mark(kPhMlpEpi);
       if (tid < 128) pc.count(kPhPairs);
     }

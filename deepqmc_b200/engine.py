@@ -732,7 +732,7 @@ class Engine:
         return out, self.MLP_PATHS[path.value]
 
     TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'w1_mainloop', 'w2_mainloop',
-                    'mlp_epilogues', 'weight_wait', 'tile_layer_pairs')
+                    'mlp_epilogues', 'weight_wait', 'mma_turn', 'tile_layer_pairs')
 
     def debug_trunk_phases(self):
         """{phase: cycles} of the whole-trunk kernel's timers (engine created with DQMC_TRUNK_PHASES=1) since the last call;
