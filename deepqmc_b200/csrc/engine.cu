@@ -78,6 +78,11 @@ struct EngineBase {
   virtual int debug_mlp(int layer, int S, const void* O, const void* X, void* Out, void* scratch, int rows, int32_t* path,
                         cudaStream_t st) = 0;
   virtual int debug_trunk_phases(uint64_t* out, int n) = 0;
+  virtual int debug_slater(const void* r, const void* R, const void* BF, int rows, int S, void* dsign, void* dlog, void* dgrad,
+                           void* dlap, int32_t* kernel, cudaStream_t st) = 0;
+  virtual int debug_det_sum(const void* r, const void* R, const void* dsign, const void* dlog, const void* dgrad,
+                            const void* dlap, int B, int S, void* sign, void* logp, void* grad, void* stats,
+                            cudaStream_t st) = 0;
   virtual int forward(const void* r, const void* R, int Rb, int B, void* sign, void* logp, void* ws, int64_t wsb,
                       cudaStream_t st) = 0;
   virtual int local_energy(const void* r, const void* R, int Rb, int B, uint64_t seed, const void* twist, void* E,
@@ -1113,6 +1118,56 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  int debug_slater(const void* r, const void* R, const void* BF, int rows, int S, void* dsign, void* dlog, void* dgrad,
+                   void* dlap, int32_t* kernel, cudaStream_t st) override {
+    if (S != 1 && S != T3 + 2) { err = "debug_slater: S must be 1 or 3N + 2"; return 2; }
+    if (rows < 1 || rows % (N * S) != 0) { err = "debug_slater: rows must be a positive multiple of N S"; return 2; }
+    if (S > 1 && (!dgrad || !dlap)) { err = "debug_slater: S = 3N + 2 needs the gradient and Laplacian outputs"; return 2; }
+    const int Bc = rows / (N * S);
+    // the activation runs in place: work on a copy so that the caller's rows stay as they were
+    T* bf = nullptr;
+    T* gadd = nullptr;
+    DQ_CHECK(cudaMalloc((void**)&bf, sizeof(T) * (size_t)rows * BFW));
+    if (cfg.backflow_add && cudaMalloc((void**)&gadd, sizeof(T) * (size_t)Bc * N * 5) != cudaSuccess) {
+      cudaFree(bf);
+      err = "debug_slater: out of device memory";
+      return 1;
+    }
+    int rc = 0;
+    if (cudaMemcpyAsync(bf, BF, sizeof(T) * (size_t)rows * BFW, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+      err = "debug_slater: copy of the backflow rows failed";
+      rc = 1;
+    }
+    if (!rc) rc = slater((const T*)r, (const T*)R, 0, Bc, S, bf, gadd, (T*)dsign, (T*)dlog, (T*)dgrad, (T*)dlap, st, nullptr,
+                         nullptr, 0, 0, kernel);
+    if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { err = "debug_slater: kernel failed"; rc = 1; }
+    cudaFree(bf);
+    cudaFree(gadd);
+    if (rc) return rc;
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
+  int debug_det_sum(const void* r, const void* R, const void* dsign, const void* dlog, const void* dgrad, const void* dlap,
+                    int B, int S, void* sign, void* logp, void* grad, void* stats, cudaStream_t st) override {
+    if (S != 1 && S != T3 + 2) { err = "debug_det_sum: S must be 1 or 3N + 2"; return 2; }
+    if (B < 1) { err = "debug_det_sum: needs at least one walker"; return 2; }
+    if (S > 1 && (!dgrad || !dlap || !grad || !stats)) { err = "debug_det_sum: S = 3N + 2 needs every jet array"; return 2; }
+    T* E = nullptr;  // the local energy finalize_kernel also writes; not part of the hook's outputs
+    DQ_CHECK(cudaMalloc((void**)&E, sizeof(T) * (size_t)B));
+    const FinalizeCfg fc = finalize_cfg(S);
+    DQ_LAUNCH(finalize_kernel<T>, dim3(B), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, (const T*)r, (const T*)R, 0,
+              (const T*)dsign, (const T*)dlog, (const T*)dgrad, (const T*)dlap, P("cusp.alpha"), (const T*)d_zval,
+              (const T*)d_ecp_loc, (const int*)d_ecp_mask, B, (T*)sign, (T*)logp, E, (T*)stats, (T*)grad,
+              cfg.conf_linear ? P("conf.w") : (const T*)nullptr, (const T*)nullptr,
+              cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr, PhArgs<T>());
+    const bool ok = cudaStreamSynchronize(st) == cudaSuccess;
+    cudaFree(E);
+    if (!ok) { err = "debug_det_sum: kernel failed"; return 1; }
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
   int debug_gemm(const char* wname, const char* bname, const void* A, const void* Res, void* C, int Mr, int S,
                  int sliced, int backend, cudaStream_t st) override {
     int64_t o = off(wname);
@@ -1525,40 +1580,45 @@ struct Engine : EngineBase {
     return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, X, st, nullptr, qa);
   }
 
-  // backflow heads -> Slater determinants -> det sum / cusp / potentials (shared by all trunks)
-  int tail(const T* r, const T* R, int Rb, int Bc, int S, int Bstat, T* sign, T* logp, T* E, T* stats, T* grad, Ws& w,
-           T* X, cudaStream_t st, const T* jastrow = nullptr, const T* qa = nullptr) {
-    // per-spin backflow heads: rows of electron e across walkers, weights by spin
-    gemm(X, bf_in, "bf.up", "bf.dn", cfg.n_up, BFW, gnn ? P("bfb.up") : nullptr, nullptr, 0, w.BF, BFW, Bc * S, BFW, bf_in, S, 1, N,
-         st, 0, gnn ? P("bfb.dn") : nullptr);
+  // Backflow activation -> K signed log-determinants (+ 3N tangents, Laplacian for S > 1), the kernel picked for the shape:
+  // BF [Bc N S][BFW] holds the backflow head rows before activation (row (b N + i) S + s) and is activated IN PLACE; Gadd
+  // [Bc N][5] receives the additive branch's electron factor.  env_base / v0 / vper: the non-local ECP's envelope table
+  // (slater_fwd2_kernel), qa: the pseudo-Hamiltonian metric (slater_kernel), both null outside those passes.  With mos_out
+  // set, the orbital matrices are written there instead of determinants.  *kernel (if given) = {DQMC_SLATER_KERNEL_*, the
+  // template instance NS / NM, 0 for the runtime-N kernels}.  The forward tails and dqmc_debug_slater both call this.
+  int slater(const T* r, const T* R, int Rb, int Bc, int S, T* BF, T* Gadd, T* dsign, T* dlog, T* dgrad, T* dlap,
+             cudaStream_t st, const T* qa, const T* env_base, int64_t v0, int vper, int32_t* kernel = nullptr) {
     if (cfg.mult_act == 1)  // default mult_act 1 + 2 tanh(x / 4) of the BackflowOp (nn_wave_function.py:14-33)
-      DQ_LAUNCH(act_fl_kernel<T>, dim3(Bc * N, (KN + 127) / 128), dim3(128), 0, st, w.BF, KN, (const T*)nullptr, 0, S, KN, T(1), 2);
+      DQ_LAUNCH(act_fl_kernel<T>, dim3(Bc * N, (KN + 127) / 128), dim3(128), 0, st, BF, KN, (const T*)nullptr, 0, S, KN, T(1), 2);
     const int full_det = cfg.factorized_det ? 0 : 1;
     const int mult_on = cfg.backflow_add == 1 ? 0 : 1;
     const T* gadd = nullptr;
     if (cfg.backflow_add) {
       // additive branch (wf/nn_wave_function.py:26-32): add_act on its head, electron-local factor cutoff * |envelope|
       if (qa) { err = "additive backflow with a pseudo-Hamiltonian is not supported"; return 2; }
-      DQ_LAUNCH(act_fl_kernel<T>, dim3(Bc * N, (KN + 127) / 128), dim3(128), 0, st, w.BF + add_off, BFW, (const T*)nullptr, 0, S, KN,
+      DQ_LAUNCH(act_fl_kernel<T>, dim3(Bc * N, (KN + 127) / 128), dim3(128), 0, st, BF + add_off, BFW, (const T*)nullptr, 0, S, KN,
                 T(1), 3);
       DQ_LAUNCH(bf_add_factor_kernel<T>, dim3((Bc * N + 63) / 64), dim3(64), 0, st, r, R, Rb, N, M, cfg.n_up, K, P("env.pi_up"),
-                P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), env_rep, full_det, w.Gadd, Bc * N);
-      gadd = w.Gadd;
+                P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), env_rep, full_det, Gadd, Bc * N);
+      gadd = Gadd;
     }
     if (mos_out) {  // Ansatz.apply(..., return_mos=True): orbital matrices instead of determinants
       const size_t tot = (size_t)Bc * K * N * N;
       DQ_LAUNCH(orbitals_kernel<T>, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, r, R, Rb, N, M, cfg.n_up, K,
-                P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)w.BF, BFW, env_rep, full_det,
+                P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, BFW, env_rep, full_det,
                 mos_out, tot, gadd, add_off, mult_on);
       return 0;
     }
+    int32_t which = DQMC_SLATER_KERNEL_GENERIC, inst = 0;
     const int sl_wpb = slater_warps_per_block<T>(N);
     if ((N <= 4 || (N <= 6 && std::is_same<T, float>::value)) && !qa && !gadd && !std::getenv("DQMC_SLATER_GENERIC")) {
       const int tot = Bc * K;
+      which = DQMC_SLATER_KERNEL_SMALL;
 #define DQ_SL_SMALL(NS_)                                                                                           \
+  inst = NS_;                                                                                                      \
   DQ_LAUNCH((slater_small_kernel<T, NS_>), dim3((tot + 63) / 64), dim3(64), 0, st, r, R, Rb, M, cfg.n_up, K, S, tot,    \
-            P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)w.BF, KN, w.dsign, w.dlog, \
-            w.dgrad, w.dlap, env_rep, full_det)
+            P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, dsign, dlog, \
+            dgrad, dlap, env_rep, full_det)
       switch (N) {
         case 2: DQ_SL_SMALL(2); break;
         case 3: DQ_SL_SMALL(3); break;
@@ -1570,32 +1630,53 @@ struct Engine : EngineBase {
     } else if (S == 1 && N <= 32 && slater_fwd2_ok && !gadd) {
       const int nthr = 32 * K < 256 ? 32 * K : 256;
       const int grid = Bc < 3 * n_sms ? Bc : 3 * n_sms;
+      which = DQMC_SLATER_KERNEL_FWD2;
       // register-resident LU: the row array is sized to the electron count where an exact instance exists (every padded
       // column costs a shuffle + FMA per elimination step)
 #define DQ_SL_FWD2(NMV)                                                                                                        \
+  inst = NMV;                                                                                                                  \
   DQ_LAUNCH((slater_fwd2_kernel<T, NMV>), dim3(grid), dim3(nthr), slater_fwd2_smem_bytes<T>(N, M, K), st, r, R, Rb, N, M,      \
-            cfg.n_up, K, Bc, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)w.BF, KN, w.dsign, \
-            w.dlog, env_rep, full_det, ecp_env, (long long)ecp_v0, ecp_vper)
-      if (N == 14) DQ_SL_FWD2(14);
-      else if (N <= 16) DQ_SL_FWD2(16);
-      else if (N == 28) DQ_SL_FWD2(28);
-      else if (N == 30) DQ_SL_FWD2(30);
-      else DQ_SL_FWD2(32);
+            cfg.n_up, K, Bc, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, dsign,     \
+            dlog, env_rep, full_det, env_base, (long long)v0, vper)
+      if (N == 14) { DQ_SL_FWD2(14); }
+      else if (N <= 16) { DQ_SL_FWD2(16); }
+      else if (N == 28) { DQ_SL_FWD2(28); }
+      else if (N == 30) { DQ_SL_FWD2(30); }
+      else { DQ_SL_FWD2(32); }
 #undef DQ_SL_FWD2
     } else if (S == 1 && N <= 32 && !gadd && !std::getenv("DQMC_SLATER_GENERIC")) {
       const int wpb = K < 8 ? K : 8;
+      which = DQMC_SLATER_KERNEL_FWD_REG;
       DQ_LAUNCH(slater_fwd_reg_kernel<T>, dim3(Bc), dim3(32 * wpb), sizeof(T) * N * M, st, r, R, Rb, N, M, cfg.n_up, K,
-                P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)w.BF, KN, w.dsign, w.dlog,
+                P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, dsign, dlog,
                 env_rep, full_det);
     } else
     DQ_LAUNCH(slater_kernel<T>, dim3((Bc * K + sl_wpb - 1) / sl_wpb), dim3(32 * sl_wpb), slater_smem_bytes<T>(N), st, r, R,
-              Rb, N, M, cfg.n_up, K, S, Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)w.BF, BFW, w.dsign, w.dlog,
-              w.dgrad, w.dlap, env_rep, full_det, qa, gadd, add_off, mult_on);
+              Rb, N, M, cfg.n_up, K, S, Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, BFW, dsign, dlog,
+              dgrad, dlap, env_rep, full_det, qa, gadd, add_off, mult_on);
+    if (kernel) { kernel[0] = which; kernel[1] = inst; }
+    return 0;
+  }
+
+  // the determinant sum's configuration (finalize_kernel): cusp, ECP and nuclear-cusp terms as the engine was created
+  FinalizeCfg finalize_cfg(int S) const {
     FinalizeCfg fc;
     fc.N = N; fc.M = M; fc.n_up = cfg.n_up; fc.K = K; fc.S = S; fc.cusp_kind = cfg.cusp_kind;
     fc.cusp_same_scale = cfg.cusp_same_scale; fc.cusp_anti_scale = cfg.cusp_anti_scale;
     fc.ecp_terms = cfg.ecp_loc_terms;
     fc.nuc_cusp_kind = cfg.nuc_cusp_kind;
+    return fc;
+  }
+
+  // backflow heads -> Slater determinants -> det sum / cusp / potentials (shared by all trunks)
+  int tail(const T* r, const T* R, int Rb, int Bc, int S, int Bstat, T* sign, T* logp, T* E, T* stats, T* grad, Ws& w,
+           T* X, cudaStream_t st, const T* jastrow = nullptr, const T* qa = nullptr) {
+    // per-spin backflow heads: rows of electron e across walkers, weights by spin
+    gemm(X, bf_in, "bf.up", "bf.dn", cfg.n_up, BFW, gnn ? P("bfb.up") : nullptr, nullptr, 0, w.BF, BFW, Bc * S, BFW, bf_in, S, 1, N,
+         st, 0, gnn ? P("bfb.dn") : nullptr);
+    int rc = slater(r, R, Rb, Bc, S, w.BF, w.Gadd, w.dsign, w.dlog, w.dgrad, w.dlap, st, qa, ecp_env, ecp_v0, ecp_vper);
+    if (rc || mos_out) return rc;
+    const FinalizeCfg fc = finalize_cfg(S);
     DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb,
               (const T*)w.dsign, (const T*)w.dlog, (const T*)w.dgrad, (const T*)w.dlap, P("cusp.alpha"),
               (const T*)d_zval, (const T*)d_ecp_loc, (const int*)d_ecp_mask, Bstat, sign, logp, E, stats, grad,
@@ -2605,6 +2686,21 @@ int dqmc_debug_mlp(dqmc_handle h, int32_t layer, int32_t S, const void* O, const
   DQ_NEED_DEVICE(h);
   if (!O || !X || !Out || !scratch) { h->e->err = "dqmc_debug_mlp: null array"; return 2; }
   return h->e->debug_mlp(layer, S, O, X, Out, scratch, rows, path, (cudaStream_t)stream);
+}
+int dqmc_debug_slater(dqmc_handle h, const void* r, const void* R, const void* BF, int32_t rows, int32_t S, void* det_sign,
+                      void* det_log, void* det_grad, void* det_lap, int32_t* kernel, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!r || !R || !BF || !det_sign || !det_log) { h->e->err = "dqmc_debug_slater: null array"; return 2; }
+  return h->e->debug_slater(r, R, BF, rows, S, det_sign, det_log, det_grad, det_lap, kernel, (cudaStream_t)stream);
+}
+int dqmc_debug_det_sum(dqmc_handle h, const void* r, const void* R, const void* det_sign, const void* det_log,
+                       const void* det_grad, const void* det_lap, int32_t B, int32_t S, void* sign, void* logp, void* grad,
+                       void* stats, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!r || !R || !det_sign || !det_log || !sign || !logp) { h->e->err = "dqmc_debug_det_sum: null array"; return 2; }
+  return h->e->debug_det_sum(r, R, det_sign, det_log, det_grad, det_lap, B, S, sign, logp, grad, stats, (cudaStream_t)stream);
 }
 int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n) {
   if (!h) return 2;

@@ -14,6 +14,10 @@ namespace dq {
 //   full determinant, jnp.linalg.slogdet = partial-pivot LU sign/log convention).
 //   d_t log|det A| = tr(A^-1 A^t);  lap log|det A| = tr(A^-1 A^L) - sum_t tr((A^-1 A^t)^2)
 // BF: augmented rows [b][i][s][K*N] (orbital index k*N + mu, wf/omni.py:78-88).
+// Every Slater kernel below follows slogdet's convention for an exactly singular A (a zero pivot: a zero orbital column or
+// electron row, or an envelope flushed to zero): no division by the zero pivot, sign 0 and log -inf.  A^-1 does not exist
+// there, so the gradient and Laplacian outputs of such a determinant carry no meaning (the determinant sum weighs them by
+// exp(-inf) = 0).
 // ------------------------------------------------------------------------------------------
 // lane-strided walk over a rows x cols index space without per-item division
 struct LaneWalk {
@@ -221,7 +225,9 @@ __global__ void slater_kernel(const T* __restrict__ r, const T* __restrict__ R, 
     sgn *= (prow != c ? -sg : sg);
     for (int rr = lane; rr < N; rr += 32) fcol[rr] = aug[rr * N2 + c];
     __syncwarp();
-    const T ipv = T(1) / pv;
+    // an exactly singular matrix (the whole remaining column is zero): no division by the zero pivot -- the pivot row is
+    // scaled to zero, so the elimination below changes nothing -- and (sign 0, log -inf) as slogdet gives
+    const T ipv = pv != T(0) ? T(1) / pv : T(0);
     for (int j = lane; j < 2 * N; j += 32) aug[c * N2 + j] *= ipv;
     __syncwarp();
     for (LaneWalk w(lane, 2 * N); w.i < N; w.next()) {
@@ -380,6 +386,7 @@ __global__ void slater_small_kernel(const T* __restrict__ r, const T* __restrict
     logdet += m_log(m_abs(pv));
     const T sg = pv > T(0) ? T(1) : (pv < T(0) ? T(-1) : T(0));
     sgn *= (prow != c ? -sg : sg);
+    if (pv == T(0)) continue;  // exactly singular: no division by zero, (sign 0, log -inf) like slogdet
     const T ipv = T(1) / pv;
 #pragma unroll
     for (int j = 0; j < NS; ++j) { A[c][j] *= ipv; Ai[c][j] *= ipv; }
@@ -505,7 +512,7 @@ __global__ void slater_fwd_reg_kernel(const T* __restrict__ r, const T* __restri
       logdet += m_log(m_abs(pv));
       sgn *= pv > T(0) ? T(1) : (pv < T(0) ? T(-1) : T(0));
       const bool elim = !((used >> lane) & 1u);  // rows not yet used (prow itself is used now)
-      const T f = elim ? a[c] / pv : T(0);
+      const T f = (elim && pv != T(0)) ? a[c] / pv : T(0);  // exactly singular: (sign 0, log -inf) like slogdet
 #pragma unroll
       for (int j = c + 1; j < NM; ++j) {
         const T pj = __shfl_sync(0xffffffffu, a[j], prow);

@@ -731,6 +731,54 @@ class Engine:
         self._check(rc, 'dqmc_debug_mlp')
         return out, self.MLP_PATHS[path.value]
 
+    SLATER_KERNELS = ('slater_small_kernel', 'slater_fwd2_kernel', 'slater_fwd_reg_kernel', 'slater_kernel')
+
+    def _nuclei(self):
+        return self._prep(self.hamil.mol.coords)
+
+    def debug_slater(self, r, BF, S=1):
+        """The engine's Slater determinants (backflow activation + the determinant kernel it picks) on walker positions
+        r [B, N, 3] and pre-activation backflow head rows BF [B N S, BFW] (row (b N + i) S + s; BFW = K N, 2 K N for
+        backflow_transform 'both'), the nuclei of the Hamiltonian -> (det_sign [B, K], det_log [B, K], det_grad [B, K, 3N] or
+        None, det_lap [B, K] or None, kernel name with its template instance, e.g. 'slater_fwd2_kernel<30>').  BF is not
+        changed (self-test hook)."""
+        r, BF = self._prep(r), self._prep(BF)
+        N, K = self.spec.n_elec, self.spec.n_determinants
+        B = r.shape[0]
+        assert r.shape == (B, N, 3) and BF.dim() == 2 and BF.shape[0] == B * N * S, (tuple(r.shape), tuple(BF.shape))
+        mk = lambda *s: torch.empty(*s, dtype=self.dtype, device=self.device)
+        sign, log = mk(B, K), mk(B, K)
+        grad, lap = (mk(B, K, 3 * N), mk(B, K)) if S > 1 else (None, None)
+        kernel = (C.c_int32 * 2)(-1, -1)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        R = self._nuclei()  # held until the call returns
+        rc = self.lib.dqmc_debug_slater(self.h, r.data_ptr(), R.data_ptr(), BF.data_ptr(), BF.shape[0], S,
+                                        sign.data_ptr(), log.data_ptr(), ptr(grad), ptr(lap), kernel, self._stream())
+        self._check(rc, 'dqmc_debug_slater')
+        name = self.SLATER_KERNELS[kernel[0]] + (f'<{kernel[1]}>' if kernel[1] else '')
+        return sign, log, grad, lap, name
+
+    def debug_det_sum(self, r, det_sign, det_log, det_grad=None, det_lap=None):
+        """The engine's determinant sum (finalize_kernel; no Jastrow, no pseudo-Hamiltonian) on det_sign / det_log [B, K] and,
+        for the forward-Laplacian pass, det_grad [B, K, 3N] / det_lap [B, K] -> (sign [B], log|psi| [B], grad log|psi|
+        [B, 3N] or None, stats [6, B] or None: stats[4] = lap log|psi|, stats[5] = |grad log|psi||^2) (self-test hook)."""
+        r, det_sign, det_log = self._prep(r), self._prep(det_sign), self._prep(det_log)
+        N = self.spec.n_elec
+        B = r.shape[0]
+        S = 3 * N + 2 if det_grad is not None else 1
+        mk = lambda *s: torch.empty(*s, dtype=self.dtype, device=self.device)
+        sign, log = mk(B), mk(B)
+        grad, stats = (mk(B, 3 * N), mk(6, B)) if S > 1 else (None, None)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        dg = self._prep(det_grad) if det_grad is not None else None
+        dl = self._prep(det_lap) if det_lap is not None else None
+        R = self._nuclei()
+        rc = self.lib.dqmc_debug_det_sum(self.h, r.data_ptr(), R.data_ptr(), det_sign.data_ptr(),
+                                         det_log.data_ptr(), ptr(dg), ptr(dl), B, S, sign.data_ptr(), log.data_ptr(),
+                                         ptr(grad), ptr(stats), self._stream())
+        self._check(rc, 'dqmc_debug_det_sum')
+        return sign, log, grad, stats
+
     TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'w1_mainloop', 'w2_mainloop',
                     'mlp_epilogues', 'weight_wait', 'mma_turn', 'tile_layer_pairs')
 

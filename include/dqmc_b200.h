@@ -279,6 +279,38 @@ enum {
 int dqmc_debug_mlp(dqmc_handle h, int32_t layer, int32_t S, const void* O, const void* X, void* Out, void* scratch, int32_t rows,
                    int32_t* path, void* stream);
 
+/* Self-test hook: the Slater determinants of the engine, run by the same Engine::slater the forward tails call: the backflow
+ * activation (mult_act, the additive head's add_act and its electron factor) and the determinant kernel the engine picks for
+ * the shape, on caller-supplied inputs.  r [B][N][3] walker positions, R [M][3] the nuclei; BF [rows][BFW] the backflow head
+ * rows BEFORE activation, exactly as the bf.up / bf.dn GEMM writes them: rows = B N S, row (b N + i) S + s; BFW = K N, or
+ * 2 K N with backflow_transform 'both' (the multiplicative head, then the additive one).  The activation runs on a copy: BF
+ * is not changed.  S = 1: plain forward; S = 3N + 2: slot 0 the value, slots 1 .. 3N the r-tangents, slot 3N + 1 the
+ * r-Laplacian.  Outputs det_sign / det_log [B][K] (slogdet convention: an exactly singular matrix gives sign 0, log -inf);
+ * for S = 3N + 2 also det_grad [B][K][3N] and det_lap [B][K] (not meaningful where the matrix is singular).
+ * kernel (if not null) receives two values: the kernel that ran, one of DQMC_SLATER_KERNEL_*, and its template instance (NS
+ * of slater_small_kernel, NM of slater_fwd2_kernel, 0 for the runtime-N kernels).
+ * Status 2 for S other than 1 or 3N + 2, rows not a positive multiple of N S, or null arrays.
+ * reference: wf/env.py:57-75, wf/nn_wave_function.py:14-33, :111-151. */
+enum {
+  DQMC_SLATER_KERNEL_SMALL = 0,    /* slater_small_kernel<NS>: one thread per determinant, N <= 4 (fp32: N <= 6) */
+  DQMC_SLATER_KERNEL_FWD2 = 1,     /* slater_fwd2_kernel<NM>: persistent plain forward, N <= 32 */
+  DQMC_SLATER_KERNEL_FWD_REG = 2,  /* slater_fwd_reg_kernel: plain forward, lane = row, when fwd2 does not fit */
+  DQMC_SLATER_KERNEL_GENERIC = 3   /* slater_kernel: warp Gauss-Jordan with an explicit inverse, every other case */
+};
+int dqmc_debug_slater(dqmc_handle h, const void* r, const void* R, const void* BF, int32_t rows, int32_t S, void* det_sign,
+                      void* det_log, void* det_grad, void* det_lap, int32_t* kernel, void* stream);
+
+/* Self-test hook: the determinant sum (finalize_kernel with the engine's cusp, conf_coeff and nuclear-cusp settings; no
+ * Jastrow, no pseudo-Hamiltonian) on caller-supplied determinants det_sign / det_log [B][K], and for S = 3N + 2 det_grad
+ * [B][K][3N] / det_lap [B][K]; r [B][N][3], R [M][3] as in dqmc_debug_slater (the e-e cusp and the potentials read them).
+ * -> sign / logp [B] (log|psi| = log|sum_k c_k s_k exp(l_k)|, sign 0 and log -inf when the sum vanishes); for S = 3N + 2
+ * also grad [B][3N] = grad log|psi| and stats [6][B] in the layout of dqmc_local_energy (stats[4] = lap log|psi|,
+ * stats[5] = |grad log|psi||^2).  Status 2 for S other than 1 or 3N + 2, B < 1, or null arrays.
+ * reference: wf/nn_wave_function.py:152-171. */
+int dqmc_debug_det_sum(dqmc_handle h, const void* r, const void* R, const void* det_sign, const void* det_log,
+                       const void* det_grad, const void* det_lap, int32_t B, int32_t S, void* sign, void* logp, void* grad,
+                       void* stats, void* stream);
+
 /* Measurement aid: the phase timers of the whole-trunk kernel, summed over every launch since the last call, then reset.  On
  * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 10.  out[0..9]: clock64()
  * cycles of the consumer warpgroups in tile load, QKV mainloop, QKV epilogue, attention, Wo / W1 / W2 mainloops, MLP

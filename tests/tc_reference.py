@@ -6,7 +6,7 @@ import torch
 
 def weight(eng, name, dtype=torch.float64):
     """Parameter `name` of the engine's table as the device sees it (rounded to fp32 for an fp32 engine), as a [K, N] tensor."""
-    flat = torch.as_tensor(eng._flat, device='cuda:0')
+    flat = torch.as_tensor(eng._flat, device=eng.device)
     off, K, Nc = eng.entries[name]
     w = flat[off:off + K * Nc].reshape(K, Nc)
     return (w.float() if eng.dtype == torch.float32 else w).to(dtype)

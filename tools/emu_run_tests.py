@@ -12,8 +12,12 @@ round's GPU minutes ran out was first checked here (DESIGN.md section 8).  What 
     LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0:detect_stack_use_after_return=0).
 The wgmma / TMA kernels are not emulated (the build sets DQMC_NO_TCGEN05): engines are created with gemm_backend = 0.
 
-Usage:  python tools/emu_run_tests.py [--lib PATH] [--nobuild] [--asan] test_name [test_name ...]
-        python tools/emu_run_tests.py --all-small          (every test small enough for the emulator, both files)
+The emulator replaces ex2.approx / rcp.approx / redux.sync by exact code: it checks layouts and protocols, never accuracy.
+
+Usage:  python tools/emu_run_tests.py [--lib PATH] [--nobuild] [--asan] test_name[substring] [test_name ...]
+        python tools/emu_run_tests.py --all-small          (every test small enough for the emulator, parity files)
+Tests come from test_gpu_parity.py, test_gpu_z_next_rows.py and test_gpu_slater_conformance.py; stacked parametrize marks run
+as their cartesian product, and `name[substring]` keeps the cases whose arguments' repr contains the substring.
 """
 import argparse
 import importlib
@@ -93,25 +97,42 @@ def main():
         if hasattr(mod, 'torch'):
             mod.torch = TorchProxy()
 
+    import itertools
+
+    import pytest
+
+    pytest_param_type = type(pytest.param(0))
     import test_gpu_parity as P
+    import test_gpu_slater_conformance as SC
     import test_gpu_z_next_rows as Z
 
-    P.DEV = Z.DEV = 'cpu'
+    P.DEV = Z.DEV = SC.DEV = 'cpu'
+    torch.cuda.synchronize = lambda *args, **kw: None
     names = list(a.names)
     if a.all_small:
         names += [n for mod in (P, Z) for n in vars(mod) if n.startswith('test_') and n not in TOO_BIG and n not in names]
     for name in names:
-        f = getattr(Z, name, None) or getattr(P, name)
-        marks = [m for m in getattr(f, 'pytestmark', []) if m.name == 'parametrize']
+        # name or name[substring]: the cases whose printed arguments contain the substring
+        name, _, sel = name.partition('[')
+        sel = sel.rstrip(']')
+        f = getattr(Z, name, None) or getattr(P, name, None) or getattr(SC, name)
         wants_tmp = 'tmp_path' in f.__code__.co_varnames[:f.__code__.co_argcount]
-        cases = [()]
-        if marks:
-            argnames, values = marks[0].args[:2]
-            n_args = len(argnames.split(',')) if isinstance(argnames, str) else len(argnames)
-            cases = [(v,) if n_args == 1 else tuple(v) for v in values]
-        for vals in cases:
-            f(*((pathlib.Path(tempfile.mkdtemp()),) if wants_tmp else ()), *vals)
-            print('ok', name, *vals, flush=True)
+        # stacked parametrize marks: the cartesian product of their cases, passed by argument name
+        axes = []
+        for m in (m for m in getattr(f, 'pytestmark', []) if m.name == 'parametrize'):
+            argnames, values = m.args[:2]
+            argnames = [s.strip() for s in argnames.split(',')] if isinstance(argnames, str) else list(argnames)
+            tups = [tuple(v.values) if isinstance(v, pytest_param_type) else (v,) if len(argnames) == 1 else tuple(v)
+                    for v in values]
+            axes.append([dict(zip(argnames, t)) for t in tups])
+        for combo in itertools.product(*axes):
+            kw = {k: v for d in combo for k, v in d.items()}
+            if sel and sel not in repr(kw):
+                continue
+            if wants_tmp:
+                kw['tmp_path'] = pathlib.Path(tempfile.mkdtemp())
+            f(**kw)
+            print('ok', name, kw, flush=True)
 
 
 if __name__ == '__main__':
