@@ -89,6 +89,43 @@ __device__ __forceinline__ void cp_async_wait_group() {
 #endif
 }
 
+// The (up, down) pair that virtual walker p of the spin pass swaps (reference: physics.py:186-223).  down_idx < 0: exact
+// estimator, all n_up n_down pairs, p = a n_down + (beta - n_up); otherwise spin-raising, beta = down_idx and p = a.
+__host__ __device__ __forceinline__ void spin_pair(int p, int n_up, int N, int down_idx, int& a, int& beta) {
+  if (down_idx < 0) {
+    const int nd = N - n_up;
+    a = p / nd;
+    beta = n_up + (p - a * nd);
+  } else {
+    a = p;
+    beta = down_idx;
+  }
+}
+
+// Compact virtual-walker forwards: virtual walker v is base walker v / vper with one or two electrons moved; the consumers
+// (embed_fwd_kernel, the whole-trunk kernel's tile load, slater_fwd2_kernel) take every other electron's rows from tables of
+// the base walkers.  Two layouts:
+//   layout == kVirtEcp: non-local ECP quadrature (ecp_points_kernel, v = ((w J + j) N + i) 12 + q): electron e0 = (v / 12) % N
+//     moved to a quadrature point, e1 = -1;
+//   layout >= -1: spin swaps (spin_pairs_kernel, v = w vper + p): up electron e0 and down electron e1 of pair p exchange
+//     positions; layout is the down_idx of spin_pair (-1: all pairs).
+constexpr int kVirtEcp = -2;
+// Virtual-walker indices are 32-bit: a group's virtual walkers are one plain-forward batch (int walker count).
+struct VirtualMove {
+  int base, e0, e1;
+};
+__host__ __device__ __forceinline__ VirtualMove virtual_move(int v, int vper, int N, int n_up, int layout) {
+  VirtualMove m;
+  m.base = v / vper;
+  if (layout == kVirtEcp) {
+    m.e0 = (v / 12) % N;
+    m.e1 = -1;
+  } else {
+    spin_pair(v - m.base * vper, n_up, N, layout, m.e0, m.e1);
+  }
+  return m;
+}
+
 template <class T>
 __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll

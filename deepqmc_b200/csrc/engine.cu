@@ -93,6 +93,8 @@ struct EngineBase {
                        const void* nu, void* stats, void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int vjp_params(const void* r, const void* R, int Rb, int B, const void* weights, void* sign, void* logp,
                          void* grad_params, void* ws, int64_t wsb, cudaStream_t st) = 0;
+  virtual int spin(const void* r, const void* R, int Rb, int B, const void* sign, const void* logp, int down_idx, void* s2,
+                   void* ratio, void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int orbitals(const void* r, const void* R, int Rb, int B, void* out, void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int set_ph(int n_tab, int n_grid, double r_max, const double* tables, const int32_t* tab_of_nuc) = 0;
   virtual int debug_gemm(const char* wname, const char* bname, const void* A, const void* Res, void* C, int Mr, int S,
@@ -351,12 +353,14 @@ struct Engine : EngineBase {
   int Mn = 0, env_rep = 1;
   size_t max_smem = 0;
   int n_sms = 132;
-  // non-local ECP group in flight: envelope table of its base walkers [nb][N][K N] (null outside the quadrature forwards),
-  // index of the current chunk's first virtual walker, virtual walkers per base walker (J N 12)
+  // compact virtual-walker group in flight (non-local ECP quadrature or spin swaps): envelope table of its base walkers
+  // [nb][N][K N] (null outside those forwards), index of the current chunk's first virtual walker, virtual walkers per base
+  // walker (J N 12, or the swapped pairs), and the layout of virtual_move (common.cuh)
   const T* ecp_env = nullptr;
   const T* ecp_emb = nullptr;  // ... and their embedding rows [nb][N][d] (whole-trunk kernel only)
   int64_t ecp_v0 = 0;
   int ecp_vper = 0;
+  int virt_layout = kVirtEcp;
 #if !defined(DQMC_NO_TCGEN05)
   struct TcWeight {
     float* hi = nullptr; float* lo = nullptr; CUtensorMap mh, ml; int N = 0, K = 0;
@@ -807,6 +811,20 @@ struct Engine : EngineBase {
     const int64_t V = nb * J * N * 12;
     return ecp_prefix_bytes(nb) + (int64_t)chunk_bytes((int)V, 1);
   }
+  // spin pass for nb walkers with P swapped pairs each: virtual walkers r_virt[V][N][3], sign[V], log[V], the base walkers'
+  // sign[nb], log[nb], envelope table and embedding rows + one forward chunk over all V = nb P virtual walkers
+  int64_t spin_prefix_bytes(int64_t nb, int64_t P) const {
+    const int64_t V = nb * P;
+    return (int64_t)align_up(sizeof(T) * V * 3 * N) + 2 * (int64_t)align_up(sizeof(T) * V) + 2 * (int64_t)align_up(sizeof(T) * nb) +
+           (int64_t)align_up(sizeof(T) * nb * N * K * N) + (int64_t)align_up(sizeof(T) * nb * N * d);
+  }
+  int64_t spin_group_cap(int64_t P) const {
+    const int64_t vcap = 2000000000LL / ((int64_t)N * 3 * d);
+    return std::max<int64_t>(1, vcap / std::max<int64_t>(P, 1));
+  }
+  int64_t spin_bytes(int64_t nb, int64_t P) const {  // P >= 1 (the base forward of nb <= nb P walkers fits the same chunk)
+    return spin_prefix_bytes(nb, P) + (int64_t)chunk_bytes((int)(nb * P), 1);
+  }
   int64_t mcmc_prefix_bytes(int B) const {
     return (int64_t)align_up(sizeof(T) * (size_t)B * 3 * N) + 2 * (int64_t)align_up(sizeof(T) * (size_t)B) + 256;
   }
@@ -834,6 +852,10 @@ struct Engine : EngineBase {
     if (mode == DQMC_MODE_VJP) return vjp_chunk_bytes(B);
     if (mode == DQMC_MODE_MCMC) return mcmc_prefix_bytes(B) + (int64_t)chunk_bytes(B, 1);
     if (mode == DQMC_MODE_LANGEVIN) return langevin_prefix_bytes(B) + force_prefix_bytes(B) + (int64_t)chunk_bytes(B, T3 + 2);
+    if (mode == DQMC_MODE_SPIN) {  // sized for the exact estimator, the larger of the two; no down electrons: no forwards
+      const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
+      return P ? spin_bytes(std::min<int64_t>(B, spin_group_cap(P)), P) : 0;
+    }
     int S = mode == DQMC_MODE_FORWARD ? 1 : T3 + 2;
     int64_t need = (int64_t)chunk_bytes(B, S);
     if (mode == DQMC_MODE_LOCAL_ENERGY && J > 0) need = std::max<int64_t>(need, ecp_bytes(std::min<int64_t>(B, ecp_group_cap())));
@@ -849,6 +871,10 @@ struct Engine : EngineBase {
       case DQMC_MODE_LANGEVIN: return langevin_prefix_bytes(B) + force_prefix_bytes(B) + (int64_t)chunk_bytes(1, S);
       case DQMC_MODE_LOCAL_ENERGY:
         return std::max<int64_t>((int64_t)chunk_bytes(1, S), J > 0 ? ecp_prefix_bytes(1) + (int64_t)chunk_bytes(1, 1) : 0);
+      case DQMC_MODE_SPIN: {
+        const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
+        return P ? spin_prefix_bytes(1, P) + (int64_t)chunk_bytes(1, 1) : 0;
+      }
       default: return (int64_t)chunk_bytes(1, 1);
     }
   }
@@ -876,6 +902,7 @@ struct Engine : EngineBase {
         rc = langevin(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, B, 1, 0.5, -1, 0, 0, 0, nullptr, nullptr,
                       nullptr, ws, wsb, nullptr);
         break;
+      case DQMC_MODE_SPIN: rc = spin(nullptr, nullptr, 0, B, nullptr, nullptr, -1, nullptr, nullptr, ws, wsb, nullptr); break;
       default: err = "unknown mode"; rc = 2;
     }
     if (carved) *carved = dry_hwm - plan_base();
@@ -1042,6 +1069,7 @@ struct Engine : EngineBase {
       tc::TrunkParams p;
       p.X0 = X0; p.ldx = d; p.Out = Out; p.ldout = d; p.maps = d_trunk_maps; p.scratch = d_trunk_scratch;
       p.Xbase = Xbase; p.v0 = Xbase ? (long long)ecp_v0 : 0; p.vper = Xbase ? ecp_vper : 0;
+      p.n_up = cfg.n_up; p.vlayout = virt_layout; p.wspin = P("emb.w") + (size_t)(4 * M) * d;  // the +-1 spin feature's row
       int np2 = 1;
       while (np2 < N) np2 *= 2;  // walker slot of the tile: electrons rounded up to a power of two (<= 32)
       p.walkers = rows / N; p.N = N; p.NP = np2; p.L = cfg.n_layers; p.a_scale = kActScale;
@@ -1139,7 +1167,7 @@ struct Engine : EngineBase {
       rc = 1;
     }
     if (!rc) rc = slater((const T*)r, (const T*)R, 0, Bc, S, bf, gadd, (T*)dsign, (T*)dlog, (T*)dgrad, (T*)dlap, st, nullptr,
-                         nullptr, 0, 0, kernel);
+                         nullptr, 0, 0, kVirtEcp, kernel);
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { err = "debug_slater: kernel failed"; rc = 1; }
     cudaFree(bf);
     cudaFree(gadd);
@@ -1542,7 +1570,10 @@ struct Engine : EngineBase {
     }
     const int F = 4 * M + 1;
     const bool compact = S == 1 && embed_fwd_ok && ecp_emb && can_trunk(S);
-    if (compact) {
+    if (compact && virt_layout != kVirtEcp) {
+      // spin swaps: no embedding launch -- the whole-trunk kernel's tile load forms the two swapped rows from the base walkers'
+      // table (the embedding is linear in the spin feature)
+    } else if (compact) {
       // quadrature forwards of the non-local ECP: only the moved electron's embedding row is new, the whole-trunk kernel
       // takes the other rows from the base walkers' table
       int epb = (Bc / (2 * n_sms)) / 32 * 32;
@@ -1587,7 +1618,8 @@ struct Engine : EngineBase {
   // set, the orbital matrices are written there instead of determinants.  *kernel (if given) = {DQMC_SLATER_KERNEL_*, the
   // template instance NS / NM, 0 for the runtime-N kernels}.  The forward tails and dqmc_debug_slater both call this.
   int slater(const T* r, const T* R, int Rb, int Bc, int S, T* BF, T* Gadd, T* dsign, T* dlog, T* dgrad, T* dlap,
-             cudaStream_t st, const T* qa, const T* env_base, int64_t v0, int vper, int32_t* kernel = nullptr) {
+             cudaStream_t st, const T* qa, const T* env_base, int64_t v0, int vper, int vlayout = kVirtEcp,
+             int32_t* kernel = nullptr) {
     if (cfg.mult_act == 1)  // default mult_act 1 + 2 tanh(x / 4) of the BackflowOp (nn_wave_function.py:14-33)
       DQ_LAUNCH(act_fl_kernel<T>, dim3(Bc * N, (KN + 127) / 128), dim3(128), 0, st, BF, KN, (const T*)nullptr, 0, S, KN, T(1), 2);
     const int full_det = cfg.factorized_det ? 0 : 1;
@@ -1637,7 +1669,7 @@ struct Engine : EngineBase {
   inst = NMV;                                                                                                                  \
   DQ_LAUNCH((slater_fwd2_kernel<T, NMV>), dim3(grid), dim3(nthr), slater_fwd2_smem_bytes<T>(N, M, K), st, r, R, Rb, N, M,      \
             cfg.n_up, K, Bc, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, dsign,     \
-            dlog, env_rep, full_det, env_base, (long long)v0, vper)
+            dlog, env_rep, full_det, env_base, (long long)v0, vper, vlayout)
       if (N == 14) { DQ_SL_FWD2(14); }
       else if (N <= 16) { DQ_SL_FWD2(16); }
       else if (N == 28) { DQ_SL_FWD2(28); }
@@ -1674,7 +1706,8 @@ struct Engine : EngineBase {
     // per-spin backflow heads: rows of electron e across walkers, weights by spin
     gemm(X, bf_in, "bf.up", "bf.dn", cfg.n_up, BFW, gnn ? P("bfb.up") : nullptr, nullptr, 0, w.BF, BFW, Bc * S, BFW, bf_in, S, 1, N,
          st, 0, gnn ? P("bfb.dn") : nullptr);
-    int rc = slater(r, R, Rb, Bc, S, w.BF, w.Gadd, w.dsign, w.dlog, w.dgrad, w.dlap, st, qa, ecp_env, ecp_v0, ecp_vper);
+    int rc = slater(r, R, Rb, Bc, S, w.BF, w.Gadd, w.dsign, w.dlog, w.dgrad, w.dlap, st, qa, ecp_env, ecp_v0, ecp_vper,
+                    virt_layout);
     if (rc || mos_out) return rc;
     const FinalizeCfg fc = finalize_cfg(S);
     DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb,
@@ -2445,6 +2478,83 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  // <S^2> estimators (reference physics.py:159-239): every walker's virtual walkers (one up / down pair swapped each) run
+  // through the plain forward in groups of whole walkers; spin_accumulate_kernel reduces their ratios per walker.  A group
+  // whose virtual walkers do not fit the workspace at once is split across plain-forward chunks by run_batched.
+  int spin(const void* r_, const void* R_, int Rb, int B, const void* sign_, const void* logp_, int down_idx, void* s2_,
+           void* ratio_, void* ws, int64_t wsb, cudaStream_t st) override {
+    const T* r = (const T*)r_;
+    const T* R = (const T*)R_;
+    const int nd = cfg.n_down, nu = cfg.n_up;
+    if (Rb) { err = "spin: per-walker nuclei are not supported"; return 2; }
+    if (down_idx != -1 && (nd == 0 || down_idx < nu || down_idx >= N)) { err = "spin: down_idx out of range"; return 2; }
+    if (!sign_ != !logp_) { err = "spin: pass both sign and log of the walkers, or neither"; return 2; }
+    if (B < 1) return 0;
+    const int64_t Pn = down_idx < 0 ? (int64_t)nu * nd : nu;
+    const double D = nu - nd;
+    const double c0 = down_idx < 0 ? D / 2 * (D / 2 + 1) + nd : 1.0;
+    if (Pn == 0) {  // no down electrons: the constant, no forwards
+      DQ_LAUNCH(spin_accumulate_kernel<T>, dim3((B + 3) / 4), dim3(128), 0, st, (const T*)nullptr, (const T*)nullptr,
+                (const T*)nullptr, (const T*)nullptr, 0, B, c0, (T*)s2_, (T*)nullptr);
+      DQ_CHECK(cudaGetLastError());
+      return 0;
+    }
+    int64_t Be = std::min<int64_t>(B, spin_group_cap(Pn));
+    if (spin_bytes(Be, Pn) > wsb) {  // largest walker group whose virtual walkers fit the workspace
+      int64_t lo = 0, hi = Be;
+      while (hi - lo > 1) {
+        const int64_t mid = (lo + hi) / 2;
+        if (spin_bytes(mid, Pn) <= wsb) lo = mid; else hi = mid;
+      }
+      Be = lo;
+    }
+    if (Be < 1) Be = 1;  // one walker's virtual walkers do not fit at once: the plain-forward pass chunks them
+    if (spin_prefix_bytes(Be, Pn) + (int64_t)chunk_bytes(1, 1) > wsb) { err = "workspace too small for the spin pass"; return 3; }
+    for (int b0 = 0; b0 < B; b0 += (int)Be) {
+      const int nb = (int)std::min<int64_t>(Be, B - b0);
+      const int64_t V = (int64_t)nb * Pn;
+      char* p = (char*)ws;
+      T* rv = (T*)p; p += align_up(sizeof(T) * V * 3 * N);
+      T* sv = (T*)p; p += align_up(sizeof(T) * V);
+      T* lv = (T*)p; p += align_up(sizeof(T) * V);
+      T* s0 = (T*)p; p += align_up(sizeof(T) * nb);
+      T* l0 = (T*)p; p += align_up(sizeof(T) * nb);
+      T* envt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * K * N);
+      T* embt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * d);
+      note_hwm(p);
+      const T* rb = r + (size_t)b0 * 3 * N;
+      const int64_t rest = wsb - (p - (char*)ws);
+      int rc = 0;
+      if (!sign_) {
+        rc = run_batched(rb, R, 0, nb, 1, s0, l0, nullptr, nullptr, nullptr, p, rest, st);
+        if (rc) return rc;
+      }
+      const int64_t ne = V * 3 * N;
+      DQ_LAUNCH(spin_pairs_kernel<T>, dim3((unsigned)((ne + 255) / 256)), dim3(256), 0, st, rb, N, nu, down_idx, (int)Pn, ne, rv);
+      if (cfg.kind == DQMC_PSIFORMER && slater_fwd2_ok && N <= 32 && !dry) {
+        // a swapped walker differs from its base walker in two electrons: the forwards take every other electron's envelopes
+        // (slater_fwd2_kernel) and embedding rows (whole-trunk kernel) from tables of the base walkers
+        DQ_LAUNCH(env_table_kernel<T>, dim3(nb), dim3(256), sizeof(T) * N * M, st, rb, R, N, M, nu, K * N, P("env.pi_up"),
+                  P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), env_rep, envt);
+        ecp_env = envt; ecp_vper = (int)Pn; virt_layout = down_idx;
+        if (embed_fwd_ok && can_trunk(1)) {
+          DQ_LAUNCH(embed_fwd_kernel<T>, dim3((nb * N + 31) / 32), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, rb, R, 0, N, M,
+                    nu, 1, P("emb.w"), d, embt, nb * N, 32, 0LL, 0);
+          ecp_emb = embt;
+        }
+      }
+      rc = run_batched(rv, R, 0, (int)V, 1, sv, lv, nullptr, nullptr, nullptr, p, rest, st);
+      ecp_env = nullptr; ecp_emb = nullptr; virt_layout = kVirtEcp;
+      if (rc) return rc;
+      DQ_LAUNCH(spin_accumulate_kernel<T>, dim3((nb + 3) / 4), dim3(128), 0, st,
+                sign_ ? (const T*)sign_ + b0 : (const T*)s0, sign_ ? (const T*)logp_ + b0 : (const T*)l0,
+                (const T*)sv, (const T*)lv, (int)Pn, nb, c0, (T*)s2_ + b0, ratio_ ? (T*)ratio_ + (size_t)b0 * Pn : (T*)nullptr);
+      if (dry) break;  // planning pass: the first group is the largest
+    }
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
   int mcmc(void* r_, void* sign_, void* logp_, int32_t* age, void* tau_, const void* R_, int Rb, int B, int n_sub,
            double target, int max_age, uint64_t seed, uint64_t step0, uint64_t woff, const void* nn, const void* nu,
            void* stats_, void* ws, int64_t wsb, cudaStream_t st, double p_exchange, const int32_t* ex_flags,
@@ -2635,6 +2745,15 @@ int dqmc_wf_vjp_params(dqmc_handle h, const void* r, const void* R, int32_t R_ba
   if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
   return h->e->vjp_params(r, R, R_batched, n_walkers, weights, out_sign, out_log, out_grad_params, workspace, workspace_bytes,
                           (cudaStream_t)stream);
+}
+int dqmc_spin(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, const void* sign,
+              const void* log, int32_t down_idx, void* out_s2, void* out_ratio, void* workspace, int64_t workspace_bytes,
+              void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
+  return h->e->spin(r, R, R_batched, n_walkers, sign, log, down_idx, out_s2, out_ratio, workspace, workspace_bytes,
+                    (cudaStream_t)stream);
 }
 int dqmc_set_pseudo_hamiltonian(dqmc_handle h, int32_t n_tab, int32_t n_grid, double r_max, const double* tables,
                                 const int32_t* tab_of_nuc) {

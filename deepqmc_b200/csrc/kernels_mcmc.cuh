@@ -415,4 +415,45 @@ __global__ void ecp_accumulate_kernel(const T* __restrict__ r, const T* __restri
   }
 }
 
+// Virtual walkers of the spin pass: r_virt[b P + p] = r[b] with the positions of electrons a and beta of pair p swapped.
+// One thread per coordinate of r_virt.
+template <class T>
+__global__ void spin_pairs_kernel(const T* __restrict__ r, int N, int n_up, int down_idx, int P, int64_t n_elem,
+                                  T* __restrict__ r_virt) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_elem) return;
+  const int64_t v = idx / (3 * N);
+  const int e = (int)(idx - v * 3 * N), i = e / 3, c = e - 3 * i;
+  const int64_t b = v / P;
+  int a, beta;
+  spin_pair((int)(v - b * P), n_up, N, down_idx, a, beta);
+  const int src = i == a ? beta : (i == beta ? a : i);
+  r_virt[idx] = r[(b * N + src) * 3 + c];
+}
+
+// Spin estimators from the swapped forwards (reference: physics.py:159-239).  rho_p = sign' sign exp(log' - log) in fp64;
+// s2[b] = c0 - sum_p rho_p with c0 = D/2 (D/2 + 1) + n_down (exact) or 1 (spin-raising).  One WARP per walker: lane l sums
+// the pairs p = l, l + 32, ... in order, then a fixed shuffle tree -- no atomics, so a repeated call is bitwise identical.
+// P = 0 (no down electrons): s2 = c0 without reading the forwards.  ratio[B][P] (nullable) receives rho.
+template <class T>
+__global__ void spin_accumulate_kernel(const T* __restrict__ sign0, const T* __restrict__ log0, const T* __restrict__ sign_v,
+                                       const T* __restrict__ log_v, int P, int B, double c0, T* __restrict__ s2,
+                                       T* __restrict__ ratio) {
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;  // warp-uniform
+  double total = 0.0;
+  if (P > 0) {
+    const double l0 = (double)log0[b], s0 = (double)sign0[b];
+    for (int p = lane; p < P; p += 32) {
+      const size_t v = (size_t)b * P + p;
+      const double rho = (double)sign_v[v] * s0 * ::exp((double)log_v[v] - l0);
+      total += rho;
+      if (ratio) ratio[v] = (T)rho;
+    }
+  }
+  total = warp_sum(total);
+  if (lane == 0) s2[b] = (T)(c0 - total);
+}
+
 }  // namespace dq

@@ -672,7 +672,8 @@ __global__ void __launch_bounds__(256, 3)
 slater_fwd2_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M, int n_up, int K,
                    int B, const T* __restrict__ pi_up, const T* __restrict__ pi_dn, const T* __restrict__ zeta_up,
                    const T* __restrict__ zeta_dn, const T* __restrict__ BF, int ldb, T* __restrict__ det_sign,
-                   T* __restrict__ det_log, int rep, int full_det, const T* __restrict__ env_base, long long v0, int vper) {
+                   T* __restrict__ det_log, int rep, int full_det, const T* __restrict__ env_base, long long v0, int vper,
+                   int vlayout) {
   DQMC_DYN_SMEM(smem_raw);
   const int NP = N | 1, KN = K * N;
   T* As = reinterpret_cast<T*>(smem_raw);  // [K][N][NP]
@@ -689,25 +690,32 @@ slater_fwd2_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batch
     const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
     __syncthreads();  // previous walker's determinants are in registers / written
     if (env_base) {
-      // Quadrature forward of the non-local ECP: walker v0 + b is base walker (v0 + b) / vper with ONE electron moved
-      // (ecp_points_kernel: v = ((w J + j) N + i) 12 + q).  The envelopes depend on the electron's own position only, so
-      // all rows but the moved one come from the base walker's table env_base[w][i][k N + mu] (env_table_kernel): 12 M
-      // instead of N M exponentials per orbital (the envelope sums were 3/4 of this kernel's MUFU-bound first phase).
-      const long long v = v0 + b;
-      const int bw = (int)(v / vper), imv = (int)((v / 12) % N);
-      for (int m = tid; m < M; m += nt) {
+      // Compact virtual-walker forward (virtual_move, common.cuh): walker v0 + b is a base walker with one electron moved
+      // (non-local ECP quadrature) or an up / down pair swapped (spin pass).  The envelopes depend on the electron's own
+      // position and spin only, so all rows but the moved ones come from the base walker's table env_base[w][i][k N + mu]
+      // (env_table_kernel), the moved rows are evaluated afresh with the electron's own spin: 12 M (ECP) instead of N M
+      // exponentials per orbital (the envelope sums were 3/4 of this kernel's MUFU-bound first phase).
+      const VirtualMove mv = virtual_move((int)(v0 + b), vper, N, n_up, vlayout);
+      const int bw = mv.base, nmv = mv.e1 < 0 ? 1 : 2;
+      for (int idx = tid; idx < nmv * M; idx += nt) {
+        const int t = idx / M, m = idx - t * M, imv = t ? mv.e1 : mv.e0;
         const T dx0 = rb[3 * imv] - Rb[3 * m], dx1 = rb[3 * imv + 1] - Rb[3 * m + 1], dx2 = rb[3 * imv + 2] - Rb[3 * m + 2];
-        rho[m] = m_sqrt(Num<T>::eps() + dx0 * dx0 + dx1 * dx1 + dx2 * dx2);
+        rho[idx] = m_sqrt(Num<T>::eps() + dx0 * dx0 + dx1 * dx1 + dx2 * dx2);
       }
       __syncthreads();
-      const int sbm = imv >= n_up;
       for (int o = tid; o < KN; o += nt) {
         const int k = o / N, mu = o - k * N;
-        const T* pi = (sbm ? pi_dn : pi_up) + (size_t)o * M * rep;
-        const T* ze = (sbm ? zeta_dn : zeta_up) + (size_t)o * M * rep;
-        T enew = T(0);
-        for (int m = 0; m < M; ++m)
-          for (int t = 0; t < rep; ++t) enew += pi[m * rep + t] * env_exp_scaled(env_scale(-m_abs(ze[m * rep + t])) * rho[m]);
+        auto env_new = [&](int im, const T* rj) {  // envelope of orbital o for electron im (own spin) at distances rj
+          const int sbm = im >= n_up;
+          const T* pi = (sbm ? pi_dn : pi_up) + (size_t)o * M * rep;
+          const T* ze = (sbm ? zeta_dn : zeta_up) + (size_t)o * M * rep;
+          T e = T(0);
+          for (int m = 0; m < M; ++m)
+            for (int t = 0; t < rep; ++t) e += pi[m * rep + t] * env_exp_scaled(env_scale(-m_abs(ze[m * rep + t])) * rj[m]);
+          return e;
+        };
+        const T enew0 = env_new(mv.e0, rho);
+        const T enew1 = nmv > 1 ? env_new(mv.e1, rho + M) : T(0);
         const T* eb = env_base + (size_t)bw * N * KN + o;
         const T* bfp = BF + (size_t)b * N * ldb + o;
         T* arow = As + (size_t)k * N * NP + mu;
@@ -727,7 +735,9 @@ slater_fwd2_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batch
             for (int i = 0; i < cnt; ++i, ep += KN, bp += ldb, ap += NP) *ap = *ep * *bp;
           }
         }
-        if (full_det || ((imv < n_up) == mu_up)) arow[imv * NP] = enew * bfp[(size_t)imv * ldb];  // the moved electron's row
+        // the moved electrons' rows
+        if (full_det || ((mv.e0 < n_up) == mu_up)) arow[mv.e0 * NP] = enew0 * bfp[(size_t)mv.e0 * ldb];
+        if (nmv > 1 && (full_det || ((mv.e1 < n_up) == mu_up))) arow[mv.e1 * NP] = enew1 * bfp[(size_t)mv.e1 * ldb];
       }
     } else {
     for (int idx = tid; idx < 2 * M * NS; idx += nt) {

@@ -39,10 +39,11 @@ constexpr int kTrScratchPerCta = kTrQkvBytes + 128 * 256 * 4;  // + residual str
 using TrSmem = MlpSmem;
 
 struct TrunkParams {
-  const float* X0; int ldx;      // embedding rows [rows][256]  (vper > 0: [walkers][256], the moved electron's row only)
-  const float* Xbase;            // vper > 0 (non-local-ECP quadrature forwards): embedding rows of the group's base walkers
-  long long v0; int vper;        //   [base][N][256]; walker w of this launch is virtual walker v0 + w = base (v0 + w) / vper
-                                 //   with electron ((v0 + w) / 12) % N moved (ecp_points_kernel layout)
+  const float* X0; int ldx;      // embedding rows [rows][256]  (vper > 0, ECP layout: [walkers][256], the moved electron's row)
+  const float* Xbase;            // vper > 0 (compact virtual-walker forwards): embedding rows of the group's base walkers
+  long long v0; int vper;        //   [base][N][256]; walker w of this launch is virtual walker v0 + w, whose base walker and
+  int n_up, vlayout;             //   moved electrons virtual_move(v0 + w, vper, N, n_up, vlayout) gives (common.cuh)
+  const float* wspin;            // swap layout: embedding weights of the +-1 spin feature [256]
   float* Out; int ldout;         // trunk output rows [rows][256]
   const CUtensorMap* maps;       // device array [L][4][2]: (Wqkv, Wo, W1, W2) x (hi, lo); boxes of 32 halves x 256 rows
   const float* b1[kTrMaxLayers];
@@ -105,12 +106,24 @@ trunk_f16_kernel(TrunkParams p) {
         x[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (row >= 0) {
           const float* xrow = p.X0 + (size_t)row * p.ldx;
+          float sw = 0.f;
           if (p.vper > 0) {
-            const int walker = (int)(row / N), el = (int)(row % N);
-            const long long v = p.v0 + walker;
-            xrow = el == (int)((v / 12) % N) ? p.X0 + (size_t)walker * p.ldx : p.Xbase + ((size_t)(v / p.vper) * N + el) * p.ldx;
+            const int walker = tile * G + (r >> lnp), el = r & (NP - 1);
+            const VirtualMove mv = virtual_move((int)p.v0 + walker, p.vper, N, p.n_up, p.vlayout);
+            if (mv.e1 < 0) {  // ECP: the moved electron's row is new
+              xrow = el == mv.e0 ? p.X0 + (size_t)walker * p.ldx : p.Xbase + ((size_t)mv.base * N + el) * p.ldx;
+            } else {  // spin swap: up electron e0 sits at r_e1 and down electron e1 at r_e0, each with its own spin:
+                      // emb(r, +-1) = emb(r, -+1) +- 2 w_spin
+              const int src = el == mv.e0 ? mv.e1 : (el == mv.e1 ? mv.e0 : el);
+              xrow = p.Xbase + ((size_t)mv.base * N + src) * p.ldx;
+              sw = el == mv.e0 ? 2.f : (el == mv.e1 ? -2.f : 0.f);
+            }
           }
           x[i] = __ldg((const float4*)(xrow + c));
+          if (sw != 0.f) {
+            const float4 ws = __ldg((const float4*)(p.wspin + c));
+            x[i].x += sw * ws.x; x[i].y += sw * ws.y; x[i].z += sw * ws.z; x[i].w += sw * ws.w;
+          }
         }
       }
 #pragma unroll

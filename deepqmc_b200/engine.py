@@ -14,7 +14,7 @@ from . import _lib
 from . import params as PN
 from .spec import AnsatzSpec
 
-MODE_FORWARD, MODE_LOCAL_ENERGY, MODE_VJP, MODE_MCMC, MODE_LANGEVIN = 0, 1, 2, 3, 4
+MODE_FORWARD, MODE_LOCAL_ENERGY, MODE_VJP, MODE_MCMC, MODE_LANGEVIN, MODE_SPIN = 0, 1, 2, 3, 4, 5
 _TORCH_DTYPE = {0: torch.float64, 1: torch.float32}
 
 
@@ -577,6 +577,27 @@ class Engine:
                 v = v.to(device=self.device, dtype=self.dtype)
                 grads[k] = grads[k] + v.reshape(grads[k].shape) if k in grads else v
         return sign, log, grads
+
+    def spin(self, r, R, sign=None, log=None, down_idx=-1, want_ratios=False, max_ws_bytes=None):
+        """-> (s2[B], ratios[B, P] or None).  down_idx = -1: exact <S^2> per walker over all n_up n_down swaps (P = n_up n_down,
+        p = a n_down + (b - n_up)); down_idx in [n_up, N): the spin-raising contribution of that down electron (P = n_up,
+        p = a).  sign / log of the walkers are optional (computed inside the call when missing)
+        (reference: physics.py:159-239; dqmc_spin)."""
+        r = self._prep(r)
+        B = r.shape[0]
+        R, Rb = self._R(R, B)
+        n_up, n_down = self.spec.n_up, self.spec.n_down
+        P = n_up * n_down if down_idx < 0 else n_up
+        s2 = torch.empty(B, dtype=self.dtype, device=self.device)
+        ratio = torch.empty(B, P, dtype=self.dtype, device=self.device) if want_ratios else None
+        sg = self._prep(sign) if sign is not None else None
+        lg = self._prep(log) if log is not None else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        ws = self.workspace(B, MODE_SPIN, max_ws_bytes)
+        rc = self.lib.dqmc_spin(self.h, r.data_ptr(), R.data_ptr(), Rb, B, ptr(sg), ptr(lg), int(down_idx), s2.data_ptr(),
+                                ptr(ratio), ws.data_ptr(), ws.numel(), self._stream())
+        self._check(rc, 'dqmc_spin')
+        return s2, ratio
 
     def mcmc_sweep(self, state, R, n_sub, target_acceptance=0.57, max_age=None, seed=0, step0=0, walker_offset=0,
                    noise_normal=None, noise_uniform=None, max_ws_bytes=None, exchange_probability=0.0, exchange_flags=None,

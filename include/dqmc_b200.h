@@ -30,7 +30,8 @@ extern "C" {
 enum { DQMC_PSIFORMER = 0, DQMC_FERMINET = 1, DQMC_TRANSPSIFORMER = 2, DQMC_PAULINET = 3 };
 enum { DQMC_F64 = 0, DQMC_F32 = 1 };
 enum { DQMC_GEMM_SIMT = 0, DQMC_GEMM_TCGEN05 = 1 };
-enum { DQMC_MODE_FORWARD = 0, DQMC_MODE_LOCAL_ENERGY = 1, DQMC_MODE_VJP = 2, DQMC_MODE_MCMC = 3, DQMC_MODE_LANGEVIN = 4 };
+enum { DQMC_MODE_FORWARD = 0, DQMC_MODE_LOCAL_ENERGY = 1, DQMC_MODE_VJP = 2, DQMC_MODE_MCMC = 3, DQMC_MODE_LANGEVIN = 4,
+       DQMC_MODE_SPIN = 5 };
 
 /* Ansatz + Hamiltonian constants that fix the kernel shapes.
  * reference: src/deepqmc/conf/ansatz/psiformer.yaml, ferminet.yaml (SURVEY.md 8(a0));
@@ -187,6 +188,26 @@ int dqmc_langevin_sweep(dqmc_handle h, void* r, void* sign, void* log, void* for
 int dqmc_wf_vjp_params(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers,
                        const void* weights, void* out_sign, void* out_log, void* out_grad_params, void* workspace,
                        int64_t workspace_bytes, void* stream);
+
+/* Total spin <S^2> per walker -> out_s2[B].
+ *   down_idx = -1: exact estimator over all n_up n_down (up a, down b) pairs,
+ *                  s2 = D/2 (D/2 + 1) + n_down - sum_{a,b} rho_ab,  D = n_up - n_down;
+ *   down_idx in [n_up, N): spin-raising contribution 1 - sum_a rho_{a,down_idx}.
+ * rho = sign' sign exp(log' - log), (sign', log') = psi with the positions of a and b swapped, formed and summed in fp64
+ * in a fixed order (a repeated call is bitwise identical).  sign / log [B] of the base walkers are given together or both
+ * null (null: a plain forward inside the call; exactly one of them: status 2).  out_ratio [B][P] (nullable) receives rho:
+ * P = n_up n_down with p = a n_down + (b - n_up), or P = n_up with p = a.  Every swapped walker is one plain forward.
+ * Psiformer engines take the N - 2 unmoved electrons' envelope rows (slater_fwd2_kernel) and embedding rows (whole-trunk
+ * kernel; the two swapped rows are formed from the table as emb(r, +-1) = emb(r, -+1) +- 2 w_spin) from tables of the base
+ * walkers; the other kinds run dqmc_wf_forward's path on the swapped walkers.  Walkers are grouped to fit the workspace,
+ * one walker's pairs split across forward chunks if need be.  n_walkers = 0 is a no-op; n_down = 0 gives the constant
+ * D/2 (D/2 + 1) without forwards (and needs no workspace) for down_idx = -1, and status 2 otherwise.  Status 2 also for
+ * down_idx out of range and for R_batched = 1.  Workspace: dqmc_workspace_bytes(h, B, DQMC_MODE_SPIN).
+ * replaces: physics.py:159-239 evaluate_spin / make_stochastic_spin_raising_operator (observable.py:193-200 SpinMonitor,
+ *           loss/spin.py). */
+int dqmc_spin(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, const void* sign,
+              const void* log, int32_t down_idx, void* out_s2, void* out_ratio, void* workspace, int64_t workspace_bytes,
+              void* stream);
 
 /* Switch the handle's Hamiltonian to a pseudo-Hamiltonian (fully local replacement of the semi-local ECP):
  * tables[n_tab][2][n_grid] (host, fp64) = r V_loc(r) and r V_L2(r) per tabulated element on the uniform grid
