@@ -22,7 +22,7 @@ SYMBOLS = [
     'dqmc_set_pseudo_hamiltonian', 'dqmc_wf_orbitals', 'dqmc_mcmc_sweep_exchange',
     'dqmc_workspace_bytes_min', 'dqmc_debug_plan', 'dqmc_stats_pack', 'dqmc_debug_mlp_block', 'dqmc_debug_trunk',
     'dqmc_profile_end_classes', 'dqmc_debug_trunk_phases', 'dqmc_debug_attention', 'dqmc_debug_mlp',
-    'dqmc_debug_slater', 'dqmc_debug_det_sum', 'dqmc_spin',
+    'dqmc_debug_slater', 'dqmc_debug_det_sum', 'dqmc_spin', 'dqmc_ecp_forward_count',
 ]
 
 
@@ -102,6 +102,8 @@ def load(path: str | None = None) -> C.CDLL:
     lib.dqmc_set_pseudo_hamiltonian.argtypes = [vp, i32, i32, C.c_double, C.POINTER(C.c_double), C.POINTER(i32)]
     lib.dqmc_launch_count.argtypes = [vp]
     lib.dqmc_launch_count.restype = i64
+    lib.dqmc_ecp_forward_count.argtypes = [vp]
+    lib.dqmc_ecp_forward_count.restype = i64
     lib.dqmc_profile_begin.argtypes = [vp]
     lib.dqmc_debug_gemm.argtypes = [vp, C.c_char_p, C.c_char_p, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.dqmc_profile_end.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(i64)]

@@ -102,25 +102,39 @@ __host__ __device__ __forceinline__ void spin_pair(int p, int n_up, int N, int d
   }
 }
 
-// Compact virtual-walker forwards: virtual walker v is base walker v / vper with one or two electrons moved; the consumers
+// Non-local ECP cutoff: the (electron, ECP nucleus) pair at squared distance d2 runs its 12 quadrature forwards unless d2 exceeds
+// rc2, the nucleus' squared cutoff radius (engine.cu ecp_cutoff_rc2: beyond it sum_l (2l+1) sum_t |beta_lt| exp(-alpha_lt d2)
+// < 2^-100).  d2 in double, as ecp_accumulate_kernel weights the pair; the pair list builder (ecp_pairs_kernel) and the
+// accumulator both decide here.  A NaN distance keeps its pair, so rc2 = +inf (DQMC_ECP_CUTOFF=0) keeps every pair of every walker.
+template <class T>
+__host__ __device__ __forceinline__ bool ecp_pair_active(const T* ri, const T* RI, double rc2, double& d2) {
+  const double dx = (double)ri[0] - (double)RI[0], dy = (double)ri[1] - (double)RI[1], dz = (double)ri[2] - (double)RI[2];
+  d2 = dx * dx + dy * dy + dz * dz;
+  return !(d2 > rc2);
+}
+
+// Compact virtual-walker forwards: virtual walker v is a base walker with one or two electrons moved; the consumers
 // (embed_fwd_kernel, the whole-trunk kernel's tile load, slater_fwd2_kernel) take every other electron's rows from tables of
 // the base walkers.  Two layouts:
-//   layout == kVirtEcp: non-local ECP quadrature (ecp_points_kernel, v = ((w J + j) N + i) 12 + q): electron e0 = (v / 12) % N
-//     moved to a quadrature point, e1 = -1;
-//   layout >= -1: spin swaps (spin_pairs_kernel, v = w vper + p): up electron e0 and down electron e1 of pair p exchange
-//     positions; layout is the down_idx of spin_pair (-1: all pairs).
+//   layout == kVirtEcp: non-local ECP quadrature (ecp_points_kernel, v = 12 a + q): active pair a of the group's pair list
+//     (ecp_pairs_kernel) is p = pairs[a] = (w J + j) N + i, vper = 12 J N; base walker w = p / (J N), electron e0 = p % N moved
+//     to a quadrature point, e1 = -1;
+//   layout >= -1: spin swaps (spin_pairs_kernel, v = w vper + p): base walker v / vper, up electron e0 and down electron e1 of
+//     pair p exchange positions; layout is the down_idx of spin_pair (-1: all pairs); pairs is unused.
 constexpr int kVirtEcp = -2;
 // Virtual-walker indices are 32-bit: a group's virtual walkers are one plain-forward batch (int walker count).
 struct VirtualMove {
   int base, e0, e1;
 };
-__host__ __device__ __forceinline__ VirtualMove virtual_move(int v, int vper, int N, int n_up, int layout) {
+__host__ __device__ __forceinline__ VirtualMove virtual_move(int v, int vper, int N, int n_up, int layout, const int* pairs) {
   VirtualMove m;
-  m.base = v / vper;
   if (layout == kVirtEcp) {
-    m.e0 = (v / 12) % N;
+    const int p = pairs[v / 12];
+    m.base = p / (vper / 12);
+    m.e0 = p % N;
     m.e1 = -1;
   } else {
+    m.base = v / vper;
     spin_pair(v - m.base * vper, n_up, N, layout, m.e0, m.e1);
   }
   return m;

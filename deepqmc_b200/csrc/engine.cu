@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <map>
 #include <mutex>
 #include <string>
@@ -35,11 +36,42 @@ struct ParamEntry {
 
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
+// Squared cutoff radius of one non-local ECP nucleus, nl[l][alpha | beta][t] as the accumulator reads it: the largest d2 with
+// w(d2) = sum_l (2l+1) sum_t |beta_lt| exp(-alpha_lt d2) >= 2^-100.  A pair's term in V_nl is at most w(d2) max_q |psi ratio|
+// (sum_q |P_l(cos th_q)| <= 12), so the pairs beyond it are skipped (common.cuh ecp_pair_active).  w falls monotonically
+// when every alpha with beta != 0 is positive, and the bisection runs to adjacent doubles.  +inf: no cutoff (on == false,
+// DQMC_ECP_CUTOFF=0, or a term that does not decay).
+template <class T>
+static double ecp_cutoff_rc2(const T* nl, int L, int Tn, bool on) {
+  const double inf = std::numeric_limits<double>::infinity(), eps = std::ldexp(1.0, -100);
+  if (!on) return inf;
+  for (int l = 0; l < L; ++l)
+    for (int t = 0; t < Tn; ++t)
+      if ((double)nl[(l * 2 + 1) * Tn + t] != 0.0 && !((double)nl[(l * 2) * Tn + t] > 0.0)) return inf;
+  auto w = [&](double d2) {
+    double s = 0.0;
+    for (int l = 0; l < L; ++l)
+      for (int t = 0; t < Tn; ++t)
+        s += (2 * l + 1) * std::fabs((double)nl[(l * 2 + 1) * Tn + t]) * std::exp(-(double)nl[(l * 2) * Tn + t] * d2);
+    return s;
+  };
+  if (w(0.0) < eps) return -inf;  // no pair is ever active
+  double lo = 0.0, hi = 1.0;
+  while (w(hi) >= eps) { lo = hi; hi *= 2; }
+  for (;;) {
+    const double mid = lo + 0.5 * (hi - lo);
+    if (mid <= lo || mid >= hi) break;
+    (w(mid) >= eps ? lo : hi) = mid;
+  }
+  return lo;
+}
+
 struct EngineBase {
   dqmc_config cfg;
   int device = 0;
   std::string err;
   int64_t launches = 0;
+  int64_t ecp_forwards = 0;  // quadrature virtual walkers run by the non-local ECP pass (12 per active pair)
   std::vector<ParamEntry> entries;
   int64_t total = 0;
   // Planning pass: the host code of an entry point is walked with every CUDA call skipped, so that the number of workspace
@@ -313,6 +345,7 @@ struct Engine : EngineBase {
   T* d_ecp_loc = nullptr;
   T* d_nl_params = nullptr;
   int* d_nl_nuc = nullptr;
+  double* d_nl_rc2 = nullptr;  // [J] squared cutoff radius of each non-local nucleus slot (ecp_cutoff_rc2)
   int J = 0;  // nuclei with a non-local channel
   // pseudo-Hamiltonian (reference ecp/pseudo_hamiltonian.py): tables r V_loc / r V_L2 per element on a uniform grid
   T* d_ph_tabs = nullptr;
@@ -361,6 +394,7 @@ struct Engine : EngineBase {
   int64_t ecp_v0 = 0;
   int ecp_vper = 0;
   int virt_layout = kVirtEcp;
+  const int* ecp_pairs = nullptr;  // the ECP group's active-pair list (ecp_pairs_kernel) of virtual_move's ECP layout
 #if !defined(DQMC_NO_TCGEN05)
   struct TcWeight {
     float* hi = nullptr; float* lo = nullptr; CUtensorMap mh, ml; int N = 0, K = 0;
@@ -494,6 +528,12 @@ struct Engine : EngineBase {
         DQ_CHECK(cudaMemcpy(d_nl_params, np.data(), sizeof(T) * np.size(), cudaMemcpyHostToDevice));
         DQ_CHECK(cudaMalloc((void**)&d_nl_nuc, sizeof(int) * J));
         DQ_CHECK(cudaMemcpy(d_nl_nuc, nuc.data(), sizeof(int) * J, cudaMemcpyHostToDevice));
+        const char* ev = std::getenv("DQMC_ECP_CUTOFF");
+        const bool cutoff = !(ev && std::atoi(ev) == 0);
+        std::vector<double> rc2(J);
+        for (int j = 0; j < J; ++j) rc2[j] = ecp_cutoff_rc2(np.data() + (size_t)nuc[j] * L * 2 * Tn, L, Tn, cutoff);
+        DQ_CHECK(cudaMalloc((void**)&d_nl_rc2, sizeof(double) * J));
+        DQ_CHECK(cudaMemcpy(d_nl_rc2, rc2.data(), sizeof(double) * J, cudaMemcpyHostToDevice));
       }
     }
 #ifndef DQMC_EMU
@@ -609,6 +649,7 @@ struct Engine : EngineBase {
     if (d_ecp_loc) cudaFree(d_ecp_loc);
     if (d_nl_params) cudaFree(d_nl_params);
     if (d_nl_nuc) cudaFree(d_nl_nuc);
+    if (d_nl_rc2) cudaFree(d_nl_rc2);
     if (d_ph_tabs) cudaFree(d_ph_tabs);
     if (d_ph_nuc) cudaFree(d_ph_nuc);
 #if !defined(DQMC_NO_TCGEN05)
@@ -794,12 +835,15 @@ struct Engine : EngineBase {
     return (int)lo;
   }
   // non-local ECP pass for nb walkers: virtual walkers r_virt[V][N][3], sign[V], log[V] + one
-  // forward chunk over all V = nb * J * N * 12 virtual walkers
+  // forward chunk over all V = nb * J * N * 12 virtual walkers.  Sized for every pair active, so the
+  // plan does not depend on the walkers; the cutoff only shortens the list the forwards run over.
   int64_t ecp_prefix_bytes(int64_t nb) const {
     const int64_t V = nb * J * N * 12;
     return (int64_t)align_up(sizeof(T) * V * 3 * N) + 2 * (int64_t)align_up(sizeof(T) * V) +
            (int64_t)align_up(sizeof(T) * nb * N * K * N) +  // + envelope table of the group's base walkers
-           (int64_t)align_up(sizeof(T) * nb * N * d);        // + their embedding rows
+           (int64_t)align_up(sizeof(T) * nb * N * d) +      // + their embedding rows
+           (int64_t)align_up(sizeof(int) * nb * J * N) +    // + active-pair list
+           (int64_t)align_up(sizeof(int) * (nb + 1));       // + per-walker offsets into it, pair count
   }
   // walkers per ECP group are bounded by the 32-bit row cap of the plain-forward chunk: the plan never asks for more
   int64_t ecp_group_cap() const {
@@ -1069,7 +1113,7 @@ struct Engine : EngineBase {
       tc::TrunkParams p;
       p.X0 = X0; p.ldx = d; p.Out = Out; p.ldout = d; p.maps = d_trunk_maps; p.scratch = d_trunk_scratch;
       p.Xbase = Xbase; p.v0 = Xbase ? (long long)ecp_v0 : 0; p.vper = Xbase ? ecp_vper : 0;
-      p.n_up = cfg.n_up; p.vlayout = virt_layout; p.wspin = P("emb.w") + (size_t)(4 * M) * d;  // the +-1 spin feature's row
+      p.n_up = cfg.n_up; p.vlayout = virt_layout; p.pairs = ecp_pairs; p.wspin = P("emb.w") + (size_t)(4 * M) * d;  // the +-1 spin feature's row
       int np2 = 1;
       while (np2 < N) np2 *= 2;  // walker slot of the tile: electrons rounded up to a power of two (<= 32)
       p.walkers = rows / N; p.N = N; p.NP = np2; p.L = cfg.n_layers; p.a_scale = kActScale;
@@ -1167,7 +1211,7 @@ struct Engine : EngineBase {
       rc = 1;
     }
     if (!rc) rc = slater((const T*)r, (const T*)R, 0, Bc, S, bf, gadd, (T*)dsign, (T*)dlog, (T*)dgrad, (T*)dlap, st, nullptr,
-                         nullptr, 0, 0, kVirtEcp, kernel);
+                         nullptr, 0, 0, kVirtEcp, nullptr, kernel);
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { err = "debug_slater: kernel failed"; rc = 1; }
     cudaFree(bf);
     cudaFree(gadd);
@@ -1579,14 +1623,14 @@ struct Engine : EngineBase {
       int epb = (Bc / (2 * n_sms)) / 32 * 32;
       epb = epb < 32 ? 32 : (epb > 512 ? 512 : epb);
       DQ_LAUNCH(embed_fwd_kernel<T>, dim3((Bc + epb - 1) / epb), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, r, R, Rb, N,
-                M, cfg.n_up, 1, P("emb.w"), d, w.X, Bc, epb, (long long)ecp_v0, ecp_vper);
+                M, cfg.n_up, 1, P("emb.w"), d, w.X, Bc, epb, (long long)ecp_v0, ecp_vper, ecp_pairs);
     } else if (S == 1 && embed_fwd_ok) {
       // plain forwards (Metropolis, ECP quadrature): register-tiled projection, W staged per block
       const int tot = Bc * N;
       int epb = (tot / (2 * n_sms)) / 32 * 32;
       epb = epb < 32 ? 32 : (epb > 512 ? 512 : epb);
       DQ_LAUNCH(embed_fwd_kernel<T>, dim3((tot + epb - 1) / epb), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, r, R, Rb, N,
-                M, cfg.n_up, 1, P("emb.w"), d, w.X, tot, epb, 0LL, 0);
+                M, cfg.n_up, 1, P("emb.w"), d, w.X, tot, epb, 0LL, 0, (const int*)nullptr);
     } else {
       const int epb = S == 1 ? 8 : 1;  // plain forwards: several electrons per block (tiny per-electron work)
       DQ_LAUNCH(embed_kernel<T>, dim3((Bc * N + epb - 1) / epb), dim3(128), sizeof(T) * 5 * F, st, r, R, Rb, N, M,
@@ -1619,7 +1663,7 @@ struct Engine : EngineBase {
   // template instance NS / NM, 0 for the runtime-N kernels}.  The forward tails and dqmc_debug_slater both call this.
   int slater(const T* r, const T* R, int Rb, int Bc, int S, T* BF, T* Gadd, T* dsign, T* dlog, T* dgrad, T* dlap,
              cudaStream_t st, const T* qa, const T* env_base, int64_t v0, int vper, int vlayout = kVirtEcp,
-             int32_t* kernel = nullptr) {
+             const int* pairs = nullptr, int32_t* kernel = nullptr) {
     if (cfg.mult_act == 1)  // default mult_act 1 + 2 tanh(x / 4) of the BackflowOp (nn_wave_function.py:14-33)
       DQ_LAUNCH(act_fl_kernel<T>, dim3(Bc * N, (KN + 127) / 128), dim3(128), 0, st, BF, KN, (const T*)nullptr, 0, S, KN, T(1), 2);
     const int full_det = cfg.factorized_det ? 0 : 1;
@@ -1669,7 +1713,7 @@ struct Engine : EngineBase {
   inst = NMV;                                                                                                                  \
   DQ_LAUNCH((slater_fwd2_kernel<T, NMV>), dim3(grid), dim3(nthr), slater_fwd2_smem_bytes<T>(N, M, K), st, r, R, Rb, N, M,      \
             cfg.n_up, K, Bc, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, dsign,     \
-            dlog, env_rep, full_det, env_base, (long long)v0, vper, vlayout)
+            dlog, env_rep, full_det, env_base, (long long)v0, vper, vlayout, pairs)
       if (N == 14) { DQ_SL_FWD2(14); }
       else if (N <= 16) { DQ_SL_FWD2(16); }
       else if (N == 28) { DQ_SL_FWD2(28); }
@@ -1707,7 +1751,7 @@ struct Engine : EngineBase {
     gemm(X, bf_in, "bf.up", "bf.dn", cfg.n_up, BFW, gnn ? P("bfb.up") : nullptr, nullptr, 0, w.BF, BFW, Bc * S, BFW, bf_in, S, 1, N,
          st, 0, gnn ? P("bfb.dn") : nullptr);
     int rc = slater(r, R, Rb, Bc, S, w.BF, w.Gadd, w.dsign, w.dlog, w.dgrad, w.dlap, st, qa, ecp_env, ecp_v0, ecp_vper,
-                    virt_layout);
+                    virt_layout, ecp_pairs);
     if (rc || mos_out) return rc;
     const FinalizeCfg fc = finalize_cfg(S);
     DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb,
@@ -2445,30 +2489,44 @@ struct Engine : EngineBase {
         T* lv = (T*)p; p += align_up(sizeof(T) * V);
         T* envt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * K * N);
         T* embt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * d);
+        int* pairs = (int*)p; p += align_up(sizeof(int) * (size_t)nb * J * N);
+        int* offs = (int*)p; p += align_up(sizeof(int) * (size_t)(nb + 1));
         note_hwm(p);
+        if (Rb) { err = "non-local ECP with per-walker nuclei is not supported"; return 2; }
         const T* rb = r + (size_t)b0 * 3 * N;
         const T* Rbp = R + (Rb ? (size_t)b0 * 3 * M : 0);
         const T* tw = twist ? (const T*)twist + (size_t)b0 * J * N : nullptr;
-        DQ_LAUNCH(ecp_points_kernel<T>, dim3(nb * J * N), dim3(64), 0, st, rb, Rbp, Rb, N, M, J, (const int*)d_nl_nuc, tw,
-                  seed, (uint64_t)b0, rv);
-        if (Rb) { err = "non-local ECP with per-walker nuclei is not supported"; return 2; }
+        // the pairs inside the cutoff radius; the group's quadrature forwards run over them alone
+        DQ_LAUNCH(ecp_pairs_kernel<T>, dim3(1), dim3(1024), 0, st, rb, Rbp, Rb, N, M, J, (const int*)d_nl_nuc,
+                  (const double*)d_nl_rc2, nb, offs, pairs, offs + nb);
+        int n_act = nb * J * N;  // the planning pass sizes every buffer for all pairs
+        if (!dry) {
+          DQ_CHECK(cudaMemcpyAsync(&n_act, offs + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+          DQ_CHECK(cudaStreamSynchronize(st));
+          ecp_forwards += (int64_t)n_act * 12;
+        }
+        V = (int64_t)n_act * 12;
+        if (n_act > 0)
+          DQ_LAUNCH(ecp_points_kernel<T>, dim3(n_act), dim3(64), 0, st, rb, Rbp, Rb, N, M, J, (const int*)d_nl_nuc, tw,
+                    seed, (uint64_t)b0, (const int*)pairs, rv);
         const bool use_table = slater_fwd2_ok && N <= 32 && !dry && !std::getenv("DQMC_ECP_ENV_TABLE_OFF");
         if (use_table) {  // the quadrature forwards take the unmoved electrons' envelopes from the base walkers' table
           DQ_LAUNCH(env_table_kernel<T>, dim3(nb), dim3(256), sizeof(T) * N * M, st, rb, R, N, M, cfg.n_up, K * N,
                     P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), cfg.n_env_per_nuc > 1 ? cfg.n_env_per_nuc : 1,
                     envt);
-          ecp_env = envt; ecp_vper = (int)vper;
+          ecp_env = envt; ecp_vper = (int)vper; ecp_pairs = pairs;
           if (embed_fwd_ok && can_trunk(1) && !std::getenv("DQMC_ECP_EMB_TABLE_OFF")) {
             DQ_LAUNCH(embed_fwd_kernel<T>, dim3((nb * N + 31) / 32), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, rb, R, 0, N, M,
-                      cfg.n_up, 1, P("emb.w"), d, embt, nb * N, 32, 0LL, 0);
+                      cfg.n_up, 1, P("emb.w"), d, embt, nb * N, 32, 0LL, 0, (const int*)nullptr);
             ecp_emb = embt;
           }
         }
-        rc = run_batched(rv, R, 0, (int)V, 1, sv, lv, nullptr, nullptr, nullptr, p, wsb - (p - (char*)ws), st);
-        ecp_env = nullptr; ecp_emb = nullptr;
+        if (V > 0) rc = run_batched(rv, R, 0, (int)V, 1, sv, lv, nullptr, nullptr, nullptr, p, wsb - (p - (char*)ws), st);
+        ecp_env = nullptr; ecp_emb = nullptr; ecp_pairs = nullptr;
         if (rc) return rc;
         DQ_LAUNCH(ecp_accumulate_kernel<T>, dim3((nb + 3) / 4), dim3(128), 0, st, rb, Rbp, Rb, N, M, J,
-                  (const int*)d_nl_nuc, (const T*)d_nl_params, cfg.ecp_nl_lmax_p1, cfg.ecp_nl_terms,
+                  (const int*)d_nl_nuc, (const T*)d_nl_params, (const double*)d_nl_rc2, (const int*)offs,
+                  cfg.ecp_nl_lmax_p1, cfg.ecp_nl_terms,
                   (const T*)sign + b0, (const T*)logp + b0, (const T*)sv, (const T*)lv, nb, B, (T*)E + b0,
                   (T*)stats + b0);
         if (dry) break;  // planning pass: the first group is the largest
@@ -2539,7 +2597,7 @@ struct Engine : EngineBase {
         ecp_env = envt; ecp_vper = (int)Pn; virt_layout = down_idx;
         if (embed_fwd_ok && can_trunk(1)) {
           DQ_LAUNCH(embed_fwd_kernel<T>, dim3((nb * N + 31) / 32), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, rb, R, 0, N, M,
-                    nu, 1, P("emb.w"), d, embt, nb * N, 32, 0LL, 0);
+                    nu, 1, P("emb.w"), d, embt, nb * N, 32, 0LL, 0, (const int*)nullptr);
           ecp_emb = embt;
         }
       }
@@ -2774,6 +2832,7 @@ int dqmc_stats_pack(dqmc_handle h, const void* E_loc, const void* stats, int32_t
   return h->e->stats_pack(E_loc, stats, n_walkers, out11, (cudaStream_t)stream);
 }
 int64_t dqmc_launch_count(dqmc_handle h) { return h ? h->e->launches : -1; }
+int64_t dqmc_ecp_forward_count(dqmc_handle h) { return h ? h->e->ecp_forwards : -1; }
 
 int dqmc_debug_gemm(dqmc_handle h, const char* weight, const char* bias, const void* A, const void* Res, void* C,
                     int32_t rows, int32_t S, int32_t sliced, int32_t backend, void* stream) {

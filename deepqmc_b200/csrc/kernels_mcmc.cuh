@@ -307,9 +307,10 @@ __global__ void stats_pack_kernel(const T* __restrict__ E, const T* __restrict__
 // ------------------------------------------------------------------------------------------
 // Non-local ECP: 12-point icosahedron quadrature, rotated onto r_i - R_I with a random twist
 // about the local z axis.  reference: src/deepqmc/ecp/ecp_utils.py:24-60,
-// gaussian_type_ecp.py:161-255.  One block per (walker b, ecp nucleus slot j, electron i);
-// writes 12 virtual walkers r_virt[v][N][3], v = ((b*J + j)*N + i)*12 + q.
-// phi: injected twists [B][J][N] in [0, pi/5) or nullptr -> Philox.
+// gaussian_type_ecp.py:161-255.  One block per active pair a of the group (ecp_pairs_kernel): pair p = pairs[a] =
+// (b*J + j)*N + i (walker b, ecp nucleus slot j, electron i); writes 12 virtual walkers r_virt[v][N][3], v = a*12 + q.
+// phi: injected twists [B][J][N] in [0, pi/5) or nullptr -> Philox.  Twist and Philox counter belong to the pair (b, j, i),
+// not to its place in the list: a pair's quadrature points do not depend on which other pairs are active.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void ico_vertex(int q, double& th, double& ph) {
   const double pi = 3.141592653589793, at2 = 1.1071487177940904;  // atan(2)
@@ -325,10 +326,10 @@ __device__ __forceinline__ void ico_vertex(int q, double& th, double& ph) {
 template <class T>
 __global__ void ecp_points_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M,
                                   int J, const int* __restrict__ nl_nuc, const T* __restrict__ phi, uint64_t seed,
-                                  uint64_t walker_offset, T* __restrict__ r_virt) {
+                                  uint64_t walker_offset, const int* __restrict__ pairs, T* __restrict__ r_virt) {
   __shared__ double pts[12][3];
-  const int blk = blockIdx.x;
-  const int i = blk % N, j = (blk / N) % J, b = blk / (N * J);
+  const int blk = blockIdx.x, pr = pairs[blk];
+  const int i = pr % N, j = (pr / N) % J, b = pr / (N * J);
   const T* rb = r + (size_t)b * 3 * N;
   const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
   const int I = nl_nuc[j];
@@ -368,13 +369,78 @@ __global__ void ecp_points_kernel(const T* __restrict__ r, const T* __restrict__
   }
 }
 
+// Active (nucleus, electron) pairs of a group of B walkers (ecp_pair_active, common.cuh), in the order walker, nucleus slot,
+// electron: pairs[] = the group-local pair indices (b J + j) N + i, offs[b] = the walker's first entry, *total = the count.
+// One block: warp w counts walkers w, w + 32, ... (ballot per 32 pairs), a block scan turns the counts into offsets, the
+// warps write their walkers' pairs at the ballot ranks.  The list is a subsequence of all B J N pairs in their natural order.
+template <class T>
+__global__ void __launch_bounds__(1024)
+ecp_pairs_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M, int J,
+                 const int* __restrict__ nl_nuc, const double* __restrict__ rc2, int B, int* __restrict__ offs,
+                 int* __restrict__ pairs, int* __restrict__ total) {
+  __shared__ int wsum[32];
+  __shared__ int carry;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5, JN = J * N;
+  auto active = [&](int b, int p) {
+    if (p >= JN) return false;
+    const int j = p / N, i = p - j * N, I = nl_nuc[j];
+    const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
+    double d2;
+    return ecp_pair_active(r + ((size_t)b * N + i) * 3, Rb + 3 * I, rc2[j], d2);
+  };
+  for (int b = warp; b < B; b += nw) {
+    int cnt = 0;
+    for (int p0 = 0; p0 < JN; p0 += 32) cnt += __popc(__ballot_sync(0xffffffffu, active(b, p0 + lane)));
+    if (lane == 0) offs[b] = cnt;
+  }
+  if (tid == 0) carry = 0;
+  for (int base = 0; base < B; base += blockDim.x) {  // exclusive scan of offs[0 .. B) in place
+    __syncthreads();  // counts written / previous round's carry and wsum read
+    const int idx = base + tid;
+    const int c = idx < B ? offs[idx] : 0;
+    int x = c;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_sync(0xffffffffu, x, lane >= o ? lane - o : lane);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      int s = lane < nw ? wsum[lane] : 0;
+      for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_sync(0xffffffffu, s, lane >= o ? lane - o : lane);
+        if (lane >= o) s += y;
+      }
+      if (lane < nw) wsum[lane] = s;
+    }
+    __syncthreads();
+    if (idx < B) offs[idx] = carry + (warp ? wsum[warp - 1] : 0) + x - c;
+    __syncthreads();
+    if (tid == 0) carry += wsum[nw - 1];
+  }
+  __syncthreads();
+  if (tid == 0) *total = carry;
+  for (int b = warp; b < B; b += nw) {
+    int slot = offs[b];
+    for (int p0 = 0; p0 < JN; p0 += 32) {
+      const bool act = active(b, p0 + lane);
+      const unsigned m = __ballot_sync(0xffffffffu, act);
+      if (act) pairs[slot + __popc(m & ((1u << lane) - 1u))] = b * JN + p0 + lane;
+      slot += __popc(m);
+    }
+  }
+}
+
 // V_nl[b] = sum_{j,i,l} (2l+1)/12 v_l(|r_i - R_I|) sum_q P_l(cos th_q) psi(r_i->q)/psi(r)
 // (reference: ecp/gaussian_type_ecp.py:161-255).  One WARP per walker: lanes stride over the
 // (nucleus, electron) pairs, 12 quadrature ratios each, warp-shuffle reduction; accumulation in
-// double.  Adds V_nl to E_loc and to stats[3].
+// double.  Only the pairs inside the cutoff (ecp_pair_active) have quadrature forwards: the walker's
+// active pairs are entries offs[b], offs[b] + 1, ... of the group's pair list (ecp_pairs_kernel), in
+// the order of this loop; a pair outside adds nothing.  Adds V_nl to E_loc and to stats[3].
 template <class T>
 __global__ void ecp_accumulate_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M,
                                       int J, const int* __restrict__ nl_nuc, const T* __restrict__ nl_params,
+                                      const double* __restrict__ rc2, const int* __restrict__ offs,
                                       int L, int Tm, const T* __restrict__ sign0, const T* __restrict__ log0,
                                       const T* __restrict__ sign_v, const T* __restrict__ log_v, int B, int Bstat,
                                       T* __restrict__ out_E, T* __restrict__ out_stats) {
@@ -385,16 +451,21 @@ __global__ void ecp_accumulate_kernel(const T* __restrict__ r, const T* __restri
   const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
   const double l0 = (double)log0[b], s0 = (double)sign0[b];
   double total = 0.0;
-  for (int p = lane; p < J * N; p += 32) {
+  int slot = offs[b];
+  for (int p0 = 0; p0 < J * N; p0 += 32) {  // warp-uniform trip count: every lane takes part in the ballot
+    const int p = p0 + lane;
     const int j = p / N, i = p - j * N;
-    const int I = nl_nuc[j];
+    const int I = p < J * N ? nl_nuc[j] : 0;
+    double d2 = 0.0;
+    const bool act = p < J * N && ecp_pair_active(rb + 3 * i, Rb + 3 * I, rc2[j], d2);
+    const unsigned m = __ballot_sync(0xffffffffu, act);
+    const int a = slot + __popc(m & ((1u << lane) - 1u));
+    slot += __popc(m);
+    if (!act) continue;
     const T* nl = nl_params + (size_t)I * L * 2 * Tm;
-    double dx = (double)rb[3 * i] - (double)Rb[3 * I], dy = (double)rb[3 * i + 1] - (double)Rb[3 * I + 1],
-           dz = (double)rb[3 * i + 2] - (double)Rb[3 * I + 2];
-    double d2 = dx * dx + dy * dy + dz * dz;
     double integ[4] = {0, 0, 0, 0};
     for (int q = 0; q < 12; ++q) {
-      size_t v = ((size_t)b * J * N + p) * 12 + q;
+      size_t v = (size_t)a * 12 + q;
       double ratio = ::exp((double)log_v[v] - l0) * (double)sign_v[v] * s0;
       double th, ph;
       ico_vertex(q, th, ph);

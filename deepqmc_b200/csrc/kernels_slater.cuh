@@ -673,7 +673,7 @@ slater_fwd2_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batch
                    int B, const T* __restrict__ pi_up, const T* __restrict__ pi_dn, const T* __restrict__ zeta_up,
                    const T* __restrict__ zeta_dn, const T* __restrict__ BF, int ldb, T* __restrict__ det_sign,
                    T* __restrict__ det_log, int rep, int full_det, const T* __restrict__ env_base, long long v0, int vper,
-                   int vlayout) {
+                   int vlayout, const int* __restrict__ pairs) {
   DQMC_DYN_SMEM(smem_raw);
   const int NP = N | 1, KN = K * N;
   T* As = reinterpret_cast<T*>(smem_raw);  // [K][N][NP]
@@ -695,7 +695,7 @@ slater_fwd2_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batch
       // position and spin only, so all rows but the moved ones come from the base walker's table env_base[w][i][k N + mu]
       // (env_table_kernel), the moved rows are evaluated afresh with the electron's own spin: 12 M (ECP) instead of N M
       // exponentials per orbital (the envelope sums were 3/4 of this kernel's MUFU-bound first phase).
-      const VirtualMove mv = virtual_move((int)(v0 + b), vper, N, n_up, vlayout);
+      const VirtualMove mv = virtual_move((int)(v0 + b), vper, N, n_up, vlayout, pairs);
       const int bw = mv.base, nmv = mv.e1 < 0 ? 1 : 2;
       for (int idx = tid; idx < nmv * M; idx += nt) {
         const int t = idx / M, m = idx - t * M, imv = t ? mv.e1 : mv.e0;

@@ -128,9 +128,10 @@ template <class T>
 __global__ void __launch_bounds__(256)
 embed_fwd_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M, int n_up,
                  int log_rescale, const T* __restrict__ W, int d, T* __restrict__ X, int total, int epb,
-                 long long v0 = 0, int vper = 0) {
+                 long long v0 = 0, int vper = 0, const int* __restrict__ pairs = nullptr) {
   // vper > 0: compact mode of the non-local-ECP quadrature forwards -- row t is the MOVED electron of virtual walker v = v0 + t
-  // (virtual_move, ECP layout); the other electrons' rows are those of the base walker (see trunk_tc.cuh)
+  // (virtual_move, ECP layout over the active-pair list `pairs`); the other electrons' rows are those of the base walker (see
+  // trunk_tc.cuh)
   DQMC_DYN_SMEM(smem_raw);
   const int F = 4 * M + 1;
   T* Ws = reinterpret_cast<T*>(smem_raw);  // [F][d]
@@ -148,7 +149,7 @@ embed_fwd_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched
       T f0 = T(0), g0 = T(0), g1 = T(0), g2 = T(0);
       if (bi < e_end) {
         const int b = vper > 0 ? bi : bi / N;
-        const T* ri = r + (vper > 0 ? ((size_t)bi * N + (size_t)virtual_move((int)(v0 + bi), vper, N, n_up, kVirtEcp).e0) : (size_t)bi) * 3;
+        const T* ri = r + (vper > 0 ? ((size_t)bi * N + (size_t)virtual_move((int)(v0 + bi), vper, N, n_up, kVirtEcp, pairs).e0) : (size_t)bi) * 3;
         const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
         const T dx0 = ri[0] - Rb[3 * m], dx1 = ri[1] - Rb[3 * m + 1], dx2 = ri[2] - Rb[3 * m + 2];
         const T rho = m_sqrt(Num<T>::eps() + dx0 * dx0 + dx1 * dx1 + dx2 * dx2);
@@ -164,7 +165,7 @@ embed_fwd_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched
     }
     if (tid < 32) {
       const int bi = e0 + tid;
-      const int el_i = vper > 0 ? virtual_move((int)(v0 + bi), vper, N, n_up, kVirtEcp).e0 : bi % N;
+      const int el_i = vper > 0 ? (bi < e_end ? virtual_move((int)(v0 + bi), vper, N, n_up, kVirtEcp, pairs).e0 : 0) : bi % N;
       ft[(F - 1) * 32 + tid] = (bi < e_end && el_i < n_up) ? T(1) : T(-1);
     }
     __syncthreads();

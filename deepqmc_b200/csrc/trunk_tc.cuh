@@ -42,7 +42,8 @@ struct TrunkParams {
   const float* X0; int ldx;      // embedding rows [rows][256]  (vper > 0, ECP layout: [walkers][256], the moved electron's row)
   const float* Xbase;            // vper > 0 (compact virtual-walker forwards): embedding rows of the group's base walkers
   long long v0; int vper;        //   [base][N][256]; walker w of this launch is virtual walker v0 + w, whose base walker and
-  int n_up, vlayout;             //   moved electrons virtual_move(v0 + w, vper, N, n_up, vlayout) gives (common.cuh)
+  int n_up, vlayout;             //   moved electrons virtual_move(v0 + w, vper, N, n_up, vlayout, pairs) gives (common.cuh)
+  const int* pairs;              //   ECP layout: the group's active-pair list
   const float* wspin;            // swap layout: embedding weights of the +-1 spin feature [256]
   float* Out; int ldout;         // trunk output rows [rows][256]
   const CUtensorMap* maps;       // device array [L][4][2]: (Wqkv, Wo, W1, W2) x (hi, lo); boxes of 32 halves x 256 rows
@@ -109,7 +110,7 @@ trunk_f16_kernel(TrunkParams p) {
           float sw = 0.f;
           if (p.vper > 0) {
             const int walker = tile * G + (r >> lnp), el = r & (NP - 1);
-            const VirtualMove mv = virtual_move((int)p.v0 + walker, p.vper, N, p.n_up, p.vlayout);
+            const VirtualMove mv = virtual_move((int)p.v0 + walker, p.vper, N, p.n_up, p.vlayout, p.pairs);
             if (mv.e1 < 0) {  // ECP: the moved electron's row is new
               xrow = el == mv.e0 ? p.X0 + (size_t)walker * p.ldx : p.Xbase + ((size_t)mv.base * N + el) * p.ldx;
             } else {  // spin swap: up electron e0 sits at r_e1 and down electron e1 at r_e0, each with its own spin:

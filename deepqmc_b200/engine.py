@@ -831,6 +831,11 @@ class Engine:
     def launch_count(self):
         return self.lib.dqmc_launch_count(self.h)
 
+    @property
+    def ecp_forward_count(self):
+        """Non-local ECP quadrature forwards run so far (12 per electron-nucleus pair inside the cutoff radius)."""
+        return self.lib.dqmc_ecp_forward_count(self.h)
+
     def close(self):
         if getattr(self, 'h', None):
             self.lib.dqmc_destroy(self.h)

@@ -238,6 +238,9 @@ int dqmc_debug_plan(dqmc_handle h, int32_t n_walkers, int32_t mode, int64_t work
 
 /* Number of kernels this handle has launched so far (bench.py's gpu_launches claim). */
 int64_t dqmc_launch_count(dqmc_handle h);
+/* Number of non-local ECP quadrature forwards (virtual walkers, 12 per active electron-nucleus pair) this handle has run so far
+   in local-energy calls: pairs beyond the nucleus' cutoff radius run none (DQMC_ECP_CUTOFF=0: every pair runs). */
+int64_t dqmc_ecp_forward_count(dqmc_handle h);
 
 /* Self-test hook: run ONE dense-layer row GEMM  C = (Res) + A @ W[weight] (+ bias on value rows)
  * with the named weight of the handle's parameter table, on the requested backend

@@ -243,6 +243,11 @@ template <class T> inline T __shfl_down_sync(unsigned, T v, int d) {
   return emu::shfl_idx(v, lane + d < 32 ? lane + d : lane);
 }
 inline int __popc(unsigned x) { return __builtin_popcount(x); }
+inline unsigned __ballot_sync(unsigned, int pred) {  // every lane of the warp calls it (as the kernels do)
+  unsigned m = pred ? 1u << (emu::S().fibers[emu::S().cur].lin & 31) : 0u;
+  for (int o = 16; o > 0; o >>= 1) m |= __shfl_xor_sync(0xffffffffu, m, o);
+  return m;
+}
 template <class T> inline T atomicAdd(T* p, T v) { T o = *p; *p = o + v; return o; }
 template <class T> inline T atomicMax(T* p, T v) { T o = *p; if (v > o) *p = v; return o; }
 

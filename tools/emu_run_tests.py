@@ -16,7 +16,7 @@ The emulator replaces ex2.approx / rcp.approx / redux.sync by exact code: it che
 
 Usage:  python tools/emu_run_tests.py [--lib PATH] [--nobuild] [--asan] test_name[substring] [test_name ...]
         python tools/emu_run_tests.py --all-small          (every test small enough for the emulator, parity files)
-Tests come from test_gpu_parity.py, test_gpu_z_next_rows.py and test_gpu_slater_conformance.py; stacked parametrize marks run
+Tests come from test_gpu_parity.py, test_gpu_z_next_rows.py, test_gpu_ecp_cutoff.py and test_gpu_slater_conformance.py; stacked parametrize marks run
 as their cartesian product, and `name[substring]` keeps the cases whose arguments' repr contains the substring.
 """
 import argparse
@@ -33,7 +33,9 @@ sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
 # full-size / tensor-core tests: hours on the emulator, or not emulable
 TOO_BIG = {'test_full_size_properties_4096_walkers', 'test_benzene_full_psiformer_fp32_tensor_core_vs_fp64',
-           'test_ferminet_n2_full_fp32_tensor_core_vs_fp64', 'test_engine_external_fixtures'}
+           'test_ferminet_n2_full_fp32_tensor_core_vs_fp64', 'test_engine_external_fixtures',
+           'test_benzene_fp32_cutoff_equals_all_pairs', 'test_benzene_walker_isolation_mixed_active_counts',
+           'test_cutoff_quadrature_chunking_bitwise'}
 
 
 def build(out, asan=False):
@@ -102,20 +104,21 @@ def main():
     import pytest
 
     pytest_param_type = type(pytest.param(0))
+    import test_gpu_ecp_cutoff as EC
     import test_gpu_parity as P
     import test_gpu_slater_conformance as SC
     import test_gpu_z_next_rows as Z
 
-    P.DEV = Z.DEV = SC.DEV = 'cpu'
+    P.DEV = Z.DEV = SC.DEV = EC.DEV = 'cpu'
     torch.cuda.synchronize = lambda *args, **kw: None
     names = list(a.names)
     if a.all_small:
-        names += [n for mod in (P, Z) for n in vars(mod) if n.startswith('test_') and n not in TOO_BIG and n not in names]
+        names += [n for mod in (P, Z, EC) for n in vars(mod) if n.startswith('test_') and n not in TOO_BIG and n not in names]
     for name in names:
         # name or name[substring]: the cases whose printed arguments contain the substring
         name, _, sel = name.partition('[')
         sel = sel.rstrip(']')
-        f = getattr(Z, name, None) or getattr(P, name, None) or getattr(SC, name)
+        f = getattr(Z, name, None) or getattr(P, name, None) or getattr(EC, name, None) or getattr(SC, name)
         wants_tmp = 'tmp_path' in f.__code__.co_varnames[:f.__code__.co_argcount]
         # stacked parametrize marks: the cartesian product of their cases, passed by argument name
         axes = []
