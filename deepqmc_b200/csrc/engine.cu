@@ -81,6 +81,7 @@ struct EngineBase {
   bool plan_only = false;
   mutable const char* dry_hwm = nullptr;  // highest workspace address carved during a dry pass
   void note_hwm(const void* q) const { if (dry && (const char*)q > dry_hwm) dry_hwm = (const char*)q; }
+  mutable std::vector<unsigned char*> emu_guards;  // emulator builds only: guard zones behind the carved workspace buffers
   // optional per-launch timing of the dominant (GEMM) kernels with CUDA events on the caller's stream
   bool prof = false;
   double prof_flops = 0;
@@ -251,6 +252,61 @@ struct EngineBase {
   }
 };
 
+// Bump allocator over a caller's workspace: every buffer of every entry point is carved through one.  Buffers are 256-byte
+// aligned; emulator builds (tools/cuda_emu) put a 256-byte guard zone behind each one, verified after each chunk
+// (Engine::check_guards), so a buffer that is individually too small (with a consistent total) cannot hide.  The guard bytes
+// are part of what take() advances by, so the PLAN (a dry pass of the same code) contains them too: emulator and hardware
+// builds plan by the same rule, there is no build-dependent slack.
+struct Arena {
+  const EngineBase* e;
+  char* base;
+  char* top;    // next free byte
+  int64_t cap;  // bytes of the workspace behind base
+  Arena(const EngineBase* e_, void* base_, int64_t cap_ = INT64_MAX) : e(e_), base((char*)base_), top((char*)base_), cap(cap_) {}
+  template <class U>
+  U* take(size_t n) {
+    U* q = (U*)top;
+    top += align_up(sizeof(U) * n);
+#ifdef DQMC_EMU
+    if (!e->dry) { std::memset(top, 0xC3, 256); e->emu_guards.push_back((unsigned char*)top); }
+    top += 256;
+#endif
+    e->note_hwm(top);
+    return q;
+  }
+  int64_t left() const { return cap - (top - base); }  // < 0: the buffers taken exceed the workspace
+};
+
+// Size probes and dqmc_debug_plan walk the carving code on a dummy base with every CUDA call skipped (EngineBase::dry); the
+// scope restores the caller's dry state and high-water mark, so probes nest inside a planning pass.
+static char* plan_base() { return (char*)(uintptr_t)0x100000; }
+struct DryPass {
+  EngineBase* e;
+  bool was;
+  const char* hw;
+  explicit DryPass(const EngineBase* e_) : e(const_cast<EngineBase*>(e_)), was(e->dry), hw(e->dry_hwm) {
+    e->dry = true;  // no guard writes through the dummy base
+    e->dry_hwm = plan_base();
+  }
+  ~DryPass() { e->dry = was; e->dry_hwm = hw; }
+  int64_t bytes() const { return e->dry_hwm - plan_base(); }  // highest offset carved so far
+};
+
+// largest n in [1, hi] with bytes(n) <= wsb (bytes monotone in n), 0 if there is none
+template <class F>
+static int64_t largest_fit(int64_t hi, int64_t wsb, F bytes) {
+  if (hi < 1 || bytes(1) > wsb) return 0;
+  if (bytes(hi) <= wsb) return hi;
+  int64_t lo = 1;
+  while (hi - lo > 1) {
+    const int64_t mid = (lo + hi) / 2;
+    (bytes(mid) <= wsb ? lo : hi) = mid;
+  }
+  return lo;
+}
+
+static constexpr int64_t kRowCap = 2000000000;  // elements per chunk buffer: keeps 32-bit row * ld products safe
+
 template <class T>
 __global__ void convert_kernel(const double* __restrict__ src, T* __restrict__ dst, int64_t n) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -324,16 +380,6 @@ inline cudaError_t raise_dyn_smem(F fn, int bytes) {
     ++launches;                                                  \
   } while (0)
 
-// Emulator builds (tools/cuda_emu) put a 256-byte guard behind every buffer carved from the workspace and verify the
-// guards after each chunk: a buffer that is individually too small (with a consistent total) cannot hide.
-// The guard bytes are part of what carve() / the take lambdas advance by, so the PLAN (a dry pass of the same code) contains
-// them too: emulator and hardware builds plan by the same rule, there is no build-dependent slack.
-#ifdef DQMC_EMU
-#define DQ_TAKE_GUARD() do { if (!dry) { std::memset(p, 0xC3, 256); emu_guards.push_back((unsigned char*)p); } p += 256; } while (0)
-#else
-#define DQ_TAKE_GUARD() do {} while (0)
-#endif
-
 template <class T>
 struct Engine : EngineBase {
   T* d_params = nullptr;
@@ -352,7 +398,6 @@ struct Engine : EngineBase {
   int* d_ph_nuc = nullptr;
   int ph_G = 0;
   double ph_rmax = 0;
-  mutable std::vector<unsigned char*> emu_guards;  // emulator builds only: guard zones behind the carved workspace buffers
   int check_guards() {
 #ifdef DQMC_EMU
     for (unsigned char* g : emu_guards)
@@ -362,7 +407,6 @@ struct Engine : EngineBase {
 #endif
     return 0;
   }
-  int64_t vjp_ws_cap = 0;  // bytes of the caller's workspace during a reverse pass (extent check of the chunk buffers)
   bool ph_on = false;      // tables uploaded
   bool ph_active = false;  // set around the forward-Laplacian pass of local_energy only
   T* mos_out = nullptr;    // set by orbitals(): the tail writes the orbital matrices of the chunk here and stops
@@ -743,7 +787,6 @@ struct Engine : EngineBase {
     T *G0 = nullptr, *G1 = nullptr, *G2 = nullptr, *Hs = nullptr, *Ha = nullptr, *C = nullptr, *Fc = nullptr, *HT = nullptr,
       *E0 = nullptr, *E1 = nullptr, *ET0 = nullptr, *ET1 = nullptr, *W3 = nullptr,
       *Y0 = nullptr, *Y1 = nullptr, *Jb = nullptr;  // conv-GNN trunk
-    size_t bytes;
   };
   int gnn_hmax() const {
     int h = 1;
@@ -773,136 +816,142 @@ struct Engine : EngineBase {
     for (int i = 0; i < cfg.jastrow_n; ++i) j += cfg.jastrow_dims[i];
     return j;
   }
-  // Workspace plan == the carve itself: chunk_bytes() runs carve() on a dummy base, so a buffer added to carve() can never
-  // be forgotten in the plan (round 1 planned dgrad for S > 1 only while carve() always took it).
-  static char* plan_base() { return (char*)(uintptr_t)0x100000; }
-  size_t chunk_bytes(int Bc, int S) const {
-    const bool was = dry;
-    const char* hw = dry_hwm;  // a size probe is not a carve of the caller's workspace
-    const_cast<Engine*>(this)->dry = true;  // no guard writes through the dummy base
-    const size_t n = carve(plan_base(), Bc, S).bytes;
-    const_cast<Engine*>(this)->dry = was;
-    dry_hwm = hw;
-    return n;
+  // Workspace plan == the carve itself: every planned size is a dry pass of the functions that carve the buffers (chunk_bytes
+  // runs carve(), prefixed_bytes an entry point's prefix carve followed by carve(), vjp_chunk_bytes the reverse-pass chunk),
+  // so a buffer added to a carve can never be forgotten in the plan (round 1 planned dgrad for S > 1 only while carve()
+  // always took it).
+  int64_t chunk_bytes(int Bc, int S) const {
+    DryPass dp(this);
+    carve(plan_base(), Bc, S);
+    return dp.bytes();
   }
   Ws carve(void* base, int Bc, int S) const {
     Ws w;
     size_t rows = (size_t)Bc * N * S;
-    char* p = (char*)base;
-    auto take = [&](size_t n) { T* q = (T*)p; p += align_up(sizeof(T) * n); DQ_TAKE_GUARD(); return q; };
+    Arena a(this, base);
     if (gnn) {
       const size_t e = cfg.edge_dim, hm = gnn_hmax(), dm = gnn_dmax(), em = gnn_emax(), hn = gnn_hnode_max();
       const size_t pairs8 = (size_t)Bc * N * (N + (cfg.gnn_conv_ne ? M : 0)) * 8;
-      w.X = take(rows * dm); w.O = take(rows * dm); w.G0 = take(rows * d); w.G1 = take(rows * d); w.G2 = take(rows * d);
-      w.Fc = take(rows * (3 * dm + 3 * e)); w.Hs = take(rows * e); w.Ha = take(rows * e); w.HT = take(rows * hn);
-      w.C = take(rows * 3 * e);
-      w.E0 = take(pairs8 * em); w.E1 = take(pairs8 * em); w.ET0 = take(pairs8 * em); w.ET1 = take(pairs8 * em);
-      w.W3 = take(pairs8 * 3 * e);
-      w.Y0 = take(rows * hm); w.Y1 = take(rows * hm); w.Jb = take((size_t)Bc * S * gnn_jsum());
+      w.X = a.take<T>(rows * dm); w.O = a.take<T>(rows * dm); w.G0 = a.take<T>(rows * d); w.G1 = a.take<T>(rows * d);
+      w.G2 = a.take<T>(rows * d); w.Fc = a.take<T>(rows * (3 * dm + 3 * e)); w.Hs = a.take<T>(rows * e);
+      w.Ha = a.take<T>(rows * e); w.HT = a.take<T>(rows * hn); w.C = a.take<T>(rows * 3 * e);
+      w.E0 = a.take<T>(pairs8 * em); w.E1 = a.take<T>(pairs8 * em); w.ET0 = a.take<T>(pairs8 * em); w.ET1 = a.take<T>(pairs8 * em);
+      w.W3 = a.take<T>(pairs8 * 3 * e);
+      w.Y0 = a.take<T>(rows * hm); w.Y1 = a.take<T>(rows * hm); w.Jb = a.take<T>((size_t)Bc * S * gnn_jsum());
       w.A = w.M1 = w.QKV = nullptr;
-      w.BF = take(rows * KN);
+      w.BF = a.take<T>(rows * KN);
     } else if (cfg.kind == DQMC_FERMINET) {
       const size_t dm = fermi_dmax(), em = fermi_emax(), fin = 3 * dm + 2 * em;
-      w.X = take(rows * dm); w.O = take(rows * dm); w.QKV = take(rows * fin);  // H, H2, F
-      w.A = take(rows * N * em); w.M1 = take(rows * N * em);                   // E, E2
-      w.BF = take(rows * BFW);
+      w.X = a.take<T>(rows * dm); w.O = a.take<T>(rows * dm); w.QKV = a.take<T>(rows * fin);  // H, H2, F
+      w.A = a.take<T>(rows * N * em); w.M1 = a.take<T>(rows * N * em);                        // E, E2
+      w.BF = a.take<T>(rows * BFW);
     } else {
-      w.X = take(rows * d); w.O = take(rows * d); w.A = take(rows * d); w.M1 = take(rows * d);
-      w.QKV = take(rows * 3 * d); w.BF = take(rows * BFW);
+      w.X = a.take<T>(rows * d); w.O = a.take<T>(rows * d); w.A = a.take<T>(rows * d); w.M1 = a.take<T>(rows * d);
+      w.QKV = a.take<T>(rows * 3 * d); w.BF = a.take<T>(rows * BFW);
     }
-    w.dsign = take((size_t)Bc * K); w.dlog = take((size_t)Bc * K); w.dlap = take((size_t)Bc * K);
-    w.dgrad = take((size_t)Bc * K * (S > 1 ? T3 : 1));
-    if (ph_on && S > 1) w.QA = take((size_t)Bc * N * PH_STRIDE);
-    if (cfg.backflow_add) w.Gadd = take((size_t)Bc * N * 5);
-    w.bytes = p - (char*)base;
-    note_hwm(p);
+    w.dsign = a.take<T>((size_t)Bc * K); w.dlog = a.take<T>((size_t)Bc * K); w.dlap = a.take<T>((size_t)Bc * K);
+    w.dgrad = a.take<T>((size_t)Bc * K * (S > 1 ? T3 : 1));
+    if (ph_on && S > 1) w.QA = a.take<T>((size_t)Bc * N * PH_STRIDE);
+    if (cfg.backflow_add) w.Gadd = a.take<T>((size_t)Bc * N * 5);
     return w;
+  }
+  // bytes of the buffers `prefix` carves followed by a forward chunk of Bc walkers with S slots
+  template <class Prefix>
+  int64_t prefixed_bytes(Prefix prefix, int64_t Bc, int S) const {
+    DryPass dp(this);
+    Arena a(this, plan_base());
+    prefix(a);
+    carve(a.top, (int)Bc, S);
+    return dp.bytes();
   }
   // largest walker chunk (<= B, <= the 32-bit row cap) whose carve fits wsb bytes
   int max_chunk(int64_t wsb, int S, int B) const {
-    int64_t c = B;
-    int64_t row_cap = (int64_t)2000000000 / ((int64_t)N * S * 3 * d);  // keep 32-bit row*ld products safe
-    if (cfg.kind == DQMC_FERMINET) row_cap = (int64_t)2000000000 / ((int64_t)N * N * S * (3 * (int64_t)fermi_dmax() + 64));
-    if (gnn) row_cap = (int64_t)2000000000 / ((int64_t)N * (N + M + S) * (8 * gnn_emax() + 3 * gnn_dmax() + 3 * cfg.edge_dim + KN));
-    if (c > row_cap) c = row_cap;
-    if (c < 1 || (int64_t)chunk_bytes(1, S) > wsb) return 0;
-    if ((int64_t)chunk_bytes((int)c, S) <= wsb) return (int)c;
-    int64_t lo = 1, hi = c;  // chunk_bytes is monotone in the chunk size
-    while (hi - lo > 1) {
-      const int64_t mid = (lo + hi) / 2;
-      if ((int64_t)chunk_bytes((int)mid, S) <= wsb) lo = mid; else hi = mid;
-    }
-    return (int)lo;
+    int64_t row_cap = kRowCap / ((int64_t)N * S * 3 * d);
+    if (cfg.kind == DQMC_FERMINET) row_cap = kRowCap / ((int64_t)N * N * S * (3 * (int64_t)fermi_dmax() + 64));
+    if (gnn) row_cap = kRowCap / ((int64_t)N * (N + M + S) * (8 * gnn_emax() + 3 * gnn_dmax() + 3 * cfg.edge_dim + KN));
+    return (int)largest_fit(std::min<int64_t>(B, row_cap), wsb, [&](int64_t n) { return chunk_bytes((int)n, S); });
   }
-  // non-local ECP pass for nb walkers: virtual walkers r_virt[V][N][3], sign[V], log[V] + one
-  // forward chunk over all V = nb * J * N * 12 virtual walkers.  Sized for every pair active, so the
-  // plan does not depend on the walkers; the cutoff only shortens the list the forwards run over.
-  int64_t ecp_prefix_bytes(int64_t nb) const {
-    const int64_t V = nb * J * N * 12;
-    return (int64_t)align_up(sizeof(T) * V * 3 * N) + 2 * (int64_t)align_up(sizeof(T) * V) +
-           (int64_t)align_up(sizeof(T) * nb * N * K * N) +  // + envelope table of the group's base walkers
-           (int64_t)align_up(sizeof(T) * nb * N * d) +      // + their embedding rows
-           (int64_t)align_up(sizeof(int) * nb * J * N) +    // + active-pair list
-           (int64_t)align_up(sizeof(int) * (nb + 1));       // + per-walker offsets into it, pair count
+  // Virtual-walker group of nb base walkers (non-local ECP quadrature points, spin swaps): the V virtual walkers r[V][N][3],
+  // their sign[V] and log[V], and the base walkers' envelope table [nb][N][K N] and embedding rows [nb][N][d] that the
+  // forwards gather the unmoved electrons from.  The ECP group adds its active-pair list int[nb J N] and the per-walker
+  // offsets into it int[nb + 1] (the last entry is the group's pair count), the spin group the base walkers' sign[nb] and
+  // log[nb].
+  struct VirtGroup {
+    T *r, *sign, *logp, *env, *emb, *sign0 = nullptr, *logp0 = nullptr;
+    int *pairs = nullptr, *offs = nullptr;
+  };
+  VirtGroup carve_virt_group(Arena& a, int64_t nb, int64_t V) const {
+    VirtGroup g;
+    g.r = a.take<T>(V * 3 * N); g.sign = a.take<T>(V); g.logp = a.take<T>(V);
+    g.env = a.take<T>(nb * N * K * N); g.emb = a.take<T>(nb * N * d);
+    return g;
   }
-  // walkers per ECP group are bounded by the 32-bit row cap of the plain-forward chunk: the plan never asks for more
-  int64_t ecp_group_cap() const {
-    const int64_t vper = (int64_t)J * N * 12;
-    const int64_t vcap = 2000000000LL / ((int64_t)N * 3 * d);
-    return std::max<int64_t>(1, vcap / vper);
+  // Sized for every pair active (V = nb J N 12), so the plan does not depend on the walkers; the cutoff only shortens the
+  // list the forwards run over.
+  VirtGroup carve_ecp_group(Arena& a, int64_t nb) const {
+    VirtGroup g = carve_virt_group(a, nb, nb * J * N * 12);
+    g.pairs = a.take<int>(nb * J * N); g.offs = a.take<int>(nb + 1);
+    return g;
   }
-  int64_t ecp_bytes(int64_t nb) const {
-    const int64_t V = nb * J * N * 12;
-    return ecp_prefix_bytes(nb) + (int64_t)chunk_bytes((int)V, 1);
+  VirtGroup carve_spin_group(Arena& a, int64_t nb, int64_t P) const {  // P swapped pairs per walker
+    VirtGroup g = carve_virt_group(a, nb, nb * P);
+    g.sign0 = a.take<T>(nb); g.logp0 = a.take<T>(nb);
+    return g;
   }
-  // spin pass for nb walkers with P swapped pairs each: virtual walkers r_virt[V][N][3], sign[V], log[V], the base walkers'
-  // sign[nb], log[nb], envelope table and embedding rows + one forward chunk over all V = nb P virtual walkers
-  int64_t spin_prefix_bytes(int64_t nb, int64_t P) const {
-    const int64_t V = nb * P;
-    return (int64_t)align_up(sizeof(T) * V * 3 * N) + 2 * (int64_t)align_up(sizeof(T) * V) + 2 * (int64_t)align_up(sizeof(T) * nb) +
-           (int64_t)align_up(sizeof(T) * nb * N * K * N) + (int64_t)align_up(sizeof(T) * nb * N * d);
+  // base walkers per virtual-walker group (vper virtual walkers each) are bounded by the 32-bit row cap of the plain-forward
+  // chunk: the plan never asks for more
+  int64_t group_cap(int64_t vper) const { return std::max<int64_t>(1, kRowCap / ((int64_t)N * 3 * d) / vper); }
+  // bytes of an ECP / spin group of nb walkers + a plain-forward chunk of Vc virtual walkers
+  int64_t ecp_bytes(int64_t nb, int64_t Vc) const { return prefixed_bytes([&](Arena& a) { carve_ecp_group(a, nb); }, Vc, 1); }
+  int64_t spin_bytes(int64_t nb, int64_t P, int64_t Vc) const {
+    return prefixed_bytes([&](Arena& a) { carve_spin_group(a, nb, P); }, Vc, 1);
   }
-  int64_t spin_group_cap(int64_t P) const {
-    const int64_t vcap = 2000000000LL / ((int64_t)N * 3 * d);
-    return std::max<int64_t>(1, vcap / std::max<int64_t>(P, 1));
+  // Metropolis / Langevin sweep over B walkers: the proposed walkers (Langevin: and their drift), their sign and log, the
+  // acceptance counter (one 256-byte slot)
+  struct Proposals { T *r, *force, *sign, *logp; int* cnt; };
+  Proposals carve_proposals(Arena& a, int B, bool with_force) const {
+    Proposals q;
+    q.r = a.take<T>((size_t)B * 3 * N); q.force = with_force ? a.take<T>((size_t)B * 3 * N) : nullptr;
+    q.sign = a.take<T>(B); q.logp = a.take<T>(B); q.cnt = a.take<int>(1);
+    return q;
   }
-  int64_t spin_bytes(int64_t nb, int64_t P) const {  // P >= 1 (the base forward of nb <= nb P walkers fits the same chunk)
-    return spin_prefix_bytes(nb, P) + (int64_t)chunk_bytes((int)(nb * P), 1);
+  struct ForceBufs { T *E, *stats, *grad; };  // value_and_force: E, 6 stats, grad of the forward-Laplacian pass
+  ForceBufs carve_force(Arena& a, int B) const {
+    ForceBufs f;
+    f.E = a.take<T>(B); f.stats = a.take<T>((size_t)6 * B); f.grad = a.take<T>((size_t)B * T3);
+    return f;
   }
-  int64_t mcmc_prefix_bytes(int B) const {
-    return (int64_t)align_up(sizeof(T) * (size_t)B * 3 * N) + 2 * (int64_t)align_up(sizeof(T) * (size_t)B) + 256;
-  }
-  int64_t force_prefix_bytes(int B) const {  // value_and_force: E, 6 stats, grad
-    return (int64_t)(align_up(sizeof(T) * (size_t)B) + align_up(sizeof(T) * (size_t)6 * B) + align_up(sizeof(T) * (size_t)B * T3));
-  }
-  int64_t langevin_prefix_bytes(int B) const {
-    return 2 * (int64_t)align_up(sizeof(T) * (size_t)B * 3 * N) + 2 * (int64_t)align_up(sizeof(T) * (size_t)B) + 256;
+  // prefix of a Metropolis (langevin false) or Langevin sweep over B walkers + a forward chunk of Bc walkers
+  int64_t sweep_bytes(int B, bool langevin, int Bc) const {
+    auto prefix = [&](Arena& a) { carve_proposals(a, B, langevin); if (langevin) carve_force(a, B); };
+    return prefixed_bytes(prefix, Bc, langevin ? T3 + 2 : 1);
   }
   // bytes one reverse-pass chunk of Bc walkers carves: a dry pass of the chunk function itself
   int64_t vjp_chunk_bytes(int Bc) {
-    const bool was = dry;
-    const char* hw = dry_hwm;
-    const int64_t cap = vjp_ws_cap;
-    dry = true; dry_hwm = plan_base(); vjp_ws_cap = INT64_MAX;
-    if (gnn) vjp_chunk_paulinet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, plan_base(), nullptr);
-    else if (cfg.kind == DQMC_FERMINET) vjp_chunk_ferminet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, plan_base(), nullptr);
-    else vjp_chunk(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, plan_base(), nullptr);
-    const int64_t n = dry_hwm - plan_base();
-    dry = was; dry_hwm = hw; vjp_ws_cap = cap;
-    return n;
+    DryPass dp(this);
+    const Arena a(this, plan_base());
+    if (gnn) vjp_chunk_paulinet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr);
+    else if (cfg.kind == DQMC_FERMINET) vjp_chunk_ferminet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr);
+    else vjp_chunk(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr);
+    return dp.bytes();
   }
   int64_t ws_bytes(int B, int mode) override {
     if (B < 1) B = 1;
     if (mode == DQMC_MODE_VJP) return vjp_chunk_bytes(B);
-    if (mode == DQMC_MODE_MCMC) return mcmc_prefix_bytes(B) + (int64_t)chunk_bytes(B, 1);
-    if (mode == DQMC_MODE_LANGEVIN) return langevin_prefix_bytes(B) + force_prefix_bytes(B) + (int64_t)chunk_bytes(B, T3 + 2);
+    if (mode == DQMC_MODE_MCMC) return sweep_bytes(B, false, B);
+    if (mode == DQMC_MODE_LANGEVIN) return sweep_bytes(B, true, B);
     if (mode == DQMC_MODE_SPIN) {  // sized for the exact estimator, the larger of the two; no down electrons: no forwards
       const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
-      return P ? spin_bytes(std::min<int64_t>(B, spin_group_cap(P)), P) : 0;
+      if (!P) return 0;
+      const int64_t nb = std::min<int64_t>(B, group_cap(P));
+      return spin_bytes(nb, P, nb * P);
     }
     int S = mode == DQMC_MODE_FORWARD ? 1 : T3 + 2;
-    int64_t need = (int64_t)chunk_bytes(B, S);
-    if (mode == DQMC_MODE_LOCAL_ENERGY && J > 0) need = std::max<int64_t>(need, ecp_bytes(std::min<int64_t>(B, ecp_group_cap())));
+    int64_t need = chunk_bytes(B, S);
+    if (mode == DQMC_MODE_LOCAL_ENERGY && J > 0) {
+      const int64_t vper = (int64_t)J * N * 12, nb = std::min<int64_t>(B, group_cap(vper));
+      need = std::max(need, ecp_bytes(nb, nb * vper));
+    }
     return need;
   }
   // least workspace with which a call for B walkers proceeds (walkers chunked down to one at a time)
@@ -911,15 +960,14 @@ struct Engine : EngineBase {
     const int S = T3 + 2;
     switch (mode) {
       case DQMC_MODE_VJP: return vjp_chunk_bytes(1);
-      case DQMC_MODE_MCMC: return mcmc_prefix_bytes(B) + (int64_t)chunk_bytes(1, 1);
-      case DQMC_MODE_LANGEVIN: return langevin_prefix_bytes(B) + force_prefix_bytes(B) + (int64_t)chunk_bytes(1, S);
-      case DQMC_MODE_LOCAL_ENERGY:
-        return std::max<int64_t>((int64_t)chunk_bytes(1, S), J > 0 ? ecp_prefix_bytes(1) + (int64_t)chunk_bytes(1, 1) : 0);
+      case DQMC_MODE_MCMC: return sweep_bytes(B, false, 1);
+      case DQMC_MODE_LANGEVIN: return sweep_bytes(B, true, 1);
+      case DQMC_MODE_LOCAL_ENERGY: return std::max<int64_t>(chunk_bytes(1, S), J > 0 ? ecp_bytes(1, 1) : 0);
       case DQMC_MODE_SPIN: {
         const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
-        return P ? spin_prefix_bytes(1, P) + (int64_t)chunk_bytes(1, 1) : 0;
+        return P ? spin_bytes(1, P, 1) : 0;
       }
-      default: return (int64_t)chunk_bytes(1, 1);
+      default: return chunk_bytes(1, 1);
     }
   }
   // dqmc_debug_plan: walk the entry point of `mode` with a workspace of wsb bytes (<= 0: the planned size) on a dummy base
@@ -928,8 +976,7 @@ struct Engine : EngineBase {
     const int64_t pl = ws_bytes(B, mode);
     if (planned) *planned = pl;
     if (wsb <= 0) wsb = pl;
-    const bool was = dry;
-    dry = true; dry_hwm = plan_base();
+    DryPass dp(this);
     void* ws = plan_base();
     int rc = 0;
     switch (mode) {
@@ -949,8 +996,7 @@ struct Engine : EngineBase {
       case DQMC_MODE_SPIN: rc = spin(nullptr, nullptr, 0, B, nullptr, nullptr, -1, nullptr, nullptr, ws, wsb, nullptr); break;
       default: err = "unknown mode"; rc = 2;
     }
-    if (carved) *carved = dry_hwm - plan_base();
-    dry = was;
+    if (carved) *carved = dp.bytes();
     return rc;
   }
 
@@ -1766,7 +1812,7 @@ struct Engine : EngineBase {
                   int64_t wsb, cudaStream_t st) {
     int Bc = max_chunk(wsb, S, B);
     if (Bc < 1) { err = "workspace too small for a single walker"; return 3; }
-    if ((int64_t)chunk_bytes(Bc, S) > wsb) { err = "internal: carved workspace exceeds the planned size"; return 3; }
+    if (chunk_bytes(Bc, S) > wsb) { err = "internal: carved workspace exceeds the planned size"; return 3; }
     if (dry) { carve(ws, Bc, S); return 0; }  // planning pass: record the extent of the largest chunk
     for (int b0 = 0; b0 < B; b0 += Bc) {
       int nb = std::min(Bc, B - b0);
@@ -1783,18 +1829,15 @@ struct Engine : EngineBase {
 
   // ---- Metropolis-adjusted Langevin sweep (SURVEY.md 8(f) N3): value + drift from the forward-Laplacian pass ----
   // state = {r, sign, log, force}; force == clean_force(grad log|psi|) with the CURRENT tau (electron_samplers.py:197-211)
-  int value_and_force(const T* r, const T* R, int Rb, int B, const T* tau, T* sign, T* logp, T* force, char* p, int64_t rest,
+  int value_and_force(const T* r, const T* R, int Rb, int B, const T* tau, T* sign, T* logp, T* force, void* ws, int64_t wsb,
                       cudaStream_t st) {
-    T* E = (T*)p; p += align_up(sizeof(T) * (size_t)B);
-    T* stt = (T*)p; p += align_up(sizeof(T) * (size_t)6 * B);
-    T* grad = (T*)p; p += align_up(sizeof(T) * (size_t)B * T3);
-    rest -= force_prefix_bytes(B);
-    note_hwm(p);
-    if (rest < 0) { err = "workspace too small (Langevin force buffers)"; return 3; }
-    int rc = run_batched(r, R, Rb, B, T3 + 2, sign, logp, E, stt, grad, p, rest, st);
+    Arena a(this, ws, wsb);
+    const ForceBufs f = carve_force(a, B);
+    if (a.left() < 0) { err = "workspace too small (Langevin force buffers)"; return 3; }
+    int rc = run_batched(r, R, Rb, B, T3 + 2, sign, logp, f.E, f.stats, f.grad, a.top, a.left(), st);
     if (rc) return rc;
-    DQ_LAUNCH(langevin_force_kernel<T>, dim3((B * N + 127) / 128), dim3(128), 0, st, (const T*)grad, r, R, Rb, (const T*)d_znuc, tau,
-              N, M, B * N, force);
+    DQ_LAUNCH(langevin_force_kernel<T>, dim3((B * N + 127) / 128), dim3(128), 0, st, (const T*)f.grad, r, R, Rb, (const T*)d_znuc,
+              tau, N, M, B * N, force);
     return 0;
   }
   int langevin(void* r_, void* sign_, void* logp_, void* force_, int32_t* age, void* tau_, const void* R_, int Rb, int B, int n_sub,
@@ -1803,37 +1846,32 @@ struct Engine : EngineBase {
     T* r = (T*)r_; T* sign = (T*)sign_; T* logp = (T*)logp_; T* force = (T*)force_; T* tau = (T*)tau_; T* stats = (T*)stats_;
     const T* R = (const T*)R_;
     if (n_sub == 0) return langevin_update(r, R, Rb, B, tau, sign, logp, force, ws, wsb, st);
-    char* p = (char*)ws;
-    T* rp = (T*)p; p += align_up(sizeof(T) * (size_t)B * 3 * N);
-    T* fp = (T*)p; p += align_up(sizeof(T) * (size_t)B * 3 * N);
-    T* sp = (T*)p; p += align_up(sizeof(T) * (size_t)B);
-    T* lp = (T*)p; p += align_up(sizeof(T) * (size_t)B);
-    int* cnt = (int*)p; p += 256;
-    int64_t rest = wsb - (p - (char*)ws);
-    note_hwm(p);
-    if (rest < 0) { err = "workspace too small (Langevin proposal buffers)"; return 3; }
-    DQ_CHECK(cudaMemsetAsync(cnt, 0, sizeof(int), st));
+    Arena a(this, ws, wsb);
+    const Proposals q = carve_proposals(a, B, true);
+    if (a.left() < 0) { err = "workspace too small (Langevin proposal buffers)"; return 3; }
+    DQ_CHECK(cudaMemsetAsync(q.cnt, 0, sizeof(int), st));
     const int ne = B * 3 * N;
     for (int s = 0; s < n_sub; ++s) {
       const T* nns = nn ? (const T*)nn + (size_t)s * ne : nullptr;
       const T* nus = nu ? (const T*)nu + (size_t)s * B : nullptr;
-      DQ_LAUNCH(langevin_propose_kernel<T>, dim3((ne / 2 + 1 + 127) / 128), dim3(128), 0, st, (const T*)r, (const T*)force, rp,
+      DQ_LAUNCH(langevin_propose_kernel<T>, dim3((ne / 2 + 1 + 127) / 128), dim3(128), 0, st, (const T*)r, (const T*)force, q.r,
                 (const T*)tau, nns, seed, step0 + (uint64_t)s, woff * (uint64_t)(3 * N), ne);
-      int rc = value_and_force(rp, R, Rb, B, tau, sp, lp, fp, p, rest, st);
+      int rc = value_and_force(q.r, R, Rb, B, tau, q.sign, q.logp, q.force, a.top, a.left(), st);
       if (rc) return rc;
-      DQ_LAUNCH(langevin_accept_kernel<T>, dim3((B + 127) / 128), dim3(128), 0, st, r, (const T*)rp, force, (const T*)fp, sign,
-                (const T*)sp, logp, (const T*)lp, age, (const T*)tau, nus, seed, step0 + (uint64_t)s, woff, max_age, B, N, cnt);
-      DQ_LAUNCH(tau_kernel<T>, dim3(1), dim3(32), 0, st, tau, cnt, B, (T)target, stats);
+      DQ_LAUNCH(langevin_accept_kernel<T>, dim3((B + 127) / 128), dim3(128), 0, st, r, (const T*)q.r, force, (const T*)q.force,
+                sign, (const T*)q.sign, logp, (const T*)q.logp, age, (const T*)tau, nus, seed, step0 + (uint64_t)s, woff, max_age, B,
+                N, q.cnt);
+      DQ_LAUNCH(tau_kernel<T>, dim3(1), dim3(32), 0, st, tau, q.cnt, B, (T)target, stats);
     }
     DQ_LAUNCH(sampler_stats_kernel<T>, dim3(1), dim3(256), 0, st, (const T*)r, (const T*)logp, (const int*)age, (const T*)tau, B,
               N, stats);
     DQ_CHECK(cudaGetLastError());
-    return 0;
+    return check_guards();  // the proposal buffers' guards, after the last accept (and with n_sub == 0)
   }
   // n_sub == 0 with force output: (re)compute psi and the drift of the current walkers (sampler.update)
   int langevin_update(const T* r, const T* R, int Rb, int B, const T* tau, T* sign, T* logp, T* force, void* ws, int64_t wsb,
                       cudaStream_t st) {
-    int rc = value_and_force(r, R, Rb, B, tau, sign, logp, force, (char*)ws, wsb, st);
+    int rc = value_and_force(r, R, Rb, B, tau, sign, logp, force, ws, wsb, st);
     if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
     return 0;
@@ -1870,18 +1908,17 @@ struct Engine : EngineBase {
               hi > lo ? N : 0, lo, hi);
   }
 
-  int vjp_chunk(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, void* wsbase, cudaStream_t st) {
+  int vjp_chunk(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a, cudaStream_t st) {
     const int L = cfg.n_layers, rows = Bc * N, F = 4 * M + 1;
-    char* p = (char*)wsbase;
-    auto take = [&](size_t n) { T* q = (T*)p; p += align_up(sizeof(T) * n); DQ_TAKE_GUARD(); return q; };
     std::vector<T*> X(L + 1), QKV(L), O(L), A(L), M1(L);
-    for (int l = 0; l <= L; ++l) X[l] = take((size_t)rows * d);
-    for (int l = 0; l < L; ++l) { QKV[l] = take((size_t)rows * 3 * d); O[l] = take((size_t)rows * d); A[l] = take((size_t)rows * d); M1[l] = take((size_t)rows * d); }
-    T* BF = take((size_t)rows * KN); T* dBF = take((size_t)rows * KN);
-    T* dsign = take((size_t)Bc * K); T* dlog = take((size_t)Bc * K); T* dld = take((size_t)Bc * K);
-    T* dXn = take((size_t)rows * d); T* dZ = take((size_t)rows * d); T* dM1 = take((size_t)rows * d);
-    T* dA = take((size_t)rows * d); T* dO = take((size_t)rows * d); T* dQKV = take((size_t)rows * 3 * d);
-    T* dX = take((size_t)rows * d); T* Feat = take((size_t)rows * F);
+    for (int l = 0; l <= L; ++l) X[l] = a.take<T>((size_t)rows * d);
+    for (int l = 0; l < L; ++l) { QKV[l] = a.take<T>((size_t)rows * 3 * d); O[l] = a.take<T>((size_t)rows * d); A[l] = a.take<T>((size_t)rows * d); M1[l] = a.take<T>((size_t)rows * d); }
+    T* BF = a.take<T>((size_t)rows * KN); T* dBF = a.take<T>((size_t)rows * KN);
+    T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
+    T* dXn = a.take<T>((size_t)rows * d); T* dZ = a.take<T>((size_t)rows * d); T* dM1 = a.take<T>((size_t)rows * d);
+    T* dA = a.take<T>((size_t)rows * d); T* dO = a.take<T>((size_t)rows * d); T* dQKV = a.take<T>((size_t)rows * 3 * d);
+    T* dX = a.take<T>((size_t)rows * d); T* Feat = a.take<T>((size_t)rows * F);
+    if (a.left() < 0) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
     const T scale = (T)(1.0 / std::sqrt((double)dh));
     // ---- forward with every layer's activations kept --------------------------------------------------------
     DQ_LAUNCH(embed_kernel<T>, dim3((rows + 7) / 8), dim3(128), sizeof(T) * 5 * F, st, r, R, Rb, N, M, cfg.n_up, 1, 1, 1,
@@ -1957,33 +1994,30 @@ struct Engine : EngineBase {
     }
     DQ_LAUNCH(embed_feat_kernel<T>, dim3((rows * M + 127) / 128), dim3(128), 0, st, r, R, Rb, N, M, cfg.n_up, Feat, rows);
     wgrad(Feat, F, dXn, d, rows, F, d, G + off("emb.w"), 0, 0, st);
-    note_hwm(p);
-    if ((int64_t)(p - (char*)wsbase) > vjp_ws_cap) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
     return 0;
   }
 
   // FermiNet reverse pass (conf/ansatz/ferminet.yaml): node update g on concat[h, spin means of h, spin means of the
   // incoming edges], shared edge MLP u, residuals / sqrt(2).  The raw input features carry no parameters, so the
   // chain stops at the first layer's weights.
-  int vjp_chunk_ferminet(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, void* wsbase,
+  int vjp_chunk_ferminet(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a,
                          cudaStream_t st) {
     const int L = cfg.n_layers, rows = Bc * N, rowsE = Bc * N * N, de = cfg.edge_dim, d0 = 4 * M;
     const T isq2 = (T)0.70710678118654752440;
-    char* p = (char*)wsbase;
-    auto take = [&](size_t n) { T* q = (T*)p; p += align_up(sizeof(T) * n); DQ_TAKE_GUARD(); return q; };
     std::vector<T*> Hs(L + 1), Es(L), Fs(L);
     std::vector<int> dH(L + 1), dEd(L);
     dH[0] = d0;
     for (int l = 1; l <= L; ++l) dH[l] = d;
     for (int l = 0; l < L; ++l) dEd[l] = l == 0 ? 4 : de;
-    for (int l = 0; l <= L; ++l) Hs[l] = take((size_t)rows * dH[l]);
-    for (int l = 0; l < L; ++l) { Es[l] = take((size_t)rowsE * dEd[l]); Fs[l] = take((size_t)rows * (3 * dH[l] + 2 * dEd[l])); }
+    for (int l = 0; l <= L; ++l) Hs[l] = a.take<T>((size_t)rows * dH[l]);
+    for (int l = 0; l < L; ++l) { Es[l] = a.take<T>((size_t)rowsE * dEd[l]); Fs[l] = a.take<T>((size_t)rows * (3 * dH[l] + 2 * dEd[l])); }
     const int fmax = 3 * (d > d0 ? d : d0) + 2 * (de > 4 ? de : 4);
-    T* BF = take((size_t)rows * KN); T* dBF = take((size_t)rows * KN);
-    T* dsign = take((size_t)Bc * K); T* dlog = take((size_t)Bc * K); T* dld = take((size_t)Bc * K);
-    T* dXa = take((size_t)rows * d); T* dXb = take((size_t)rows * d); T* dZ = take((size_t)rows * d);
-    T* dF = take((size_t)rows * fmax);
-    T* dEa = take((size_t)rowsE * de); T* dEb = take((size_t)rowsE * de); T* dZe = take((size_t)rowsE * de);
+    T* BF = a.take<T>((size_t)rows * KN); T* dBF = a.take<T>((size_t)rows * KN);
+    T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
+    T* dXa = a.take<T>((size_t)rows * d); T* dXb = a.take<T>((size_t)rows * d); T* dZ = a.take<T>((size_t)rows * d);
+    T* dF = a.take<T>((size_t)rows * fmax);
+    T* dEa = a.take<T>((size_t)rowsE * de); T* dEb = a.take<T>((size_t)rowsE * de); T* dZe = a.take<T>((size_t)rowsE * de);
+    if (a.left() < 0) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
     // ---- forward, activations kept -----------------------------------------------------------------------------
     DQ_LAUNCH(embed_kernel<T>, dim3(Bc * N), dim3(128), sizeof(T) * 5 * d0, st, r, R, Rb, N, M, cfg.n_up, 1, 0, 0,
               (const T*)nullptr, d0, Hs[0], Bc * N, 1, (const T*)nullptr);
@@ -2069,8 +2103,6 @@ struct Engine : EngineBase {
       T* t1 = dHn; dHn = dHc; dHc = t1;
       T* t2 = dEn; dEn = dEc; dEc = t2;
     }
-    note_hwm(p);
-    if ((int64_t)(p - (char*)wsbase) > vjp_ws_cap) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
     return 0;
   }
   // ---- conv-GNN reverse pass: the reference's test ansatz (tests/conf/ansatz.yaml: hk.Embed embeddings, 'featurewise'
@@ -2080,13 +2112,12 @@ struct Engine : EngineBase {
     std::vector<T*> a;     // a[0] input, a[k] output of layer k (after its activation)
     std::vector<int> dim;  // widths
   };
-  template <class Take>
   int tape_fwd(const T* in, int din, const int* dims, int nl, const std::string& base, bool bias, int act, bool last_linear,
-               int rows_, Take& take, Tape& t, cudaStream_t st) {
+               int rows_, Arena& a, Tape& t, cudaStream_t st) {
     t.a.assign(1, const_cast<T*>(in));
     t.dim.assign(1, din);
     for (int i = 0; i < nl; ++i) {
-      T* out = take((size_t)rows_ * dims[i]);
+      T* out = a.take<T>((size_t)rows_ * dims[i]);
       const std::string q = base + std::to_string(i);
       const bool b_i = bias && (!last_linear || base[0] != 'J' || i < nl - 1);  // Jastrow: bias 'not_last'
       int rc = gemm(t.a.back(), t.dim.back(), (q + ".w").c_str(), nullptr, 0, dims[i], b_i ? P(q + ".b") : nullptr, nullptr, 0, out,
@@ -2125,7 +2156,7 @@ struct Engine : EngineBase {
     }
     return 0;
   }
-  int vjp_chunk_paulinet(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, void* wsbase,
+  int vjp_chunk_paulinet(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a,
                          cudaStream_t st) {
     const int L = cfg.n_layers, rows = Bc * N, e = cfg.edge_dim, nl = cfg.gnn_sub_n > 0 ? cfg.gnn_sub_n : 1;
     const int Mne = cfg.gnn_conv_ne ? M : 0, NS = N + Mne, nt = cfg.gnn_conv_ne ? 3 : 2, pairs = Bc * N * NS;
@@ -2133,8 +2164,6 @@ struct Engine : EngineBase {
     const bool deep = cfg.gnn_deep_edges != 0;
     const T isq2 = (T)0.70710678118654752440;
     const char* tn[3] = {"same", "anti", "ne"};
-    char* p = (char*)wsbase;
-    auto take = [&](size_t n) { T* q = (T*)p; p += align_up(sizeof(T) * n); DQ_TAKE_GUARD(); return q; };
     // ---- forward, everything kept --------------------------------------------------------------------------------
     std::vector<T*> X(L + 1), C(L), Fc(L), E(L);
     std::vector<int> xd(L + 1), ed(L);
@@ -2143,35 +2172,35 @@ struct Engine : EngineBase {
     std::vector<std::array<Tape, 2>> Ht(L);
     std::vector<Tape> Ut(L);
     xd[0] = cfg.gnn_features ? 4 * M : d;
-    X[0] = take((size_t)rows * xd[0]);
+    X[0] = a.take<T>((size_t)rows * xd[0]);
     if (cfg.gnn_features)  // raw nucleus-electron features [|d|, d]: no parameters
       DQ_LAUNCH(embed_kernel<T>, dim3(rows), dim3(128), sizeof(T) * 5 * xd[0], st, r, R, Rb, N, M, cfg.n_up, 1, 0, 0, (const T*)nullptr,
                 xd[0], X[0], rows, 1, (const T*)nullptr);
     else
       DQ_LAUNCH(gnn_embed_kernel<T>, dim3((rows * d + 127) / 128), dim3(128), 0, st, P("emb.table"), n_types, N, cfg.n_up, 1, d, X[0], rows);
-    E[0] = take((size_t)pairs * 4);
+    E[0] = a.take<T>((size_t)pairs * 4);
     ed[0] = 4;
     DQ_LAUNCH(gnn_edge_val_kernel<T>, dim3((pairs + 127) / 128), dim3(128), 0, st, r, R, Rb, N, M, Mne, E[0], pairs);
     for (int l = 0; l < L; ++l) {
       const std::string q = "G" + std::to_string(l) + ".";
       for (int t = 0; t < nt; ++t) {
-        int rc = tape_fwd(E[l], ed[l], cfg.gnn_w_dims[l], nl, q + "w_" + tn[t] + ".", cfg.gnn_w_bias != 0, 0, false, pairs, take, Wt[l][t], st);
+        int rc = tape_fwd(E[l], ed[l], cfg.gnn_w_dims[l], nl, q + "w_" + tn[t] + ".", cfg.gnn_w_bias != 0, 0, false, pairs, a, Wt[l][t], st);
         if (rc) return rc;
       }
       for (int t = 0; t < 2; ++t) {
-        int rc = tape_fwd(X[l], xd[l], cfg.gnn_h_dims[l], nl, q + "h_" + tn[t] + ".", true, 0, false, rows, take, Ht[l][t], st);
+        int rc = tape_fwd(X[l], xd[l], cfg.gnn_h_dims[l], nl, q + "h_" + tn[t] + ".", true, 0, false, rows, a, Ht[l][t], st);
         if (rc) return rc;
       }
-      C[l] = take((size_t)rows * nt * e);
+      C[l] = a.take<T>((size_t)rows * nt * e);
       DQ_LAUNCH(gnn_conv_val_kernel<T>, dim3(rows), dim3(64), 0, st, (const T*)Wt[l][0].a.back(), (const T*)Wt[l][1].a.back(),
                 (const T*)(nt == 3 ? Wt[l][2].a.back() : nullptr), (const T*)Ht[l][0].a.back(), (const T*)Ht[l][1].a.back(),
                 nt == 3 ? P(q + "hne") : (const T*)nullptr, N, Mne, cfg.n_up, e, C[l]);
       xd[l + 1] = d;
       if (cfg.gnn_concat) {  // x <- [(x +) tanh(g([x, mean_up x, mean_down x, conv_*]))] (/ sqrt 2)
         const int fin = 3 * xd[l] + nt * e;
-        Fc[l] = take((size_t)rows * fin);
+        Fc[l] = a.take<T>((size_t)rows * fin);
         DQ_LAUNCH(gnn_concat_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)X[l], xd[l], (const T*)C[l], nt * e, N, cfg.n_up, 1, Fc[l]);
-        X[l + 1] = take((size_t)rows * d);
+        X[l + 1] = a.take<T>((size_t)rows * d);
         int rc = gemm(Fc[l], fin, (q + "g.w").c_str(), nullptr, 0, d, cfg.gnn_g_bias ? P(q + "g.b") : nullptr, nullptr, 0, X[l + 1], d,
                       rows, d, fin, 1, 0, N, st);
         if (rc) return rc;
@@ -2181,7 +2210,7 @@ struct Engine : EngineBase {
       } else {  // featurewise: x <- x + sum_t tanh(g_t(conv_t)); each G_t holds the running sum
         const T* res = xd[l] == d ? X[l] : nullptr;
         for (int t = 0; t < nt; ++t) {
-          Gt[l][t] = take((size_t)rows * d);
+          Gt[l][t] = a.take<T>((size_t)rows * d);
           int rc = gemm(C[l] + t * e, nt * e, (q + "g_" + tn[t] + ".w").c_str(), nullptr, 0, d, P(q + "g_" + tn[t] + ".b"), nullptr, 0,
                         Gt[l][t], d, rows, d, e, 1, 0, N, st);
           if (rc) return rc;
@@ -2192,11 +2221,11 @@ struct Engine : EngineBase {
         X[l + 1] = Gt[l][nt - 1];
       }
       if (deep && l < L - 1) {  // shared edge MLP u + normalised residual (electron_gnn.py:160-192)
-        int rc = tape_fwd(E[l], ed[l], cfg.gnn_u_dims[l], nl, q + "u.", true, 0, false, pairs, take, Ut[l], st);
+        int rc = tape_fwd(E[l], ed[l], cfg.gnn_u_dims[l], nl, q + "u.", true, 0, false, pairs, a, Ut[l], st);
         if (rc) return rc;
         ed[l + 1] = e;
         if (ed[l] == e) {
-          E[l + 1] = take((size_t)pairs * e);
+          E[l + 1] = a.take<T>((size_t)pairs * e);
           DQ_LAUNCH((axpby_kernel<T>), dim3((unsigned)(((size_t)pairs * e + 255) / 256)), dim3(256), 0, st, (const T*)E[l],
                     (const T*)Ut[l].a.back(), isq2, E[l + 1], (size_t)pairs * e);
         } else {
@@ -2210,9 +2239,9 @@ struct Engine : EngineBase {
     Tape Jt;
     T* Js = nullptr;
     if (cfg.jastrow_n > 0) {
-      Js = take((size_t)Bc * d);
+      Js = a.take<T>((size_t)Bc * d);
       DQ_LAUNCH(sum_electrons_kernel<T>, dim3((Bc * d + 127) / 128), dim3(128), 0, st, (const T*)X[L], N, 1, d, Js, Bc * d);
-      int rc = tape_fwd(Js, d, cfg.jastrow_dims, cfg.jastrow_n, "J", true, 1, true, Bc, take, Jt, st);
+      int rc = tape_fwd(Js, d, cfg.jastrow_dims, cfg.jastrow_n, "J", true, 1, true, Bc, a, Jt, st);
       if (rc) return rc;
     }
     // per-spin backflow MLPs: hidden layers (ssp), then the orbital head (+ default mult_act)
@@ -2222,19 +2251,19 @@ struct Engine : EngineBase {
     for (int i = 0; i < cfg.backflow_n; ++i) {
       const int dout = cfg.backflow_dims[i];
       const std::string q = std::to_string(i);
-      Y[i + 1] = take((size_t)rows * dout); yd[i + 1] = dout;
+      Y[i + 1] = a.take<T>((size_t)rows * dout); yd[i + 1] = dout;
       int rc = gemm(Y[i], yd[i], ("bfh" + q + ".up").c_str(), ("bfh" + q + ".dn").c_str(), cfg.n_up, dout, P("bfb" + q + ".up"), nullptr,
                     0, Y[i + 1], dout, Bc, dout, yd[i], 1, 1, N, st, 0, P("bfb" + q + ".dn"));
       if (rc) return rc;
       DQ_LAUNCH(act_fl_kernel<T>, dim3(rows, (dout + 31) / 32), dim3(32), 0, st, Y[i + 1], dout, (const T*)nullptr, 0, 1, dout, T(1), 1);
     }
-    T* BF = take((size_t)rows * KN); T* dBF = take((size_t)rows * KN);
+    T* BF = a.take<T>((size_t)rows * KN); T* dBF = a.take<T>((size_t)rows * KN);
     int rc = gemm(Y.back(), yd.back(), "bf.up", "bf.dn", cfg.n_up, KN, P("bfb.up"), nullptr, 0, BF, KN, Bc, KN, yd.back(), 1, 1, N, st, 0,
                   P("bfb.dn"));
     if (rc) return rc;
     if (cfg.mult_act == 1)
       DQ_LAUNCH(act_fl_kernel<T>, dim3(rows, (KN + 127) / 128), dim3(128), 0, st, BF, KN, (const T*)nullptr, 0, 1, KN, T(1), 2);
-    T* dsign = take((size_t)Bc * K); T* dlog = take((size_t)Bc * K); T* dld = take((size_t)Bc * K);
+    T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
     const int full_det = cfg.factorized_det ? 0 : 1;
     const int sl_wpb = slater_warps_per_block<T>(N);
     DQ_LAUNCH(slater_kernel<T>, dim3((Bc * K + sl_wpb - 1) / sl_wpb), dim3(32 * sl_wpb), slater_smem_bytes<T>(N), st, r, R, Rb, N,
@@ -2267,16 +2296,16 @@ struct Engine : EngineBase {
     const int xm = std::max(d, xd[0]);
     const int hm = std::max(gnn_hmax(), xm), hn = std::max(gnn_hnode_max(), e), em = gnn_emax();
     const int fmax = 3 * xm + nt * e;
-    T* dXa = take((size_t)rows * xm); T* dXb = take((size_t)rows * xm);
-    T* sr0 = take((size_t)rows * std::max(hm, hn)); T* sr1 = take((size_t)rows * std::max(hm, hn));
-    T* dCb = take((size_t)rows * nt * e); T* dCt = take((size_t)rows * e);
-    T* dFb = cfg.gnn_concat ? take((size_t)rows * fmax) : nullptr;
-    T* dWb[3] = {take((size_t)pairs * e), take((size_t)pairs * e), take((size_t)pairs * e)};
-    T* sp0 = take((size_t)pairs * em); T* sp1 = take((size_t)pairs * em);
-    T* dHb[2] = {take((size_t)rows * e), take((size_t)rows * e)};
-    T* dEa = deep ? take((size_t)pairs * e) : nullptr;
-    T* dEb = deep ? take((size_t)pairs * e) : nullptr;
-    T* dUb = deep ? take((size_t)pairs * e) : nullptr;
+    T* dXa = a.take<T>((size_t)rows * xm); T* dXb = a.take<T>((size_t)rows * xm);
+    T* sr0 = a.take<T>((size_t)rows * std::max(hm, hn)); T* sr1 = a.take<T>((size_t)rows * std::max(hm, hn));
+    T* dCb = a.take<T>((size_t)rows * nt * e); T* dCt = a.take<T>((size_t)rows * e);
+    T* dFb = cfg.gnn_concat ? a.take<T>((size_t)rows * fmax) : nullptr;
+    T* dWb[3] = {a.take<T>((size_t)pairs * e), a.take<T>((size_t)pairs * e), a.take<T>((size_t)pairs * e)};
+    T* sp0 = a.take<T>((size_t)pairs * em); T* sp1 = a.take<T>((size_t)pairs * em);
+    T* dHb[2] = {a.take<T>((size_t)rows * e), a.take<T>((size_t)rows * e)};
+    T* dEa = deep ? a.take<T>((size_t)pairs * e) : nullptr;
+    T* dEb = deep ? a.take<T>((size_t)pairs * e) : nullptr;
+    T* dUb = deep ? a.take<T>((size_t)pairs * e) : nullptr;
     // orbital head
     if (cfg.mult_act == 1) {
       const size_t n = (size_t)rows * KN;
@@ -2304,8 +2333,8 @@ struct Engine : EngineBase {
     T* dXn = dXa;  // gradient w.r.t. X_L
     T* dXc = dXb;
     if (cfg.jastrow_n > 0) {  // d log|psi| / d jastrow = w_b
-      T* dJ = take((size_t)Bc);  // [Bc] scalars
-      T* js0 = take((size_t)Bc * d); T* js1 = take((size_t)Bc * d); T* dJs = take((size_t)Bc * d);
+      T* dJ = a.take<T>((size_t)Bc);  // [Bc] scalars
+      T* js0 = a.take<T>((size_t)Bc * d); T* js1 = a.take<T>((size_t)Bc * d); T* dJs = a.take<T>((size_t)Bc * d);
       DQ_CHECK(cudaMemcpyAsync(dJ, wts, sizeof(T) * Bc, cudaMemcpyDeviceToDevice, st));
       tape_bwd(Jt, dJ, "J", true, 1, true, Bc, js0, js1, dJs, false, G, st);
       const size_t n = (size_t)rows * d;
@@ -2373,8 +2402,7 @@ struct Engine : EngineBase {
     if (!cfg.gnn_features)
       DQ_LAUNCH(embed_table_bwd_kernel<T>, dim3((d + 63) / 64, 64), dim3(64), 0, st, (const T*)dXn, n_types, N, cfg.n_up, d, rows,
                 G + off("emb.table"));
-    note_hwm(p);
-    if ((int64_t)(p - (char*)wsbase) > vjp_ws_cap) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
+    if (a.left() < 0) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
     return 0;
   }
 
@@ -2389,17 +2417,9 @@ struct Engine : EngineBase {
     // walkers per chunk: activations of every layer stay resident for the reverse pass (64 buffers, 256 B alignment each)
     const bool fermi = cfg.kind == DQMC_FERMINET;
     // largest chunk whose buffers (measured by a dry pass of the chunk function) fit the caller's workspace
-    int64_t Bc = B;
-    if (vjp_chunk_bytes(1) > wsb) { err = "workspace too small for a single walker (vjp)"; return 3; }
-    if (vjp_chunk_bytes((int)Bc) > wsb) {
-      int64_t lo = 1, hi = Bc;
-      while (hi - lo > 1) {
-        const int64_t mid = (lo + hi) / 2;
-        if (vjp_chunk_bytes((int)mid) <= wsb) lo = mid; else hi = mid;
-      }
-      Bc = lo;
-    }
-    vjp_ws_cap = wsb;
+    // (not const: nvcc 12.9's front end aborts on a const local initialised through this lambda)
+    int64_t Bc = largest_fit(B, wsb, [&](int64_t n) { return vjp_chunk_bytes((int)n); });
+    if (Bc < 1) { err = "workspace too small for a single walker (vjp)"; return 3; }
     if (!fermi && !gnn)
     DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
     {  // the same warps-per-block rule as at the launch sites (at most 4 warps, at most 96 KiB)
@@ -2413,9 +2433,10 @@ struct Engine : EngineBase {
       const int nb = (int)std::min<int64_t>(Bc, B - b0);
       const T* rc_ = r + (size_t)b0 * 3 * N;
       const T* Rc_ = R + (Rb ? (size_t)b0 * 3 * M : 0);
-      int rc = gnn ? vjp_chunk_paulinet(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, ws, st)
-             : fermi ? vjp_chunk_ferminet(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, ws, st)
-                     : vjp_chunk(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, ws, st);
+      const Arena a(this, ws, wsb);
+      int rc = gnn ? vjp_chunk_paulinet(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, a, st)
+             : fermi ? vjp_chunk_ferminet(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, a, st)
+                     : vjp_chunk(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, a, st);
       if (rc) return rc;
       rc = check_guards();
       if (rc) return rc;
@@ -2458,6 +2479,49 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  // Virtual walkers (vper per base walker: ECP quadrature points, spin swaps) through the plain forward in groups of nb base
+  // walkers: the largest group whose prefix (carve_group) + one forward chunk of all its virtual walkers fits wsb, else one
+  // walker (run_batched chunks its virtual walkers).  Per group, setup() launches the kind's work before the forwards and sets
+  // V, the virtual walkers to run, and finish() reduces their results.  With `tables` (and slater_fwd2, N <= 32) the forwards
+  // take the unmoved electrons' envelopes and, with `emb_table`, embedding rows from tables of the base walkers.
+  template <class CarveGroup, class Setup, class Finish>
+  int virtual_groups(const T* r, const T* R, int B, int64_t vper, int layout, bool tables, bool emb_table, void* ws,
+                     int64_t wsb, const char* too_small, CarveGroup carve_group, Setup setup, Finish finish, cudaStream_t st) {
+    auto bytes = [&](int64_t nb, int64_t Vc) { return prefixed_bytes([&](Arena& a) { carve_group(a, nb); }, Vc, 1); };
+    int64_t Be = largest_fit(std::min<int64_t>(B, group_cap(vper)), wsb, [&](int64_t nb) { return bytes(nb, nb * vper); });
+    if (Be < 1) Be = 1;  // one walker's virtual walkers do not fit at once: the plain-forward pass chunks them
+    if (bytes(Be, 1) > wsb) { err = too_small; return 3; }
+    tables = tables && slater_fwd2_ok && N <= 32 && !dry;
+    emb_table = tables && emb_table && embed_fwd_ok && can_trunk(1);
+    for (int b0 = 0; b0 < B; b0 += (int)Be) {
+      const int nb = (int)std::min<int64_t>(Be, B - b0);
+      const T* rb = r + (size_t)b0 * 3 * N;
+      Arena a(this, ws, wsb);
+      const VirtGroup g = carve_group(a, nb);
+      int64_t V = 0;
+      int rc = setup(b0, nb, g, a, V);
+      if (rc) return rc;
+      if (tables) {
+        DQ_LAUNCH(env_table_kernel<T>, dim3(nb), dim3(256), sizeof(T) * N * M, st, rb, R, N, M, cfg.n_up, K * N, P("env.pi_up"),
+                  P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), env_rep, g.env);
+        ecp_env = g.env; ecp_vper = (int)vper; virt_layout = layout; ecp_pairs = g.pairs;
+        if (emb_table) {
+          DQ_LAUNCH(embed_fwd_kernel<T>, dim3((nb * N + 31) / 32), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, rb, R, 0, N, M,
+                    cfg.n_up, 1, P("emb.w"), d, g.emb, nb * N, 32, 0LL, 0, (const int*)nullptr);
+          ecp_emb = g.emb;
+        }
+      }
+      if (V > 0) rc = run_batched(g.r, R, 0, (int)V, 1, g.sign, g.logp, nullptr, nullptr, nullptr, a.top, a.left(), st);
+      ecp_env = nullptr; ecp_emb = nullptr; ecp_pairs = nullptr; virt_layout = kVirtEcp;
+      if (rc) return rc;
+      rc = finish(b0, nb, g);
+      if (!rc) rc = check_guards();  // the prefix's guards, also when no forward ran (V == 0)
+      if (rc) return rc;
+      if (dry) break;  // planning pass: the first group is the largest
+    }
+    return 0;
+  }
+
   int local_energy(const void* r_, const void* R_, int Rb, int B, uint64_t seed, const void* twist, void* E,
                    void* stats, void* sign, void* logp, void* grad, void* ws, int64_t wsb, cudaStream_t st) override {
     const T* r = (const T*)r_;
@@ -2468,69 +2532,37 @@ struct Engine : EngineBase {
     if (rc) return rc;
     if (J > 0) {
       // non-local ECP: virtual walkers (12 quadrature points x electrons x ECP nuclei)
-      const int64_t vper = (int64_t)J * N * 12;
-      int64_t Be = std::min<int64_t>(B, ecp_group_cap());
-      if (ecp_bytes(Be) > wsb) {  // largest walker group whose virtual walkers fit the workspace
-        int64_t lo = 0, hi = Be;
-        while (hi - lo > 1) {
-          int64_t mid = (lo + hi) / 2;
-          if (ecp_bytes(mid) <= wsb) lo = mid; else hi = mid;
-        }
-        Be = lo;
-      }
-      if (Be < 1) Be = 1;  // one walker's virtual walkers do not fit at once: the plain-forward pass chunks them
-      if (ecp_prefix_bytes(Be) + (int64_t)chunk_bytes(1, 1) > wsb) { err = "workspace too small for the non-local ECP pass"; return 3; }
-      for (int b0 = 0; b0 < B; b0 += (int)Be) {
-        int nb = (int)std::min<int64_t>(Be, B - b0);
-        int64_t V = (int64_t)nb * vper;
-        char* p = (char*)ws;
-        T* rv = (T*)p; p += align_up(sizeof(T) * V * 3 * N);
-        T* sv = (T*)p; p += align_up(sizeof(T) * V);
-        T* lv = (T*)p; p += align_up(sizeof(T) * V);
-        T* envt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * K * N);
-        T* embt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * d);
-        int* pairs = (int*)p; p += align_up(sizeof(int) * (size_t)nb * J * N);
-        int* offs = (int*)p; p += align_up(sizeof(int) * (size_t)(nb + 1));
-        note_hwm(p);
+      auto setup = [&](int b0, int nb, const VirtGroup& g, const Arena&, int64_t& V) {
         if (Rb) { err = "non-local ECP with per-walker nuclei is not supported"; return 2; }
         const T* rb = r + (size_t)b0 * 3 * N;
-        const T* Rbp = R + (Rb ? (size_t)b0 * 3 * M : 0);
         const T* tw = twist ? (const T*)twist + (size_t)b0 * J * N : nullptr;
         // the pairs inside the cutoff radius; the group's quadrature forwards run over them alone
-        DQ_LAUNCH(ecp_pairs_kernel<T>, dim3(1), dim3(1024), 0, st, rb, Rbp, Rb, N, M, J, (const int*)d_nl_nuc,
-                  (const double*)d_nl_rc2, nb, offs, pairs, offs + nb);
+        DQ_LAUNCH(ecp_pairs_kernel<T>, dim3(1), dim3(1024), 0, st, rb, R, Rb, N, M, J, (const int*)d_nl_nuc,
+                  (const double*)d_nl_rc2, nb, g.offs, g.pairs, g.offs + nb);
         int n_act = nb * J * N;  // the planning pass sizes every buffer for all pairs
         if (!dry) {
-          DQ_CHECK(cudaMemcpyAsync(&n_act, offs + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+          DQ_CHECK(cudaMemcpyAsync(&n_act, g.offs + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
           DQ_CHECK(cudaStreamSynchronize(st));
           ecp_forwards += (int64_t)n_act * 12;
         }
         V = (int64_t)n_act * 12;
         if (n_act > 0)
-          DQ_LAUNCH(ecp_points_kernel<T>, dim3(n_act), dim3(64), 0, st, rb, Rbp, Rb, N, M, J, (const int*)d_nl_nuc, tw,
-                    seed, (uint64_t)b0, (const int*)pairs, rv);
-        const bool use_table = slater_fwd2_ok && N <= 32 && !dry && !std::getenv("DQMC_ECP_ENV_TABLE_OFF");
-        if (use_table) {  // the quadrature forwards take the unmoved electrons' envelopes from the base walkers' table
-          DQ_LAUNCH(env_table_kernel<T>, dim3(nb), dim3(256), sizeof(T) * N * M, st, rb, R, N, M, cfg.n_up, K * N,
-                    P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), cfg.n_env_per_nuc > 1 ? cfg.n_env_per_nuc : 1,
-                    envt);
-          ecp_env = envt; ecp_vper = (int)vper; ecp_pairs = pairs;
-          if (embed_fwd_ok && can_trunk(1) && !std::getenv("DQMC_ECP_EMB_TABLE_OFF")) {
-            DQ_LAUNCH(embed_fwd_kernel<T>, dim3((nb * N + 31) / 32), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, rb, R, 0, N, M,
-                      cfg.n_up, 1, P("emb.w"), d, embt, nb * N, 32, 0LL, 0, (const int*)nullptr);
-            ecp_emb = embt;
-          }
-        }
-        if (V > 0) rc = run_batched(rv, R, 0, (int)V, 1, sv, lv, nullptr, nullptr, nullptr, p, wsb - (p - (char*)ws), st);
-        ecp_env = nullptr; ecp_emb = nullptr; ecp_pairs = nullptr;
-        if (rc) return rc;
-        DQ_LAUNCH(ecp_accumulate_kernel<T>, dim3((nb + 3) / 4), dim3(128), 0, st, rb, Rbp, Rb, N, M, J,
-                  (const int*)d_nl_nuc, (const T*)d_nl_params, (const double*)d_nl_rc2, (const int*)offs,
+          DQ_LAUNCH(ecp_points_kernel<T>, dim3(n_act), dim3(64), 0, st, rb, R, Rb, N, M, J, (const int*)d_nl_nuc, tw,
+                    seed, (uint64_t)b0, (const int*)g.pairs, g.r);
+        return 0;
+      };
+      auto finish = [&](int b0, int nb, const VirtGroup& g) {
+        DQ_LAUNCH(ecp_accumulate_kernel<T>, dim3((nb + 3) / 4), dim3(128), 0, st, r + (size_t)b0 * 3 * N, R, Rb, N, M, J,
+                  (const int*)d_nl_nuc, (const T*)d_nl_params, (const double*)d_nl_rc2, (const int*)g.offs,
                   cfg.ecp_nl_lmax_p1, cfg.ecp_nl_terms,
-                  (const T*)sign + b0, (const T*)logp + b0, (const T*)sv, (const T*)lv, nb, B, (T*)E + b0,
+                  (const T*)sign + b0, (const T*)logp + b0, (const T*)g.sign, (const T*)g.logp, nb, B, (T*)E + b0,
                   (T*)stats + b0);
-        if (dry) break;  // planning pass: the first group is the largest
-      }
+        return 0;
+      };
+      rc = virtual_groups(r, R, B, (int64_t)J * N * 12, kVirtEcp, !std::getenv("DQMC_ECP_ENV_TABLE_OFF"),
+                          !std::getenv("DQMC_ECP_EMB_TABLE_OFF"), ws, wsb, "workspace too small for the non-local ECP pass",
+                          [&](Arena& a, int64_t nb) { return carve_ecp_group(a, nb); }, setup, finish, st);
+      if (rc) return rc;
     }
     DQ_CHECK(cudaGetLastError());
     return 0;
@@ -2557,58 +2589,28 @@ struct Engine : EngineBase {
       DQ_CHECK(cudaGetLastError());
       return 0;
     }
-    int64_t Be = std::min<int64_t>(B, spin_group_cap(Pn));
-    if (spin_bytes(Be, Pn) > wsb) {  // largest walker group whose virtual walkers fit the workspace
-      int64_t lo = 0, hi = Be;
-      while (hi - lo > 1) {
-        const int64_t mid = (lo + hi) / 2;
-        if (spin_bytes(mid, Pn) <= wsb) lo = mid; else hi = mid;
-      }
-      Be = lo;
-    }
-    if (Be < 1) Be = 1;  // one walker's virtual walkers do not fit at once: the plain-forward pass chunks them
-    if (spin_prefix_bytes(Be, Pn) + (int64_t)chunk_bytes(1, 1) > wsb) { err = "workspace too small for the spin pass"; return 3; }
-    for (int b0 = 0; b0 < B; b0 += (int)Be) {
-      const int nb = (int)std::min<int64_t>(Be, B - b0);
-      const int64_t V = (int64_t)nb * Pn;
-      char* p = (char*)ws;
-      T* rv = (T*)p; p += align_up(sizeof(T) * V * 3 * N);
-      T* sv = (T*)p; p += align_up(sizeof(T) * V);
-      T* lv = (T*)p; p += align_up(sizeof(T) * V);
-      T* s0 = (T*)p; p += align_up(sizeof(T) * nb);
-      T* l0 = (T*)p; p += align_up(sizeof(T) * nb);
-      T* envt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * K * N);
-      T* embt = (T*)p; p += align_up(sizeof(T) * (size_t)nb * N * d);
-      note_hwm(p);
+    auto setup = [&](int b0, int nb, const VirtGroup& g, const Arena& rest, int64_t& V) {
       const T* rb = r + (size_t)b0 * 3 * N;
-      const int64_t rest = wsb - (p - (char*)ws);
-      int rc = 0;
       if (!sign_) {
-        rc = run_batched(rb, R, 0, nb, 1, s0, l0, nullptr, nullptr, nullptr, p, rest, st);
+        int rc = run_batched(rb, R, 0, nb, 1, g.sign0, g.logp0, nullptr, nullptr, nullptr, rest.top, rest.left(), st);
         if (rc) return rc;
       }
+      V = (int64_t)nb * Pn;
       const int64_t ne = V * 3 * N;
-      DQ_LAUNCH(spin_pairs_kernel<T>, dim3((unsigned)((ne + 255) / 256)), dim3(256), 0, st, rb, N, nu, down_idx, (int)Pn, ne, rv);
-      if (cfg.kind == DQMC_PSIFORMER && slater_fwd2_ok && N <= 32 && !dry) {
-        // a swapped walker differs from its base walker in two electrons: the forwards take every other electron's envelopes
-        // (slater_fwd2_kernel) and embedding rows (whole-trunk kernel) from tables of the base walkers
-        DQ_LAUNCH(env_table_kernel<T>, dim3(nb), dim3(256), sizeof(T) * N * M, st, rb, R, N, M, nu, K * N, P("env.pi_up"),
-                  P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), env_rep, envt);
-        ecp_env = envt; ecp_vper = (int)Pn; virt_layout = down_idx;
-        if (embed_fwd_ok && can_trunk(1)) {
-          DQ_LAUNCH(embed_fwd_kernel<T>, dim3((nb * N + 31) / 32), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, rb, R, 0, N, M,
-                    nu, 1, P("emb.w"), d, embt, nb * N, 32, 0LL, 0, (const int*)nullptr);
-          ecp_emb = embt;
-        }
-      }
-      rc = run_batched(rv, R, 0, (int)V, 1, sv, lv, nullptr, nullptr, nullptr, p, rest, st);
-      ecp_env = nullptr; ecp_emb = nullptr; virt_layout = kVirtEcp;
-      if (rc) return rc;
+      DQ_LAUNCH(spin_pairs_kernel<T>, dim3((unsigned)((ne + 255) / 256)), dim3(256), 0, st, rb, N, nu, down_idx, (int)Pn, ne, g.r);
+      return 0;
+    };
+    auto finish = [&](int b0, int nb, const VirtGroup& g) {
       DQ_LAUNCH(spin_accumulate_kernel<T>, dim3((nb + 3) / 4), dim3(128), 0, st,
-                sign_ ? (const T*)sign_ + b0 : (const T*)s0, sign_ ? (const T*)logp_ + b0 : (const T*)l0,
-                (const T*)sv, (const T*)lv, (int)Pn, nb, c0, (T*)s2_ + b0, ratio_ ? (T*)ratio_ + (size_t)b0 * Pn : (T*)nullptr);
-      if (dry) break;  // planning pass: the first group is the largest
-    }
+                sign_ ? (const T*)sign_ + b0 : (const T*)g.sign0, sign_ ? (const T*)logp_ + b0 : (const T*)g.logp0,
+                (const T*)g.sign, (const T*)g.logp, (int)Pn, nb, c0, (T*)s2_ + b0, ratio_ ? (T*)ratio_ + (size_t)b0 * Pn : (T*)nullptr);
+      return 0;
+    };
+    // a swapped walker differs from its base walker in two electrons: the forwards take every other electron's envelopes and
+    // embedding rows from tables of the base walkers
+    int rc = virtual_groups(r, R, B, Pn, down_idx, cfg.kind == DQMC_PSIFORMER, true, ws, wsb, "workspace too small for the spin pass",
+                            [&](Arena& a, int64_t nb) { return carve_spin_group(a, nb, Pn); }, setup, finish, st);
+    if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
     return 0;
   }
@@ -2622,15 +2624,10 @@ struct Engine : EngineBase {
     // max_age override and without step-size adaptation.  ex_flags[n_sub] (host) / ex_idx[n_sub][B][2] (device): injected.
     T* r = (T*)r_; T* sign = (T*)sign_; T* logp = (T*)logp_; T* tau = (T*)tau_; T* stats = (T*)stats_;
     const T* R = (const T*)R_;
-    char* p = (char*)ws;
-    T* rp = (T*)p; p += align_up(sizeof(T) * (size_t)B * 3 * N);
-    T* sp = (T*)p; p += align_up(sizeof(T) * (size_t)B);
-    T* lp = (T*)p; p += align_up(sizeof(T) * (size_t)B);
-    int* cnt = (int*)p; p += 256;
-    int64_t rest = wsb - (p - (char*)ws);
-    note_hwm(p);
-    if (rest < 0) { err = "workspace too small (proposal buffers)"; return 3; }
-    DQ_CHECK(cudaMemsetAsync(cnt, 0, sizeof(int), st));
+    Arena a(this, ws, wsb);
+    const Proposals q = carve_proposals(a, B, false);
+    if (a.left() < 0) { err = "workspace too small (proposal buffers)"; return 3; }
+    DQ_CHECK(cudaMemsetAsync(q.cnt, 0, sizeof(int), st));
     const int ne = B * 3 * N;
     for (int s = 0; s < n_sub; ++s) {
       const T* nns = nn ? (const T*)nn + (size_t)s * ne : nullptr;
@@ -2643,21 +2640,21 @@ struct Engine : EngineBase {
         exchange = Philox::u01(w4[0], w4[1]) < p_exchange;
       }
       if (exchange)
-        DQ_LAUNCH(exchange_propose_kernel<T>, dim3((B + 127) / 128), dim3(128), 0, st, (const T*)r, rp,
+        DQ_LAUNCH(exchange_propose_kernel<T>, dim3((B + 127) / 128), dim3(128), 0, st, (const T*)r, q.r,
                   ex_idx ? ex_idx + (size_t)s * 2 * B : (const int32_t*)nullptr, seed, step0 + (uint64_t)s, woff, cfg.n_up, N, B);
       else
-      DQ_LAUNCH(propose_kernel<T>, dim3((ne / 2 + 1 + 127) / 128), dim3(128), 0, st, (const T*)r, rp, (const T*)tau, nns,
+      DQ_LAUNCH(propose_kernel<T>, dim3((ne / 2 + 1 + 127) / 128), dim3(128), 0, st, (const T*)r, q.r, (const T*)tau, nns,
                 seed, step0 + (uint64_t)s, woff * (uint64_t)(3 * N), ne);
-      int rc = run_batched(rp, R, Rb, B, 1, sp, lp, nullptr, nullptr, nullptr, p, rest, st);
+      int rc = run_batched(q.r, R, Rb, B, 1, q.sign, q.logp, nullptr, nullptr, nullptr, a.top, a.left(), st);
       if (rc) return rc;
-      DQ_LAUNCH(accept_kernel<T>, dim3((B + 127) / 128), dim3(128), 0, st, r, (const T*)rp, sign, (const T*)sp, logp,
-                (const T*)lp, age, nus, seed, step0 + (uint64_t)s, woff, exchange ? -1 : max_age, B, N, cnt);
-      DQ_LAUNCH(tau_kernel<T>, dim3(1), dim3(32), 0, st, tau, cnt, B, exchange ? T(0) : (T)target, stats);
+      DQ_LAUNCH(accept_kernel<T>, dim3((B + 127) / 128), dim3(128), 0, st, r, (const T*)q.r, sign, (const T*)q.sign, logp,
+                (const T*)q.logp, age, nus, seed, step0 + (uint64_t)s, woff, exchange ? -1 : max_age, B, N, q.cnt);
+      DQ_LAUNCH(tau_kernel<T>, dim3(1), dim3(32), 0, st, tau, q.cnt, B, exchange ? T(0) : (T)target, stats);
     }
     DQ_LAUNCH(sampler_stats_kernel<T>, dim3(1), dim3(256), 0, st, (const T*)r, (const T*)logp, (const int*)age,
               (const T*)tau, B, N, stats);
     DQ_CHECK(cudaGetLastError());
-    return 0;
+    return check_guards();  // the proposal buffers' guards, after the last accept (and with n_sub == 0)
   }
 };
 

@@ -7,7 +7,7 @@ round's GPU minutes ran out was first checked here (DESIGN.md section 8).  What 
     shared memory of every block (tools/cuda_emu/cuda_emu.h),
   * DQMC_EMU_REVERSE=1: the threads of a block run from the highest index down (a missing barrier passes in one order at most),
   * DQMC_EMU_REVERSE_BLOCKS=1: the grid is walked backwards (blocks of one launch that depend on each other),
-  * guard zones behind every buffer carved from the engine workspace (engine.cu DQ_TAKE_GUARD), verified after each chunk,
+  * guard zones behind every buffer carved from the engine workspace (engine.cu Arena::take), verified after each chunk,
   * --asan: the kernels are compiled with AddressSanitizer (out-of-bounds global accesses; run with
     LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0:detect_stack_use_after_return=0).
 The wgmma / TMA kernels are not emulated (the build sets DQMC_NO_TCGEN05): engines are created with gemm_backend = 0.
