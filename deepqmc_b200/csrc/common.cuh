@@ -75,20 +75,6 @@ __device__ __forceinline__ void st4(T* p, const T (&v)[4]) {
   }
 }
 
-// cp.async group control for software pipelines: commit the copies issued so far as one group;
-// wait until at most `N` groups are still in flight.
-__device__ __forceinline__ void cp_async_commit() {
-#ifndef DQMC_EMU
-  asm volatile("cp.async.commit_group;" ::: "memory");
-#endif
-}
-template <int N>
-__device__ __forceinline__ void cp_async_wait_group() {
-#ifndef DQMC_EMU
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-#endif
-}
-
 // The (up, down) pair that virtual walker p of the spin pass swaps (reference: physics.py:186-223).  down_idx < 0: exact
 // estimator, all n_up n_down pairs, p = a n_down + (beta - n_up); otherwise spin-raising, beta = down_idx and p = a.
 __host__ __device__ __forceinline__ void spin_pair(int p, int n_up, int N, int down_idx, int& a, int& beta) {

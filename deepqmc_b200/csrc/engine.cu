@@ -9,6 +9,7 @@
 #include <limits>
 #include <map>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -64,6 +65,45 @@ static double ecp_cutoff_rc2(const T* nl, int L, int Tn, bool on) {
     (w(mid) >= eps ? lo : hi) = mid;
   }
   return lo;
+}
+
+// The A/B switches (DESIGN §9), read from the environment once, when an engine is created.  A flag switch is on when its
+// variable is set, whatever the value; the DQMC_ATTN_TB / DQMC_ATTN_NT values are range-checked where they are used.
+struct Switches {
+  bool tc_trunk = true;              // DQMC_TC_TRUNK=0: plain forwards without the whole-trunk kernel
+  bool tc_f16 = true;                // DQMC_TC_F16=0: plain forwards on 3xTF32 instead of 3xFP16 row GEMMs
+  std::optional<bool> attn_fl_mma;   // DQMC_ATTN_FL_MMA=0 / 1: force the SIMT / tensor-core forward-Laplacian attention
+  std::optional<int> attn_tb, attn_nt;  // DQMC_ATTN_TB, DQMC_ATTN_NT: its tangent slots per chunk, threads per block
+  bool attn_generic = false;         // DQMC_ATTN_GENERIC
+  bool no_fuse_tanh = false;         // DQMC_NO_FUSE_TANH
+  bool slater_generic = false;       // DQMC_SLATER_GENERIC
+  bool slater_fwd1 = false;          // DQMC_SLATER_FWD1
+  bool ecp_cutoff = true;            // DQMC_ECP_CUTOFF=0: every (nucleus, electron) pair runs its quadrature forwards
+  bool ecp_env_table = true;         // DQMC_ECP_ENV_TABLE_OFF
+  bool ecp_emb_table = true;         // DQMC_ECP_EMB_TABLE_OFF
+  int nsms = 0;                      // DQMC_NSMS >= 1: SM count the persistent kernels size their grids by (test hook)
+  bool trunk_phases = false;         // DQMC_TRUNK_PHASES=1: the whole-trunk kernel's phase timers
+};
+
+inline Switches read_switches() {
+  auto env = [](const char* name) { return std::getenv(name); };
+  auto num = [&](const char* name) { const char* ev = env(name); return ev ? std::optional<int>(std::atoi(ev)) : std::nullopt; };
+  Switches s;
+  s.tc_trunk = num("DQMC_TC_TRUNK").value_or(1) != 0;
+  s.tc_f16 = num("DQMC_TC_F16").value_or(1) != 0;
+  if (auto v = num("DQMC_ATTN_FL_MMA")) s.attn_fl_mma = *v != 0;
+  s.attn_tb = num("DQMC_ATTN_TB");
+  s.attn_nt = num("DQMC_ATTN_NT");
+  s.attn_generic = env("DQMC_ATTN_GENERIC");
+  s.no_fuse_tanh = env("DQMC_NO_FUSE_TANH");
+  s.slater_generic = env("DQMC_SLATER_GENERIC");
+  s.slater_fwd1 = env("DQMC_SLATER_FWD1");
+  s.ecp_cutoff = num("DQMC_ECP_CUTOFF").value_or(1) != 0;
+  s.ecp_env_table = !env("DQMC_ECP_ENV_TABLE_OFF");
+  s.ecp_emb_table = !env("DQMC_ECP_EMB_TABLE_OFF");
+  s.nsms = num("DQMC_NSMS").value_or(0);
+  s.trunk_phases = num("DQMC_TRUNK_PHASES").value_or(0) != 0;
+  return s;
 }
 
 struct EngineBase {
@@ -417,8 +457,6 @@ struct Engine : EngineBase {
   bool attn_f32 = false;
   bool gemm_ran_tc = false;   // the last gemm() call ran the tensor-core kernel (not the CUDA-core gemm_kernel)
   bool embed_fwd_ok = false;
-  bool attn_fwd_ok = false;
-  bool attn_fwd_pipelined = false;
   bool attn_mma_ok = false;  // plain-forward attention on mma.sync (attn_mma.cuh)
   bool slater_fwd2_ok = false;
   int N, M, d, K, KN, H, dh, T3;
@@ -430,6 +468,7 @@ struct Engine : EngineBase {
   int Mn = 0, env_rep = 1;
   size_t max_smem = 0;
   int n_sms = 132;
+  Switches sw;  // read_switches() at the start of init()
   // compact virtual-walker group in flight (non-local ECP quadrature or spin swaps): envelope table of its base walkers
   // [nb][N][K N] (null outside those forwards), index of the current chunk's first virtual walker, virtual walkers per base
   // walker (J N 12, or the swapped pairs), and the layout of virtual_move (common.cuh)
@@ -448,12 +487,9 @@ struct Engine : EngineBase {
     uint16_t* h16 = nullptr; CUtensorMap m16h, m16l, m16h_all, m16l_all; float wscale = 1.f; bool f16 = false, f16_all = false;
     CUtensorMap m16h_256, m16l_256; bool f16_256 = false;  // 256-row boxes of 32 halves: weight slots of the whole-trunk kernel (trunk_tc.cuh)
   };
-  bool fuse_trunk = true;  // all layers of a plain forward in one persistent launch (trunk_tc.cuh); DQMC_TC_TRUNK=0 disables
   CUtensorMap* d_trunk_maps = nullptr;       // [L][4][2]
   unsigned char* d_trunk_scratch = nullptr;  // n_sms x 512 KB: Q / K / V and residual rows of a tile
   unsigned long long* d_trunk_phase = nullptr;  // DQMC_TRUNK_PHASES=1: the whole-trunk kernel's phase timers (tc::kPhases)
-  bool f16_on = true;      // plain forwards (S = 1) on f16 wgmma with hi / lo half operands; DQMC_TC_F16=0: stay on 3xTF32
-  bool fuse_mlp = true;    // W_o + residual -> W1 + tanh -> W2 + tanh + residual in one launch (S = 1); DQMC_TC_FUSE_MLP=0 disables
   static constexpr float kActScale = 16.f;  // 2^4: |activation| < 4094 representable, absolute floor 2^-29
   std::map<std::string, TcWeight> tcw;
   bool use_tc() const { return std::is_same<T, float>::value && cfg.gemm_backend == DQMC_GEMM_TCGEN05; }
@@ -504,6 +540,7 @@ struct Engine : EngineBase {
 #endif
 
   int init() {
+    sw = read_switches();
     N = cfg.n_up + cfg.n_down; M = cfg.n_nuc; d = cfg.embedding_dim; K = cfg.n_determinants;
     KN = K * N; H = cfg.n_heads; dh = d / H; T3 = 3 * N;
     BFW = KN * (cfg.backflow_add == 2 ? 2 : 1);
@@ -572,10 +609,8 @@ struct Engine : EngineBase {
         DQ_CHECK(cudaMemcpy(d_nl_params, np.data(), sizeof(T) * np.size(), cudaMemcpyHostToDevice));
         DQ_CHECK(cudaMalloc((void**)&d_nl_nuc, sizeof(int) * J));
         DQ_CHECK(cudaMemcpy(d_nl_nuc, nuc.data(), sizeof(int) * J, cudaMemcpyHostToDevice));
-        const char* ev = std::getenv("DQMC_ECP_CUTOFF");
-        const bool cutoff = !(ev && std::atoi(ev) == 0);
         std::vector<double> rc2(J);
-        for (int j = 0; j < J; ++j) rc2[j] = ecp_cutoff_rc2(np.data() + (size_t)nuc[j] * L * 2 * Tn, L, Tn, cutoff);
+        for (int j = 0; j < J; ++j) rc2[j] = ecp_cutoff_rc2(np.data() + (size_t)nuc[j] * L * 2 * Tn, L, Tn, sw.ecp_cutoff);
         DQ_CHECK(cudaMalloc((void**)&d_nl_rc2, sizeof(double) * J));
         DQ_CHECK(cudaMemcpy(d_nl_rc2, rc2.data(), sizeof(double) * J, cudaMemcpyHostToDevice));
       }
@@ -587,33 +622,31 @@ struct Engine : EngineBase {
       if (v > 0) n_sms = v;
     }
 #endif
-    if (const char* ev = std::getenv("DQMC_NSMS")) { int x = std::atoi(ev); if (x >= 1) n_sms = x; }  // test hook
+    if (sw.nsms >= 1) n_sms = sw.nsms;
     // opt in to large dynamic shared memory
     const bool psif = cfg.kind == DQMC_PSIFORMER || trans;
-    attn_tb = attn_pick_tb<T>(N, dh, T3, 100 * 1024, Mn);
     // the specialised fp32 attention kernels do not take extra tokens yet: TransPsiformer runs the generic one
-    attn_f32 = psif && !trans && std::is_same<T, float>::value && dh % 16 == 0 && !std::getenv("DQMC_ATTN_GENERIC");
-    if (attn_f32) attn_tb = attn_f32_pick_tb(N, dh, T3, 32 * 1024);  // ~7 blocks/SM for small molecules
-    if (const char* ev = std::getenv("DQMC_ATTN_TB")) { int x = std::atoi(ev); if (x >= 1 && x <= T3) attn_tb = x; }
-    if (const char* ev = std::getenv("DQMC_ATTN_NT")) { int x = std::atoi(ev); if (x >= 32 && x <= 1024 && x % 32 == 0) attn_fl_threads = x; }
+    attn_f32 = psif && !trans && std::is_same<T, float>::value && dh % 16 == 0 && !sw.attn_generic;
+    // forward-Laplacian tangent slots per chunk: DQMC_ATTN_TB if it is in 1 .. 3N; fp32: ~7 blocks/SM for small molecules
+    if (sw.attn_tb && *sw.attn_tb >= 1 && *sw.attn_tb <= T3) attn_tb = *sw.attn_tb;
+    else attn_tb = attn_f32 ? attn_f32_pick_tb(N, dh, T3, 32 * 1024) : attn_pick_tb<T>(N, dh, T3, 100 * 1024, Mn);
     size_t s_attn = !psif ? 0 : attn_f32 ? attn_f32_smem_bytes(N, dh, attn_tb) : attn_smem_bytes<T>(N, dh, attn_tb, Mn);
     // few resident blocks per SM (large molecules: the tangent chunk fills the shared memory) -> more warps per block
     // (benzene, one 170 KB block per SM: 128 threads 707 ms per 512-walker step, 512 threads 684 ms)
-    if (!std::getenv("DQMC_ATTN_NT")) attn_fl_threads = s_attn > 110 * 1024 ? 512 : (s_attn > 56 * 1024 ? 256 : 128);
+    if (!sw.attn_nt) attn_fl_threads = s_attn > 110 * 1024 ? 512 : (s_attn > 56 * 1024 ? 256 : 128);
+    else if (*sw.attn_nt >= 32 && *sw.attn_nt <= 1024 && *sw.attn_nt % 32 == 0) attn_fl_threads = *sw.attn_nt;
     // 16 x 8 tiles: worthwhile from about 20 electrons (benzene, N = 30: 686 -> 648 ms per 512-walker step; LiH, N = 4, where
     // 7/8 of every tile is padding: 6.9 -> 15.7 ms, so small molecules keep the SIMT variant)
-    attn_fl_mma = attn_f32 && N >= 20 && N <= 32 && dh % 16 == 0;
-    if (const char* ev = std::getenv("DQMC_ATTN_FL_MMA")) attn_fl_mma = attn_f32 && N <= 32 && dh % 16 == 0 && std::atoi(ev) != 0;
-    if (attn_fl_mma && !std::getenv("DQMC_ATTN_TB")) {  // two resident blocks of 8 warps per SM
+    attn_fl_mma = attn_f32 && N <= 32 && dh % 16 == 0 && sw.attn_fl_mma.value_or(N >= 20);
+    if (attn_fl_mma && !sw.attn_tb) {  // two resident blocks of 8 warps per SM
       attn_tb = attn_f32_pick_tb(N, dh, T3, 110 * 1024);
       s_attn = attn_f32_smem_bytes(N, dh, attn_tb);
     }
     // generic kernel (extra key / value tokens: TransPsiformer) in fp32: same tensor-core products, row pitch dh + 4
-    attn_gen_mma = psif && !attn_f32 && std::is_same<T, float>::value && N >= 20 && dh % 16 == 0 && !std::getenv("DQMC_ATTN_GENERIC");
-    if (const char* ev = std::getenv("DQMC_ATTN_FL_MMA"))
-      attn_gen_mma = psif && !attn_f32 && std::is_same<T, float>::value && dh % 16 == 0 && std::atoi(ev) != 0;
+    attn_gen_mma = psif && !attn_f32 && std::is_same<T, float>::value && dh % 16 == 0 &&
+                   sw.attn_fl_mma.value_or(N >= 20 && !sw.attn_generic);
     if (attn_gen_mma) {
-      if (!std::getenv("DQMC_ATTN_TB")) attn_tb = attn_pick_tb<T>(N, dh, T3, 110 * 1024, Mn, 4);
+      if (!sw.attn_tb) attn_tb = attn_pick_tb<T>(N, dh, T3, 110 * 1024, Mn, 4);
       s_attn = attn_smem_bytes<T>(N, dh, attn_tb, Mn, 4);
     }
     size_t s_sl = slater_smem_bytes<T>(N);
@@ -626,8 +659,7 @@ struct Engine : EngineBase {
       if constexpr (std::is_same<T, float>::value) DQ_CHECK(raise_dyn_smem((attn_fl_kernel<T, true>), (int)s_attn));
     }
     DQ_CHECK(raise_dyn_smem(slater_kernel<T>, (int)s_sl));
-    slater_fwd2_ok = N <= 32 && slater_fwd2_smem_bytes<T>(N, M, K) <= 110 * 1024 && !std::getenv("DQMC_SLATER_GENERIC") &&
-                     !std::getenv("DQMC_SLATER_FWD1");
+    slater_fwd2_ok = N <= 32 && slater_fwd2_smem_bytes<T>(N, M, K) <= 110 * 1024 && !sw.slater_generic && !sw.slater_fwd1;
     if (slater_fwd2_ok) {
       DQ_CHECK(raise_dyn_smem(slater_fwd2_kernel<T, 14>, (int)slater_fwd2_smem_bytes<T>(N, M, K)));
       DQ_CHECK(raise_dyn_smem(slater_fwd2_kernel<T, 16>, (int)slater_fwd2_smem_bytes<T>(N, M, K)));
@@ -635,30 +667,8 @@ struct Engine : EngineBase {
       DQ_CHECK(raise_dyn_smem(slater_fwd2_kernel<T, 30>, (int)slater_fwd2_smem_bytes<T>(N, M, K)));
       DQ_CHECK(raise_dyn_smem(slater_fwd2_kernel<T, 32>, (int)slater_fwd2_smem_bytes<T>(N, M, K)));
     }
-    attn_fwd_ok = psif && std::is_same<T, float>::value && dh == 64 && N <= 32 && N + Mn <= 48 && d % 4 == 0 &&
-                  !std::getenv("DQMC_ATTN_GENERIC") && !std::getenv("DQMC_ATTN_FWD_OLD");
-    attn_fwd_pipelined = attn_fwd_ok && !trans && std::getenv("DQMC_ATTN_FWD2");  // measured slower than the block-per-walker kernel
-    if (attn_fwd_pipelined) {
-      const int smem2 = 6 * 4 * N * 64 * (int)sizeof(float);
-      DQ_CHECK(raise_dyn_smem(attn_fwd2_f32_kernel<8>, smem2));
-      DQ_CHECK(raise_dyn_smem(attn_fwd2_f32_kernel<16>, smem2));
-      DQ_CHECK(raise_dyn_smem(attn_fwd2_f32_kernel<32>, smem2));
-    }
-    if (attn_fwd_ok) {
-      const int smem = 4 * 2 * (N + Mn) * 64 * (int)sizeof(float);
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<48, false>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<8, false>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<16, false>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<32, false>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<4, true>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<10, true>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<14, true>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<28, true>), smem));
-      DQ_CHECK(raise_dyn_smem((attn_fwd_f32_kernel<30, true>), smem));
-    }
-    attn_mma_ok = psif && std::is_same<T, float>::value && dh == 64 && N + Mn <= 48 && d % 4 == 0 && !std::getenv("DQMC_ATTN_GENERIC") &&
-                  !(std::getenv("DQMC_ATTN_MMA") && std::atoi(std::getenv("DQMC_ATTN_MMA")) == 0);
-    embed_fwd_ok = psif && d % 4 == 0 && embed_fwd_smem_bytes<T>(M, d) <= 200 * 1024 && !std::getenv("DQMC_EMBED_GENERIC");
+    attn_mma_ok = psif && std::is_same<T, float>::value && dh == 64 && N + Mn <= 48 && d % 4 == 0 && !sw.attn_generic;
+    embed_fwd_ok = psif && d % 4 == 0 && embed_fwd_smem_bytes<T>(M, d) <= 200 * 1024;
     if (embed_fwd_ok)
       DQ_CHECK(raise_dyn_smem(embed_fwd_kernel<T>, (int)embed_fwd_smem_bytes<T>(M, d)));
     if (cfg.gemm_backend == DQMC_GEMM_TCGEN05) {
@@ -670,13 +680,10 @@ struct Engine : EngineBase {
       DQ_CHECK(raise_dyn_smem(tc::mlp_block_f16_kernel<128>, tc::MlpSmem::total()));
       DQ_CHECK(raise_dyn_smem(tc::mlp_block_f16_kernel<256>, tc::MlpSmem::total()));
       DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel, tc::TrSmem::total()));
-      if (const char* ev = std::getenv("DQMC_TC_F16")) f16_on = std::atoi(ev) != 0;
-      if (const char* ev = std::getenv("DQMC_TC_FUSE_MLP")) fuse_mlp = std::atoi(ev) != 0;
-      if (const char* ev = std::getenv("DQMC_TC_TRUNK")) fuse_trunk = std::atoi(ev) != 0;
       if (psif && !trans && d == 256 && H == 4 && N <= 32 && cfg.n_layers <= tc::kTrMaxLayers) {
         DQ_CHECK(cudaMalloc((void**)&d_trunk_maps, sizeof(CUtensorMap) * 8 * cfg.n_layers));
         DQ_CHECK(cudaMalloc((void**)&d_trunk_scratch, (size_t)n_sms * tc::kTrScratchPerCta));
-        if (const char* ev = std::getenv("DQMC_TRUNK_PHASES"); ev && std::atoi(ev) != 0) {
+        if (sw.trunk_phases) {
           DQ_CHECK(cudaMalloc((void**)&d_trunk_phase, sizeof(unsigned long long) * tc::kPhases));
           DQ_CHECK(cudaMemset(d_trunk_phase, 0, sizeof(unsigned long long) * tc::kPhases));
         }
@@ -1004,7 +1011,7 @@ struct Engine : EngineBase {
   // dense layers can absorb the tanh propagation in the tensor-core epilogue when whole slot
   // groups fit a 128-row tile with little padding
   bool can_fuse_act(int S) const {
-    if (!use_tc() || std::getenv("DQMC_NO_FUSE_TANH")) return false;
+    if (!use_tc() || sw.no_fuse_tanh) return false;
     if (S == 1) return true;
     return S <= 128 && (128 / S) * S >= 112;
   }
@@ -1028,7 +1035,7 @@ struct Engine : EngineBase {
         p.rpt = (act && S > 1) ? (128 / S) * S : tc::kBM;
         p.a_scale = 1.f; p.unscale = 1.f;
         // plain forwards: half operands (hi / lo), f16 wgmma -- twice the MMA rate, half the shared-memory bytes per k
-        const bool f16 = S == 1 && f16_on && Kc % 64 == 0 && t0.f16 && t1.f16 && t0.wscale == t1.wscale;
+        const bool f16 = S == 1 && sw.tc_f16 && Kc % 64 == 0 && t0.f16 && t1.f16 && t0.wscale == t1.wscale;
         if (f16) { p.a_scale = kActScale; p.unscale = 1.f / (kActScale * t0.wscale); }
         const int MT = (Mr + p.rpt - 1) / p.rpt, NT = (Nc + tc::kBN - 1) / tc::kBN;
         const int n_tiles = (sliced ? Nel : 1) * MT * NT;  // one tile per CTA
@@ -1076,7 +1083,7 @@ struct Engine : EngineBase {
   // Fused MLP block of a plain forward: Out = A + tanh(tanh(A W1 + b1) W2 + b2), A = X + O Wo  (one launch; fused_tc.cuh)
   bool can_fuse_mlp(int S, const std::string& pfx) const {
 #if !defined(DQMC_NO_TCGEN05)
-    if (S != 1 || !use_tc() || !f16_on || !fuse_mlp || (d != 128 && d != 256)) return false;
+    if (S != 1 || !use_tc() || !sw.tc_f16 || (d != 128 && d != 256)) return false;
     for (const char* n : {"wo", "w1", "w2"}) {
       auto it = tcw.find(pfx + n);
       if (it == tcw.end() || !it->second.f16_all) return false;
@@ -1147,7 +1154,7 @@ struct Engine : EngineBase {
   }
   bool can_trunk(int S) const {
 #if !defined(DQMC_NO_TCGEN05)
-    return S == 1 && use_tc() && f16_on && fuse_trunk && d_trunk_maps && d_trunk_scratch && cfg.n_layers >= 1 && trunk_weights_ok();
+    return S == 1 && use_tc() && sw.tc_f16 && sw.tc_trunk && d_trunk_maps && d_trunk_scratch && cfg.n_layers >= 1 && trunk_weights_ok();
 #else
     return false;
 #endif
@@ -1549,43 +1556,6 @@ struct Engine : EngineBase {
           default: DQ_ATTN_MMA(6); break;
         }
 #undef DQ_ATTN_MMA
-      } else if (S == 1 && attn_fwd_ok && attn_fwd_pipelined) {
-        which = DQMC_ATTN_KERNEL_FWD2;
-        // persistent blocks (one per SM), 6 warps each, K / V of the next pair prefetched by cp.async
-        const int n_pairs = Bc * H, wpb = 6;
-        const int smem = wpb * 4 * N * 64 * (int)sizeof(float);
-        const int nblk = (n_pairs + wpb - 1) / wpb;
-        const dim3 grid(nblk < n_sms ? nblk : n_sms), block(32 * wpb);
-        if (N <= 8)
-          DQ_LAUNCH(attn_fwd2_f32_kernel<8>, grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d,
-                    (float)scale, n_pairs);
-        else if (N <= 16)
-          DQ_LAUNCH(attn_fwd2_f32_kernel<16>, grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d,
-                    (float)scale, n_pairs);
-        else
-          DQ_LAUNCH(attn_fwd2_f32_kernel<32>, grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d,
-                    (float)scale, n_pairs);
-      } else if (S == 1 && attn_fwd_ok) {
-        which = DQMC_ATTN_KERNEL_FWD;
-        const int n_pairs = Bc * H;
-        const int smem = 4 * 2 * (N + Mn) * 64 * (int)sizeof(float);
-        const dim3 grid((n_pairs + 3) / 4), block(128);
-#define DQ_ATTN_FWD(NM_, EX_)                                                                                          \
-  DQ_LAUNCH((attn_fwd_f32_kernel<NM_, EX_>), grid, block, smem, st, (const float*)QKV, 3 * d, (float*)O, d, N, H, d, \
-        (float)scale, n_pairs, (const float*)kn, (const float*)vn, Mn)
-        switch (Mn > 0 ? -1 : N) {  // exact-size instances for the benchmark molecules, padded generic ones otherwise
-          case 4: DQ_ATTN_FWD(4, true); break;
-          case 10: DQ_ATTN_FWD(10, true); break;
-          case 14: DQ_ATTN_FWD(14, true); break;
-          case 28: DQ_ATTN_FWD(28, true); break;
-          case 30: DQ_ATTN_FWD(30, true); break;
-          default:
-            if (N + Mn <= 8) DQ_ATTN_FWD(8, false);
-            else if (N + Mn <= 16) DQ_ATTN_FWD(16, false);
-            else if (N + Mn <= 32) DQ_ATTN_FWD(32, false);
-            else DQ_ATTN_FWD(48, false);
-        }
-#undef DQ_ATTN_FWD
       } else if (attn_f32) {
         which = attn_fl_mma && S > 1 ? DQMC_ATTN_KERNEL_FL_F32_MMA : DQMC_ATTN_KERNEL_FL_F32;
         if (launch_attn_f32((const float*)QKV, (float*)O, Bc, S, tb, (float)scale, 0,
@@ -1733,7 +1703,7 @@ struct Engine : EngineBase {
     }
     int32_t which = DQMC_SLATER_KERNEL_GENERIC, inst = 0;
     const int sl_wpb = slater_warps_per_block<T>(N);
-    if ((N <= 4 || (N <= 6 && std::is_same<T, float>::value)) && !qa && !gadd && !std::getenv("DQMC_SLATER_GENERIC")) {
+    if ((N <= 4 || (N <= 6 && std::is_same<T, float>::value)) && !qa && !gadd && !sw.slater_generic) {
       const int tot = Bc * K;
       which = DQMC_SLATER_KERNEL_SMALL;
 #define DQ_SL_SMALL(NS_)                                                                                           \
@@ -1766,7 +1736,7 @@ struct Engine : EngineBase {
       else if (N == 30) { DQ_SL_FWD2(30); }
       else { DQ_SL_FWD2(32); }
 #undef DQ_SL_FWD2
-    } else if (S == 1 && N <= 32 && !gadd && !std::getenv("DQMC_SLATER_GENERIC")) {
+    } else if (S == 1 && N <= 32 && !gadd && !sw.slater_generic) {
       const int wpb = K < 8 ? K : 8;
       which = DQMC_SLATER_KERNEL_FWD_REG;
       DQ_LAUNCH(slater_fwd_reg_kernel<T>, dim3(Bc), dim3(32 * wpb), sizeof(T) * N * M, st, r, R, Rb, N, M, cfg.n_up, K,
@@ -2559,9 +2529,8 @@ struct Engine : EngineBase {
                   (T*)stats + b0);
         return 0;
       };
-      rc = virtual_groups(r, R, B, (int64_t)J * N * 12, kVirtEcp, !std::getenv("DQMC_ECP_ENV_TABLE_OFF"),
-                          !std::getenv("DQMC_ECP_EMB_TABLE_OFF"), ws, wsb, "workspace too small for the non-local ECP pass",
-                          [&](Arena& a, int64_t nb) { return carve_ecp_group(a, nb); }, setup, finish, st);
+      rc = virtual_groups(r, R, B, (int64_t)J * N * 12, kVirtEcp, sw.ecp_env_table, sw.ecp_emb_table, ws, wsb,
+                          "workspace too small for the non-local ECP pass", [&](Arena& a, int64_t nb) { return carve_ecp_group(a, nb); }, setup, finish, st);
       if (rc) return rc;
     }
     DQ_CHECK(cudaGetLastError());

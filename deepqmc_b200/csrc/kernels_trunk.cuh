@@ -962,203 +962,6 @@ __global__ void attn_fl_f32_kernel(const float* __restrict__ QKV, int ldq, float
   }
 }
 
-// ------------------------------------------------------------------------------------------
-// Plain-forward (S == 1) self-attention, fp32, N <= NMAX <= 32 electrons, head dim 64: the
-// attention of every Metropolis sub-step and non-local-ECP quadrature forward.
-// One WARP per (walker, head); lane i owns QUERY i: its q row, its full score row s[i][:] and its
-// output row live in registers, so the softmax is lane-local (no shuffles, no barriers); K and V
-// of the head are staged once in shared memory (cp.async, coalesced) and read as 128-bit
-// broadcasts.  Same algebra / reference lines as attn_fl_kernel (value part).
-// dynamic smem = warps_per_block * 2 * N * 64 * 4 bytes.
-// ------------------------------------------------------------------------------------------
-// EXACT: the key count N == NMAX is known at compile time (and there are no extra tokens) -> the per-key
-// loops carry no branches, so the compiler can hoist the shared-memory loads of several keys above the
-// FMAs that consume them (latency hiding by ILP).
-// Kn / Vn [Mn][dmodel] (nullable): key / value rows of Mn walker-independent extra tokens (TransPsiformer
-// nuclei, see attn_fl_kernel); they sit behind the N electron keys, N + Mn <= NMAX.
-template <int NMAX, bool EXACT>
-__global__ void __launch_bounds__(128)
-attn_fwd_f32_kernel(const float* __restrict__ QKV, int ldq, float* __restrict__ O, int ldo, int N, int H, int dmodel,
-                    float scale, int n_pairs, const float* __restrict__ Kn, const float* __restrict__ Vn, int Mn) {
-  constexpr int DH = 64;
-  DQMC_DYN_SMEM(smem_raw);
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  const int pair = blockIdx.x * wpb + wib;
-  if (pair >= n_pairs) return;
-  const int b = pair / H, h = pair - b * H;
-  const int NK = EXACT ? NMAX : N + Mn;
-  float* ks = reinterpret_cast<float*>(smem_raw) + (size_t)wib * 2 * NK * DH;  // [NK][64]
-  float* vs = ks + NK * DH;                                                     // [NK][64]
-  const float* base = QKV + (size_t)b * N * ldq + h * DH;
-  for (int idx = lane; idx < N * (DH / 4); idx += 32) {
-    const int j = idx >> 4, c4 = idx & 15;
-    const float* src = base + (size_t)j * ldq + 4 * c4;
-    cp_async16(ks + j * DH + 4 * c4, src + dmodel);
-    cp_async16(vs + j * DH + 4 * c4, src + 2 * dmodel);
-  }
-  if (!EXACT) {
-    for (int idx = lane; idx < Mn * (DH / 4); idx += 32) {
-      const int m = idx >> 4, c4 = idx & 15;
-      cp_async16(ks + (N + m) * DH + 4 * c4, Kn + (size_t)m * dmodel + h * DH + 4 * c4);
-      cp_async16(vs + (N + m) * DH + 4 * c4, Vn + (size_t)m * dmodel + h * DH + 4 * c4);
-    }
-  }
-  const int i = lane < N ? lane : N - 1;  // idle lanes shadow the last query (no divergence)
-  float4 q[DH / 4];
-  {
-    const float4* qp = reinterpret_cast<const float4*>(base + (size_t)i * ldq);
-#pragma unroll
-    for (int c = 0; c < DH / 4; ++c) q[c] = __ldg(qp + c);
-  }
-  cp_async_wait_all();
-  __syncwarp();
-  float sc[NMAX];
-  float mx = -3.0e38f;
-#pragma unroll
-  for (int j = 0; j < NMAX; ++j) {
-    sc[j] = -3.0e38f;
-    if (EXACT || j < NK) {
-      const float4* kp = reinterpret_cast<const float4*>(ks + j * DH);
-      float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-      for (int c = 0; c < DH / 4; c += 2) {
-        a0 += dot4(q[c], kp[c]);
-        a1 += dot4(q[c + 1], kp[c + 1]);
-      }
-      sc[j] = (a0 + a1) * scale;
-      mx = fmaxf(mx, sc[j]);
-    }
-  }
-  float sum = 0.f;
-#pragma unroll
-  for (int j = 0; j < NMAX; ++j) {
-    if (EXACT || j < NK) {
-      sc[j] = m_exp(sc[j] - mx);
-      sum += sc[j];
-    }
-  }
-  const float inv = 1.f / sum;
-  float4 o[DH / 4];
-#pragma unroll
-  for (int c = 0; c < DH / 4; ++c) o[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int j = 0; j < NMAX; ++j) {
-    if (EXACT || j < NK) {
-      const float pj = sc[j] * inv;
-      const float4* vp = reinterpret_cast<const float4*>(vs + j * DH);
-#pragma unroll
-      for (int c = 0; c < DH / 4; ++c) fma4(o[c], pj, vp[c]);
-    }
-  }
-  if (lane < N) {
-    float4* op = reinterpret_cast<float4*>(O + ((size_t)b * N + lane) * ldo + h * DH);
-#pragma unroll
-    for (int c = 0; c < DH / 4; ++c) op[c] = o[c];
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// Persistent, software-pipelined variant of attn_fwd_f32_kernel: one block per SM, every warp walks
-// over (walker, head) pairs; while a pair is being computed the K / V rows of the warp's NEXT pair
-// stream into the second shared-memory buffer (cp.async groups) and its query row is already in
-// registers, so no warp ever waits on HBM latency with an empty pipeline.
-// dynamic smem = warps_per_block * 2 buffers * 2 * N * 64 * 4 bytes.
-// ------------------------------------------------------------------------------------------
-template <int NMAX>
-__global__ void __launch_bounds__(192, 1)
-attn_fwd2_f32_kernel(const float* __restrict__ QKV, int ldq, float* __restrict__ O, int ldo, int N, int H, int dmodel,
-                     float scale, int n_pairs) {
-  constexpr int DH = 64;
-  DQMC_DYN_SMEM(smem_raw);
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, wpb = blockDim.x >> 5;
-  const int stride = gridDim.x * wpb;
-  float* buf0 = reinterpret_cast<float*>(smem_raw) + (size_t)wib * 4 * N * DH;  // [2 buffers][K | V][N][64]
-  const int i = lane < N ? lane : N - 1;  // idle lanes shadow the last query (no divergence)
-  auto stage = [&](int pair, float* kb) {  // K rows -> kb, V rows -> kb + N * DH
-    const int b = pair / H, h = pair - b * H;
-    const float* base = QKV + (size_t)b * N * ldq + h * DH;
-    for (int idx = lane; idx < N * (DH / 4); idx += 32) {
-      const int j = idx >> 4, c4 = idx & 15;
-      const float* src = base + (size_t)j * ldq + 4 * c4;
-      cp_async16(kb + j * DH + 4 * c4, src + dmodel);
-      cp_async16(kb + N * DH + j * DH + 4 * c4, src + 2 * dmodel);
-    }
-  };
-  auto load_q = [&](int pair, float4(&q)[DH / 4]) {
-    const int b = pair / H, h = pair - b * H;
-    const float4* qp = reinterpret_cast<const float4*>(QKV + ((size_t)b * N + i) * ldq + h * DH);
-#pragma unroll
-    for (int c = 0; c < DH / 4; ++c) q[c] = __ldg(qp + c);
-  };
-  int pair = blockIdx.x * wpb + wib;
-  if (pair >= n_pairs) return;
-  float4 q[DH / 4], qn[DH / 4];
-  stage(pair, buf0);
-  cp_async_commit();
-  load_q(pair, q);
-  int cur = 0;
-  for (; pair < n_pairs; pair += stride, cur ^= 1) {
-    const int nxt = pair + stride;
-    float* ks = buf0 + (size_t)cur * 2 * N * DH;
-    float* vs = ks + N * DH;
-    if (nxt < n_pairs) {
-      stage(nxt, buf0 + (size_t)(cur ^ 1) * 2 * N * DH);
-      load_q(nxt, qn);
-    }
-    cp_async_commit();
-    cp_async_wait_group<1>();  // everything but the group just committed has landed: the current K / V
-    __syncwarp();
-    float sc[NMAX];
-    float mx = -3.0e38f;
-#pragma unroll
-    for (int j = 0; j < NMAX; ++j) {
-      sc[j] = -3.0e38f;
-      if (j < N) {
-        const float4* kp = reinterpret_cast<const float4*>(ks + j * DH);
-        float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-        for (int c = 0; c < DH / 4; c += 2) {
-          a0 += dot4(q[c], kp[c]);
-          a1 += dot4(q[c + 1], kp[c + 1]);
-        }
-        sc[j] = (a0 + a1) * scale;
-        mx = fmaxf(mx, sc[j]);
-      }
-    }
-    float sum = 0.f;
-#pragma unroll
-    for (int j = 0; j < NMAX; ++j) {
-      if (j < N) {
-        sc[j] = m_exp(sc[j] - mx);
-        sum += sc[j];
-      }
-    }
-    const float inv = 1.f / sum;
-    float4 o[DH / 4];
-#pragma unroll
-    for (int c = 0; c < DH / 4; ++c) o[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int j = 0; j < NMAX; ++j) {
-      if (j < N) {
-        const float pj = sc[j] * inv;
-        const float4* vp = reinterpret_cast<const float4*>(vs + j * DH);
-#pragma unroll
-        for (int c = 0; c < DH / 4; ++c) fma4(o[c], pj, vp[c]);
-      }
-    }
-    if (lane < N) {
-      const int b = pair / H, h = pair - b * H;
-      float4* op = reinterpret_cast<float4*>(O + ((size_t)b * N + lane) * ldo + h * DH);
-#pragma unroll
-      for (int c = 0; c < DH / 4; ++c) op[c] = o[c];
-    }
-    __syncwarp();  // all lanes are done with ks / vs before the next iteration's copies overwrite them
-#pragma unroll
-    for (int c = 0; c < DH / 4; ++c) q[c] = qn[c];
-  }
-  cp_async_wait_group<0>();
-}
-
 inline size_t attn_f32_smem_bytes(int N, int dh, int TB) {
   return sizeof(float) * ((size_t)3 * N * (dh + 4) + (size_t)3 * TB * N * (dh + 4) + (size_t)N * dh +
                           (size_t)N * N * (3 + 2 * TB) + (size_t)TB * N + N + 8);

@@ -718,8 +718,7 @@ class Engine:
         self._check(rc, 'dqmc_debug_trunk')
         return out
 
-    ATTN_KERNELS = ('attn_fwd_mma_kernel', 'attn_fwd2_f32_kernel', 'attn_fwd_f32_kernel', 'attn_fl_f32_kernel', 'attn_fl_kernel',
-                    'attn_fl_f32_kernel_mma', 'attn_fl_kernel_mma')
+    ATTN_KERNELS = ('attn_fwd_mma_kernel', 'attn_fl_f32_kernel', 'attn_fl_kernel', 'attn_fl_f32_kernel_mma', 'attn_fl_kernel_mma')
 
     def debug_attention(self, layer, QKV, S=1):
         """The softmax attention of `layer` (the kernel the engine picks) on Q | K | V rows [rows, 3d] with S slots per electron

@@ -268,7 +268,7 @@ int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, voi
  * (the same Engine::attention the forward calls), on caller-supplied rows QKV [rows][3d] (Q | K | V, head h in columns
  * h dh .. h dh + dh - 1 of each) -> O [rows][d].  rows = walkers x electrons x S in the engine's slot layout: row
  * (b N + i) S + s holds slot s of electron i of walker b.  S = 1: plain forward (fp32, dh = 64, N + nuclear tokens <= 48: the
- * tensor-core attn_fwd_mma_kernel).  S = 3N + 2: forward-Laplacian pass, slot 0 the value, slots 1 .. 3N the tangents, slot
+ * tensor-core attn_fwd_mma_kernel; otherwise the forward-Laplacian kernel of the configuration with one slot).  S = 3N + 2: forward-Laplacian pass, slot 0 the value, slots 1 .. 3N the tangents, slot
  * 3N + 1 the Laplacian (the tangent chunk and the shared memory were sized for this S when the engine was created).
  * TransPsiformer: the keys and values also hold the layer's nuclear tokens from the parameter table (L<layer>.kn / .vn).
  * *kernel (if not null) receives the kernel that ran, one of DQMC_ATTN_KERNEL_*.
@@ -277,12 +277,10 @@ int dqmc_debug_trunk(dqmc_handle h, const void* X0, void* Out, int32_t rows, voi
  * folxext.py:70-171. */
 enum {
   DQMC_ATTN_KERNEL_MMA = 0,     /* attn_fwd_mma_kernel: 3xFP16 mma.sync, fp32 dh = 64, N + nuclear tokens <= 48 */
-  DQMC_ATTN_KERNEL_FWD2 = 1,    /* attn_fwd2_f32_kernel: persistent SIMT plain forward (DQMC_ATTN_FWD2) */
-  DQMC_ATTN_KERNEL_FWD = 2,     /* attn_fwd_f32_kernel: SIMT plain forward, block per walker */
-  DQMC_ATTN_KERNEL_FL_F32 = 3,  /* attn_fl_f32_kernel<., ., false>: fp32 forward-Laplacian attention, SIMT tangent chunks */
-  DQMC_ATTN_KERNEL_GENERIC = 4, /* attn_fl_kernel<T, false>: generic, any dtype, SIMT */
-  DQMC_ATTN_KERNEL_FL_F32_MMA = 5,  /* attn_fl_f32_kernel<., ., true>: tangent chunks as 3xTF32 mma.sync products */
-  DQMC_ATTN_KERNEL_GENERIC_MMA = 6  /* attn_fl_kernel<float, true>: generic fp32 kernel, tangent chunks on the tensor cores */
+  DQMC_ATTN_KERNEL_FL_F32 = 1,  /* attn_fl_f32_kernel<., ., false>: fp32 forward-Laplacian attention, SIMT tangent chunks */
+  DQMC_ATTN_KERNEL_GENERIC = 2, /* attn_fl_kernel<T, false>: generic, any dtype, SIMT */
+  DQMC_ATTN_KERNEL_FL_F32_MMA = 3,  /* attn_fl_f32_kernel<., ., true>: tangent chunks as 3xTF32 mma.sync products */
+  DQMC_ATTN_KERNEL_GENERIC_MMA = 4  /* attn_fl_kernel<float, true>: generic fp32 kernel, tangent chunks on the tensor cores */
 };
 int dqmc_debug_attention(dqmc_handle h, int32_t layer, const void* QKV, void* O, int32_t rows, int32_t S, int32_t* kernel,
                          void* stream);

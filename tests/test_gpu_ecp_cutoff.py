@@ -24,15 +24,17 @@ SMALL = dict(embedding_dim=32, n_layers=2, n_heads=4, n_determinants=4)
 _ENGINES = {}
 
 
-def _engine(mol, dtype, cutoff, **hyper):
-    """(hamil, engine) with the ccECP; cutoff False: created under DQMC_ECP_CUTOFF=0 (every pair active).  fp32 engines take
-    the tensor-core backend.  Same parameters for both settings."""
-    key = (mol, dtype, cutoff, tuple(sorted(hyper.items())))
+def _engine(mol, dtype, cutoff, env=(), **hyper):
+    """(hamil, engine) with the ccECP; cutoff False: created under DQMC_ECP_CUTOFF=0 (every pair active); env: further
+    switches set around its creation.  fp32 engines take the tensor-core backend.  Same parameters for all settings."""
+    key = (mol, dtype, cutoff, tuple(env), tuple(sorted(hyper.items())))
     if key not in _ENGINES:
         hamil = MolecularHamiltonian(mol=Molecule.from_name(mol), ecp_type='ccECP')
         mp = pytest.MonkeyPatch()
         if not cutoff:
             mp.setenv('DQMC_ECP_CUTOFF', '0')
+        for k, v in env:
+            mp.setenv(k, str(v))
         try:
             kw = dict(gemm_backend=1) if dtype == 'float32' else {}
             a = B200Ansatz(hamil, 'psiformer', dtype=dtype, **kw, **hyper)
@@ -186,21 +188,33 @@ def test_benzene_walker_isolation_mixed_active_counts():
     assert torch.equal(E2[0::2], E1[0::2]) and torch.equal(V2[0::2], V1[0::2])
 
 
+# engines without the base walkers' tables: their switches, and the table launches per ECP group they leave out
+# (env_table_kernel, embed_fwd_kernel of the embedding table)
+TABLES_OFF = {'envelope_only': ((('DQMC_ECP_EMB_TABLE_OFF', 1),), 1),
+              'none': ((('DQMC_ECP_EMB_TABLE_OFF', 1), ('DQMC_ECP_ENV_TABLE_OFF', 1)), 2)}
+
+
 @pytest.mark.parametrize('tables', ['both', 'envelope_only', 'none'])
-def test_cutoff_quadrature_chunking_bitwise(monkeypatch, tables):
+def test_cutoff_quadrature_chunking_bitwise(tables):
     """Benzene ccECP, 2 walkers: workspaces whose plain-forward chunks cut the active-pair list at offsets that are not
     multiples of 12 (mid-pair, mid-walker) give V_nl and E_loc bit for bit equal to the default workspace.  With the base
-    walkers' embedding and envelope tables, with the envelope table only, and with neither."""
-    if tables in ('envelope_only', 'none'):
-        monkeypatch.setenv('DQMC_ECP_EMB_TABLE_OFF', '1')
-    if tables == 'none':
-        monkeypatch.setenv('DQMC_ECP_ENV_TABLE_OFF', '1')
-    hamil, eng = _engine('benzene', 'float32', True)
+    walkers' embedding and envelope tables, with the envelope table only, and with neither; the engines created without a
+    table launch its kernel fewer times per ECP group than the default engine, for the same walkers and workspace."""
+    env, per_group = TABLES_OFF.get(tables, ((), 0))
+    hamil, eng = _engine('benzene', 'float32', True, env=env)
+    _, tables_on = _engine('benzene', 'float32', True)
     N, J = hamil.n_up + hamil.n_down, len(hamil.pot.nuc_with_nl_pot)
     vper = 12 * J * N
     r, R = _walkers(hamil, 2, 4, 0.7, 'float32')
     tw = _twists(2, J, N, 5, r)
-    E0, V0, n_def = _eloc(eng, r, R, tw)
+
+    def launches(e, **kw):
+        n0 = e.launch_count
+        out = _eloc(e, r, R, tw, **kw)
+        return out, e.launch_count - n0
+
+    (E0, V0, n_def), n_launch = launches(eng)
+    assert n_launch == launches(tables_on)[1] - per_group  # one ECP group (both walkers)
     per_walker = 12 * _active(hamil, np.float32, r, R).sum((1, 2))
     assert n_def == int(per_walker.sum()) and (per_walker < vper).all()
     prefix = eng.workspace_bytes(1, MODE_LOCAL_ENERGY) - eng.workspace_bytes(vper, MODE_FORWARD)
@@ -208,7 +222,8 @@ def test_cutoff_quadrature_chunking_bitwise(monkeypatch, tables):
         assert chunk % 12
         wsb = prefix + eng.workspace_bytes(chunk, MODE_FORWARD)
         assert eng.debug_plan(2, MODE_LOCAL_ENERGY, wsb)[1] == wsb
-        E1, V1, n1 = _eloc(eng, r, R, tw, max_ws_bytes=wsb)
+        (E1, V1, n1), n_launch = launches(eng, max_ws_bytes=wsb)
+        assert n_launch == launches(tables_on, max_ws_bytes=wsb)[1] - 2 * per_group  # two ECP groups (one walker each)
         assert n1 == n_def
         assert torch.isfinite(E1).all()
         assert torch.equal(V1, V0), (chunk, V1, V0)

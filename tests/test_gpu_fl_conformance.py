@@ -315,11 +315,10 @@ def test_fl_mlp_input_ranges_match_fp64(N, inp):
     _mlp_case(N, 'partial', inp)
 
 
-def test_fl_mlp_without_fused_tanh_matches_fp64(monkeypatch):
-    """N = 4 with DQMC_NO_FUSE_TANH=1 (read at every dense layer): row GEMMs + tanh_fl_kernel where the fused epilogue
-    would otherwise run."""
-    monkeypatch.setenv('DQMC_NO_FUSE_TANH', '1')
-    _mlp_case(4, 'partial', expect='gemm_tanh_fl_kernel')
+def test_fl_mlp_engine_created_without_fused_tanh_matches_fp64():
+    """N = 4 on an engine created with DQMC_NO_FUSE_TANH=1: row GEMMs + tanh_fl_kernel where the fused epilogue would
+    otherwise run."""
+    _mlp_case(4, 'partial', env=(('DQMC_NO_FUSE_TANH', 1),), expect='gemm_tanh_fl_kernel')
 
 
 @pytest.mark.parametrize('N', [4, 8])

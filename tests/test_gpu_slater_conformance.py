@@ -88,7 +88,6 @@ def _engine(N, dtype='float32', kind='psiformer', n_down=None, env=(), conf_w=No
             eng = a.engine_for(hamil, params)
         finally:
             mp.undo()
-        eng.test_switches = tuple(env)
         _ENGINES[key] = eng
     return _ENGINES[key]
 
@@ -170,17 +169,9 @@ def _run(eng, r, BF, S):
     """Two runs of the hook: bitwise equal, and the caller's rows untouched."""
     r, BF = r.to(DEV), BF.to(DEV)
     keep = BF.clone()
-    mp = pytest.MonkeyPatch()  # DQMC_SLATER_GENERIC is also read at every call
-    for k in SWITCHES:
-        mp.delenv(k, raising=False)
-    for k, v in eng.test_switches:
-        mp.setenv(k, str(v))
-    try:
-        out = eng.debug_slater(r, BF, S)
-        out2 = eng.debug_slater(r, BF, S)
-        torch.cuda.synchronize()
-    finally:
-        mp.undo()
+    out = eng.debug_slater(r, BF, S)
+    out2 = eng.debug_slater(r, BF, S)
+    torch.cuda.synchronize()
     bits = torch.int64 if BF.dtype == torch.float64 else torch.int32
     assert torch.equal(BF.view(bits), keep.view(bits))
     for a, b in zip(out[:4], out2[:4]):

@@ -51,10 +51,10 @@ def _molecule(n_elec, n_nuc=None):
 _ENGINES = {}
 
 
-def _engine(mol, kind='psiformer', ecp=None, nsms=None, **hyper):
+def _engine(mol, kind='psiformer', ecp=None, nsms=None, env=(), **hyper):
     """fp32 engine with the tensor-core backend (one per configuration, cached); nsms: DQMC_NSMS at creation (SM count the
-    persistent kernels size their grids by)."""
-    key = (mol if isinstance(mol, str) else (tuple(mol.charges), tuple(mol.coords.ravel())), kind, ecp, nsms,
+    persistent kernels size their grids by); env: further switches set around its creation."""
+    key = (mol if isinstance(mol, str) else (tuple(mol.charges), tuple(mol.coords.ravel())), kind, ecp, nsms, tuple(env),
            tuple(sorted(hyper.items())))
     if key not in _ENGINES:
         m = Molecule.from_name(mol) if isinstance(mol, str) else mol
@@ -62,6 +62,8 @@ def _engine(mol, kind='psiformer', ecp=None, nsms=None, **hyper):
         mp = pytest.MonkeyPatch()
         if nsms:
             mp.setenv('DQMC_NSMS', str(nsms))
+        for k, v in env:
+            mp.setenv(k, str(v))
         try:
             a = B200Ansatz(hamil, kind, dtype='float32', gemm_backend=1, **hyper)
             params = PN.perturb_params(a.init(0))
@@ -328,24 +330,30 @@ def test_wf_forward_walker_isolation_bitwise(mol):
 # ---- 4. ECP gather path and chunking --------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize('emb_table', [True, False])
-def test_ecp_quadrature_chunking_bitwise(monkeypatch, emb_table):
+def test_ecp_quadrature_chunking_bitwise(emb_table):
     """Benzene ccECP, 2 walkers, fixed quadrature twists: V_nl and E_loc with the default workspace (both walkers' virtual
     walkers in one plain-forward chunk) and with workspaces that cut each walker's quadrature group into chunks whose
     boundaries (virtual-walker indices) are multiples of neither 12 nor the group size -- the gathering tile load of the
     whole-trunk kernel (moved electron ((v0 + w) / 12) % N, base walker (v0 + w) / group) and the envelope table see every
-    chunk offset.  Without the embedding table (DQMC_ECP_EMB_TABLE_OFF=1, envelope table on) as well."""
-    if not emb_table:
-        monkeypatch.setenv('DQMC_ECP_EMB_TABLE_OFF', '1')
-    hamil, _, _, eng = _engine('benzene', ecp='ccECP')
+    chunk offset.  Without the embedding table (an engine created under DQMC_ECP_EMB_TABLE_OFF=1, envelope table on) as
+    well: for the same walkers and workspace it launches one embed_fwd_kernel per ECP group fewer than the default engine."""
+    hamil, _, _, eng = _engine('benzene', ecp='ccECP', env=() if emb_table else (('DQMC_ECP_EMB_TABLE_OFF', 1),))
+    table_on = None if emb_table else _engine('benzene', ecp='ccECP')[3]
     N = hamil.n_up + hamil.n_down
     J = len(hamil.pot.nuc_with_nl_pot)
     vper = 12 * J * N  # virtual walkers (quadrature forwards) per walker
     r, R = _walkers(hamil, 2, 4)
     g = torch.Generator(device='cpu').manual_seed(5)
     tw = (torch.rand(2, J, N, generator=g, dtype=torch.float64) * math.pi / 5).to(DEV).float()
-    n0 = eng.launch_count
-    E0, st0, _, _, _ = eng.local_energy(r, R, ecp_twist=tw)
-    n_default = eng.launch_count - n0
+
+    def run(e, **kw):
+        n0 = e.launch_count
+        E, st, _, _, _ = e.local_energy(r, R, ecp_twist=tw, **kw)
+        return E, st, e.launch_count - n0
+
+    E0, st0, n_default = run(eng)
+    if table_on is not None:
+        assert n_default == run(table_on)[2] - 1  # one ECP group (both walkers)
     # workspace of the ECP pass with one walker per group: its fixed part + a plain-forward chunk of `chunk` virtual walkers
     prefix = eng.workspace_bytes(1, MODE_LOCAL_ENERGY) - eng.workspace_bytes(vper, MODE_FORWARD)
     for chunk in (1001, vper - 1, 517):
@@ -356,10 +364,11 @@ def test_ecp_quadrature_chunking_bitwise(monkeypatch, emb_table):
         # and one more virtual walker would not fit
         assert eng.debug_plan(2, MODE_LOCAL_ENERGY, wsb)[1] == wsb
         assert prefix + eng.workspace_bytes(chunk + 1, MODE_FORWARD) > wsb
-        n0 = eng.launch_count
-        E1, st1, _, _, _ = eng.local_energy(r, R, ecp_twist=tw, max_ws_bytes=wsb)
+        E1, st1, n1 = run(eng, max_ws_bytes=wsb)
         torch.cuda.synchronize()
-        assert eng.launch_count - n0 > n_default  # the quadrature forwards did run in several chunks
+        assert n1 > n_default  # the quadrature forwards did run in several chunks
+        if table_on is not None:
+            assert n1 == run(table_on, max_ws_bytes=wsb)[2] - 2  # two ECP groups (one walker each)
         assert torch.isfinite(E1).all()
         assert torch.equal(st1[3], st0[3]), (chunk, st1[3], st0[3])
         assert torch.equal(E1, E0), (chunk, E1, E0)

@@ -153,7 +153,7 @@ def test_plain_forward_half_operands_vs_3xtf32(monkeypatch):
     s64, l64 = e64.wf_forward(r, R)
     assert torch.equal(s1, s0) and torch.equal(s1.double(), s64)
     # log|psi| of a walker close to a node of psi is ill-conditioned in ANY fp32 arithmetic (the CUDA-core fp32 engine shows
-    # outliers of 1e-2 on such walkers, tools/acc_study.py), so the paths are compared through the error distribution over
+    # outliers of 1e-2 on such walkers), so the paths are compared through the error distribution over
     # the walkers, not through its maximum: median / 90 % quantile against the fp64 engine.
     a32 = B200Ansatz(hamil, 'psiformer', dtype='float32', gemm_backend=0)
     e32 = a32.engine_for(hamil, params)
@@ -196,7 +196,7 @@ def test_fused_trunk_matches_fp64(mol, walkers):
     assert torch.isfinite(out).all()
     # fp32 class.  On the hardware the f16 tensor-core pipe sums the 16 products of an instruction with less than fp32 carry
     # precision, so the result is a few ulp (measured: ~7x the plain-fp32 restatement in rms) off instead of the fraction of an
-    # ulp an exact-product model gives; log|psi| and E_loc are not affected at their fp32 noise level (tools/acc_study.py).
+    # ulp an exact-product model gives; log|psi| and E_loc are not affected at their fp32 noise level.
     assert rms < 12 * rms32 + 1e-6 and err < 25 * err32 + 1e-5, (err, err32, rms, rms32)
 
 
