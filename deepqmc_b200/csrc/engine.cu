@@ -168,6 +168,10 @@ struct EngineBase {
                          void* grad_params, void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int spin(const void* r, const void* R, int Rb, int B, const void* sign, const void* logp, int down_idx, void* s2,
                    void* ratio, void* ws, int64_t wsb, cudaStream_t st) = 0;
+  virtual int grad_positions(const void* r, const void* R, int Rb, int B, void* sign, void* logp, void* grad_r, void* grad_R,
+                             void* ws, int64_t wsb, cudaStream_t st) = 0;
+  virtual int force_terms(const void* r, const void* R, int Rb, int B, const void* grad_r, void* bare, void* zvq, void* Q,
+                          cudaStream_t st) = 0;
   virtual int orbitals(const void* r, const void* R, int Rb, int B, void* out, void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int set_ph(int n_tab, int n_grid, double r_max, const double* tables, const int32_t* tab_of_nuc) = 0;
   virtual int debug_gemm(const char* wname, const char* bname, const void* A, const void* Res, void* C, int Mr, int S,
@@ -934,17 +938,22 @@ struct Engine : EngineBase {
     return prefixed_bytes(prefix, Bc, langevin ? T3 + 2 : 1);
   }
   // bytes one reverse-pass chunk of Bc walkers carves: a dry pass of the chunk function itself
-  int64_t vjp_chunk_bytes(int Bc) {
+  // (pos: the position mode of dqmc_wf_grad_positions, Psiformer kinds and FermiNet)
+  int64_t vjp_chunk_bytes(int Bc, bool pos = false) {
     DryPass dp(this);
     const Arena a(this, plan_base());
+    const PosOut none{nullptr, nullptr};
+    const PosOut* po = pos ? &none : nullptr;
     if (gnn) vjp_chunk_paulinet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr);
-    else if (cfg.kind == DQMC_FERMINET) vjp_chunk_ferminet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr);
-    else vjp_chunk(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr);
+    else if (cfg.kind == DQMC_FERMINET) vjp_chunk_ferminet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr, po);
+    else vjp_chunk(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr, po);
     return dp.bytes();
   }
+  bool has_pos_pass() const { return !gnn && !cfg.backflow_add; }
   int64_t ws_bytes(int B, int mode) override {
     if (B < 1) B = 1;
     if (mode == DQMC_MODE_VJP) return vjp_chunk_bytes(B);
+    if (mode == DQMC_MODE_GRAD_POS) return has_pos_pass() ? vjp_chunk_bytes(B, true) : 0;
     if (mode == DQMC_MODE_MCMC) return sweep_bytes(B, false, B);
     if (mode == DQMC_MODE_LANGEVIN) return sweep_bytes(B, true, B);
     if (mode == DQMC_MODE_SPIN) {  // sized for the exact estimator, the larger of the two; no down electrons: no forwards
@@ -967,6 +976,7 @@ struct Engine : EngineBase {
     const int S = T3 + 2;
     switch (mode) {
       case DQMC_MODE_VJP: return vjp_chunk_bytes(1);
+      case DQMC_MODE_GRAD_POS: return has_pos_pass() ? vjp_chunk_bytes(1, true) : 0;
       case DQMC_MODE_MCMC: return sweep_bytes(B, false, 1);
       case DQMC_MODE_LANGEVIN: return sweep_bytes(B, true, 1);
       case DQMC_MODE_LOCAL_ENERGY: return std::max<int64_t>(chunk_bytes(1, S), J > 0 ? ecp_bytes(1, 1) : 0);
@@ -1001,6 +1011,9 @@ struct Engine : EngineBase {
                       nullptr, ws, wsb, nullptr);
         break;
       case DQMC_MODE_SPIN: rc = spin(nullptr, nullptr, 0, B, nullptr, nullptr, -1, nullptr, nullptr, ws, wsb, nullptr); break;
+      case DQMC_MODE_GRAD_POS:
+        rc = grad_positions(nullptr, nullptr, 0, B, nullptr, nullptr, nullptr, nullptr, ws, wsb, nullptr);
+        break;
       default: err = "unknown mode"; rc = 2;
     }
     if (carved) *carved = dp.bytes();
@@ -1878,8 +1891,28 @@ struct Engine : EngineBase {
               hi > lo ? N : 0, lo, hi);
   }
 
-  int vjp_chunk(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a, cudaStream_t st) {
+  // Position mode of the reverse passes (dqmc_wf_grad_positions): cotangent 1 per walker, no parameter gradients, the chain
+  // carried on into the electron-nucleus features, the envelopes and the cusps.  gr [Bc][N][3] / gR [Bc][M][3] nullable.
+  struct PosOut { T* gr; T* gR; };
+  // pair-cotangent buffers of the position mode: per-(walker, determinant) envelope shares and their per-walker sum
+  struct PosBufs { T *cpart = nullptr, *cbuf = nullptr; };
+  PosBufs carve_pos(Arena& a, int Bc) const {
+    PosBufs p;
+    p.cpart = a.take<T>((size_t)Bc * K * N * M * 3);
+    p.cbuf = a.take<T>((size_t)Bc * N * M * 3);
+    return p;
+  }
+  void launch_pos_reduce(const T* r, const T* R, int Rb, int Bc, const PosBufs& pb, const T* dFeat, int ldf, int log_rescale,
+                         const T* dE, const PosOut* po, cudaStream_t st) {
+    DQ_LAUNCH(pos_grad_reduce_kernel<T>, dim3(Bc), dim3(128), 0, st, r, R, Rb, N, M, cfg.n_up, K, (const T*)pb.cpart, dFeat, ldf,
+              log_rescale, dE, cfg.cusp_kind, (T)cfg.cusp_same_scale, (T)cfg.cusp_anti_scale, P("cusp.alpha"), cfg.nuc_cusp_kind,
+              cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr, pb.cbuf, po->gr, po->gR);
+  }
+
+  int vjp_chunk(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a, cudaStream_t st,
+                const PosOut* po = nullptr) {
     const int L = cfg.n_layers, rows = Bc * N, F = 4 * M + 1;
+    auto gp = [&](const std::string& n) { return po ? (T*)nullptr : G + off(n); };  // parameter cotangent (none in position mode)
     std::vector<T*> X(L + 1), QKV(L), O(L), A(L), M1(L);
     for (int l = 0; l <= L; ++l) X[l] = a.take<T>((size_t)rows * d);
     for (int l = 0; l < L; ++l) { QKV[l] = a.take<T>((size_t)rows * 3 * d); O[l] = a.take<T>((size_t)rows * d); A[l] = a.take<T>((size_t)rows * d); M1[l] = a.take<T>((size_t)rows * d); }
@@ -1888,6 +1921,7 @@ struct Engine : EngineBase {
     T* dXn = a.take<T>((size_t)rows * d); T* dZ = a.take<T>((size_t)rows * d); T* dM1 = a.take<T>((size_t)rows * d);
     T* dA = a.take<T>((size_t)rows * d); T* dO = a.take<T>((size_t)rows * d); T* dQKV = a.take<T>((size_t)rows * 3 * d);
     T* dX = a.take<T>((size_t)rows * d); T* Feat = a.take<T>((size_t)rows * F);
+    const PosBufs pb = po ? carve_pos(a, Bc) : PosBufs();
     if (a.left() < 0) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
     const T scale = (T)(1.0 / std::sqrt((double)dh));
     // ---- forward with every layer's activations kept --------------------------------------------------------
@@ -1922,45 +1956,56 @@ struct Engine : EngineBase {
     // ---- reverse ------------------------------------------------------------------------------------------------
     DQ_LAUNCH(finalize_bwd_kernel<T>, dim3((Bc + 127) / 128), dim3(128), 0, st, r, N, cfg.n_up, K, Bc, (const T*)dsign,
               (const T*)dlog, wts, cfg.cusp_kind, (T)cfg.cusp_same_scale, (T)cfg.cusp_anti_scale, P("cusp.alpha"), dld,
-              G + off("cusp.alpha"), R, Rb, M, cfg.nuc_cusp_kind, cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr,
-              cfg.nuc_cusp_kind ? G + off("cusp.nuc") : (T*)nullptr, (const T*)nullptr, (T*)nullptr);
+              gp("cusp.alpha"), R, Rb, M, cfg.nuc_cusp_kind, cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr,
+              cfg.nuc_cusp_kind ? gp("cusp.nuc") : (T*)nullptr, (const T*)nullptr, (T*)nullptr);
     {
       const size_t pw = slater_bwd_smem_per_warp<T>(N);
       int wpb = (int)((96 * 1024) / pw);
       wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
       DQ_LAUNCH(slater_bwd_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), pw * wpb, st, r, R, Rb, N, M, cfg.n_up, K,
                 Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, (const T*)dld, dBF,
-                G + off("env.pi_up"), G + off("env.pi_dn"), G + off("env.zeta_up"), G + off("env.zeta_dn"), env_rep, 1);
+                gp("env.pi_up"), gp("env.pi_dn"), gp("env.zeta_up"), gp("env.zeta_dn"), env_rep, 1, pb.cpart);
     }
     // backflow heads: dX_L = dBF W_spin^T, dW_spin += X_L[spin rows]^T dBF[spin rows]
     gemm_raw(dBF, KN, PT("bf.up"), PT("bf.dn"), cfg.n_up, d, nullptr, 0, dXn, d, Bc, d, KN, 1, st);
-    wgrad(X[L], d, dBF, KN, rows, d, KN, G + off("bf.up"), 0, cfg.n_up, st);
-    wgrad(X[L], d, dBF, KN, rows, d, KN, G + off("bf.dn"), cfg.n_up, N, st);
+    if (!po) {
+      wgrad(X[L], d, dBF, KN, rows, d, KN, G + off("bf.up"), 0, cfg.n_up, st);
+      wgrad(X[L], d, dBF, KN, rows, d, KN, G + off("bf.dn"), cfg.n_up, N, st);
+    }
     const size_t nel = (size_t)rows * d;
     for (int l = L - 1; l >= 0; --l) {
       const std::string q = "L" + std::to_string(l) + ".";
       // X_{l+1} = A + tanh(M1 W2 + b2)
       DQ_LAUNCH(tanh_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dXn, (const T*)X[l + 1],
                 (const T*)A[l], dZ, nel);
-      bgrad(dZ, d, rows, d, G + off(q + "b2"), st);
-      wgrad(M1[l], d, dZ, d, rows, d, d, G + off(q + "w2"), 0, 0, st);
+      if (!po) {
+        bgrad(dZ, d, rows, d, G + off(q + "b2"), st);
+        wgrad(M1[l], d, dZ, d, rows, d, d, G + off(q + "w2"), 0, 0, st);
+      }
       gemm_raw(dZ, d, PT(q + "w2"), nullptr, 0, d, nullptr, 0, dM1, d, rows, d, d, 0, st);
       // M1 = tanh(A W1 + b1)
       DQ_LAUNCH(tanh_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dM1, (const T*)M1[l],
                 (const T*)nullptr, dZ, nel);
-      bgrad(dZ, d, rows, d, G + off(q + "b1"), st);
-      wgrad(A[l], d, dZ, d, rows, d, d, G + off(q + "w1"), 0, 0, st);
+      if (!po) {
+        bgrad(dZ, d, rows, d, G + off(q + "b1"), st);
+        wgrad(A[l], d, dZ, d, rows, d, d, G + off(q + "w1"), 0, 0, st);
+      }
       gemm_raw(dZ, d, PT(q + "w1"), nullptr, 0, d, dXn, d, dA, d, rows, d, d, 0, st);  // dA = dX_{l+1} + dZ1 W1^T
       // A = X + O Wo
-      wgrad(O[l], d, dA, d, rows, d, d, G + off(q + "wo"), 0, 0, st);
+      if (!po) wgrad(O[l], d, dA, d, rows, d, d, G + off(q + "wo"), 0, 0, st);
       gemm_raw(dA, d, PT(q + "wo"), nullptr, 0, d, nullptr, 0, dO, d, rows, d, d, 0, st);
       DQ_LAUNCH(attn_bwd_kernel<T>, dim3(Bc, H), dim3(128), attn_bwd_smem_bytes<T>(N, dh, Mn), st, (const T*)QKV[l], 3 * d,
                 (const T*)dO, d, N, dh, d, scale, dQKV, Mn > 0 ? P(q + "kn") : (const T*)nullptr,
-                Mn > 0 ? P(q + "vn") : (const T*)nullptr, Mn, Mn > 0 ? G + off(q + "kn") : (T*)nullptr,
-                Mn > 0 ? G + off(q + "vn") : (T*)nullptr);
-      wgrad(X[l], d, dQKV, 3 * d, rows, d, 3 * d, G + off(q + "wqkv"), 0, 0, st);
+                Mn > 0 ? P(q + "vn") : (const T*)nullptr, Mn, Mn > 0 ? gp(q + "kn") : (T*)nullptr,
+                Mn > 0 ? gp(q + "vn") : (T*)nullptr);
+      if (!po) wgrad(X[l], d, dQKV, 3 * d, rows, d, 3 * d, G + off(q + "wqkv"), 0, 0, st);
       gemm_raw(dQKV, 3 * d, PT(q + "wqkv"), nullptr, 0, d, dA, d, dX, d, rows, d, 3 * d, 0, st);  // dX_l = dA + dQKV Wqkv^T
       T* t = dXn; dXn = dX; dX = t;
+    }
+    if (po) {  // dFeat = dX0 W_emb^T (the spin column is not read), then features, envelopes and cusps per walker
+      gemm_raw(dXn, d, PT("emb.w"), nullptr, 0, F, nullptr, 0, Feat, F, rows, F, d, 0, st);
+      launch_pos_reduce(r, R, Rb, Bc, pb, Feat, F, 1, (const T*)nullptr, po, st);
+      return 0;
     }
     DQ_LAUNCH(embed_feat_kernel<T>, dim3((rows * M + 127) / 128), dim3(128), 0, st, r, R, Rb, N, M, cfg.n_up, Feat, rows);
     wgrad(Feat, F, dXn, d, rows, F, d, G + off("emb.w"), 0, 0, st);
@@ -1969,9 +2014,10 @@ struct Engine : EngineBase {
 
   // FermiNet reverse pass (conf/ansatz/ferminet.yaml): node update g on concat[h, spin means of h, spin means of the
   // incoming edges], shared edge MLP u, residuals / sqrt(2).  The raw input features carry no parameters, so the
-  // chain stops at the first layer's weights.
+  // parameter chain stops at the first layer's weights; the position mode carries it on to the raw node and edge features.
   int vjp_chunk_ferminet(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a,
-                         cudaStream_t st) {
+                         cudaStream_t st, const PosOut* po = nullptr) {
+    auto gp = [&](const std::string& n) { return po ? (T*)nullptr : G + off(n); };
     const int L = cfg.n_layers, rows = Bc * N, rowsE = Bc * N * N, de = cfg.edge_dim, d0 = 4 * M;
     const T isq2 = (T)0.70710678118654752440;
     std::vector<T*> Hs(L + 1), Es(L), Fs(L);
@@ -1984,9 +2030,11 @@ struct Engine : EngineBase {
     const int fmax = 3 * (d > d0 ? d : d0) + 2 * (de > 4 ? de : 4);
     T* BF = a.take<T>((size_t)rows * KN); T* dBF = a.take<T>((size_t)rows * KN);
     T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
-    T* dXa = a.take<T>((size_t)rows * d); T* dXb = a.take<T>((size_t)rows * d); T* dZ = a.take<T>((size_t)rows * d);
+    const int dx = po ? std::max(d, d0) : d, dex = po ? std::max(de, 4) : de;  // the position mode reaches layer 0's inputs
+    T* dXa = a.take<T>((size_t)rows * dx); T* dXb = a.take<T>((size_t)rows * dx); T* dZ = a.take<T>((size_t)rows * d);
     T* dF = a.take<T>((size_t)rows * fmax);
-    T* dEa = a.take<T>((size_t)rowsE * de); T* dEb = a.take<T>((size_t)rowsE * de); T* dZe = a.take<T>((size_t)rowsE * de);
+    T* dEa = a.take<T>((size_t)rowsE * dex); T* dEb = a.take<T>((size_t)rowsE * dex); T* dZe = a.take<T>((size_t)rowsE * de);
+    const PosBufs pb = po ? carve_pos(a, Bc) : PosBufs();
     if (a.left() < 0) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
     // ---- forward, activations kept -----------------------------------------------------------------------------
     DQ_LAUNCH(embed_kernel<T>, dim3(Bc * N), dim3(128), sizeof(T) * 5 * d0, st, r, R, Rb, N, M, cfg.n_up, 1, 0, 0,
@@ -2023,23 +2071,25 @@ struct Engine : EngineBase {
     // ---- reverse -------------------------------------------------------------------------------------------------
     DQ_LAUNCH(finalize_bwd_kernel<T>, dim3((Bc + 127) / 128), dim3(128), 0, st, r, N, cfg.n_up, K, Bc, (const T*)dsign,
               (const T*)dlog, wts, cfg.cusp_kind, (T)cfg.cusp_same_scale, (T)cfg.cusp_anti_scale, P("cusp.alpha"), dld,
-              G + off("cusp.alpha"), R, Rb, M, cfg.nuc_cusp_kind, cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr,
-              cfg.nuc_cusp_kind ? G + off("cusp.nuc") : (T*)nullptr, (const T*)nullptr, (T*)nullptr);
+              gp("cusp.alpha"), R, Rb, M, cfg.nuc_cusp_kind, cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr,
+              cfg.nuc_cusp_kind ? gp("cusp.nuc") : (T*)nullptr, (const T*)nullptr, (T*)nullptr);
     {
       const size_t pw = slater_bwd_smem_per_warp<T>(N);
       int wpb = (int)((96 * 1024) / pw);
       wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
       DQ_LAUNCH(slater_bwd_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), pw * wpb, st, r, R, Rb, N, M, cfg.n_up, K,
                 Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, (const T*)dld, dBF,
-                G + off("env.pi_up"), G + off("env.pi_dn"), G + off("env.zeta_up"), G + off("env.zeta_dn"), env_rep, 1);
+                gp("env.pi_up"), gp("env.pi_dn"), gp("env.zeta_up"), gp("env.zeta_dn"), env_rep, 1, pb.cpart);
     }
     T* dHn = dXa;   // gradient w.r.t. H_{l+1}
     T* dHc = dXb;   // gradient w.r.t. H_l (being built)
     T* dEn = dEa;   // gradient w.r.t. E_{l+1} (valid for l < L - 1)
     T* dEc = dEb;
     gemm_raw(dBF, KN, PT("bf.up"), PT("bf.dn"), cfg.n_up, d, nullptr, 0, dHn, d, Bc, d, KN, 1, st);
-    wgrad(Hs[L], d, dBF, KN, rows, d, KN, G + off("bf.up"), 0, cfg.n_up, st);
-    wgrad(Hs[L], d, dBF, KN, rows, d, KN, G + off("bf.dn"), cfg.n_up, N, st);
+    if (!po) {
+      wgrad(Hs[L], d, dBF, KN, rows, d, KN, G + off("bf.up"), 0, cfg.n_up, st);
+      wgrad(Hs[L], d, dBF, KN, rows, d, KN, G + off("bf.dn"), cfg.n_up, N, st);
+    }
     for (int l = L - 1; l >= 0; --l) {
       const std::string q = "F" + std::to_string(l) + ".";
       const int dc = dH[l], ec = dEd[l], fin = 3 * dc + 2 * ec;
@@ -2048,9 +2098,11 @@ struct Engine : EngineBase {
       // H_{l+1} = s (H_l + tanh(F Wg + bg))  |  tanh(F Wg + bg)
       DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dHn, (const T*)Hs[l + 1],
                 (const T*)(res_h ? Hs[l] : nullptr), res_h ? isq2 : T(1), dZ, nel);
-      bgrad(dZ, d, rows, d, G + off(q + "bg"), st);
-      wgrad(Fs[l], fin, dZ, d, rows, fin, d, G + off(q + "wg"), 0, 0, st);
-      if (l > 0) {
+      if (!po) {
+        bgrad(dZ, d, rows, d, G + off(q + "bg"), st);
+        wgrad(Fs[l], fin, dZ, d, rows, fin, d, G + off(q + "wg"), 0, 0, st);
+      }
+      if (l > 0 || po) {
         gemm_raw(dZ, d, PT(q + "wg"), nullptr, 0, fin, nullptr, 0, dF, fin, rows, fin, d, 0, st);
         DQ_LAUNCH(fermi_agg_bwd_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)dF, dc, ec, N, cfg.n_up,
                   (const T*)(res_h ? dHn : nullptr), isq2, dHc, dEc);
@@ -2060,9 +2112,11 @@ struct Engine : EngineBase {
         const size_t nee = (size_t)rowsE * de;
         DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nee + 255) / 256)), dim3(256), 0, st, (const T*)dEn, (const T*)Es[l + 1],
                   (const T*)(res_e ? Es[l] : nullptr), res_e ? isq2 : T(1), dZe, nee);
-        bgrad(dZe, de, rowsE, de, G + off(q + "bu"), st);
-        wgrad(Es[l], ec, dZe, de, rowsE, ec, de, G + off(q + "wu"), 0, 0, st);
-        if (l > 0) {
+        if (!po) {
+          bgrad(dZe, de, rowsE, de, G + off(q + "bu"), st);
+          wgrad(Es[l], ec, dZe, de, rowsE, ec, de, G + off(q + "wu"), 0, 0, st);
+        }
+        if (l > 0 || po) {
           gemm_raw(dZe, de, PT(q + "wu"), nullptr, 0, ec, dEc, ec, dEc, ec, rowsE, ec, de, 0, st);  // dE_l += dZe Wu^T
           if (res_e) {
             const size_t ne2 = (size_t)rowsE * ec;
@@ -2073,6 +2127,7 @@ struct Engine : EngineBase {
       T* t1 = dHn; dHn = dHc; dHc = t1;
       T* t2 = dEn; dEn = dEc; dEc = t2;
     }
+    if (po) launch_pos_reduce(r, R, Rb, Bc, pb, dHn, d0, 0, dEn, po, st);  // dH_0 [rows][4 M], dE_0 [rows N][4]
     return 0;
   }
   // ---- conv-GNN reverse pass: the reference's test ansatz (tests/conf/ansatz.yaml: hk.Embed embeddings, 'featurewise'
@@ -2260,7 +2315,8 @@ struct Engine : EngineBase {
       wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
       DQ_LAUNCH(slater_bwd_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), pw * wpb, st, r, R, Rb, N, M, cfg.n_up, K,
                 Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, (const T*)dld, dBF,
-                G + off("env.pi_up"), G + off("env.pi_dn"), G + off("env.zeta_up"), G + off("env.zeta_dn"), env_rep, full_det);
+                G + off("env.pi_up"), G + off("env.pi_dn"), G + off("env.zeta_up"), G + off("env.zeta_dn"), env_rep, full_det,
+                (T*)nullptr);
     }
     // scratch for the reverse sweep
     const int xm = std::max(d, xd[0]);
@@ -2412,6 +2468,62 @@ struct Engine : EngineBase {
       if (rc) return rc;
       if (dry) break;  // planning pass: the first chunk is the largest
     }
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
+  // d log|psi| / d r and / d R per walker: the parameter reverse pass in its position mode, chunked like vjp_params
+  int grad_positions(const void* r_, const void* R_, int Rb, int B, void* sign, void* logp, void* grad_r, void* grad_R, void* ws,
+                     int64_t wsb, cudaStream_t st) override {
+    if (gnn) { err = "dqmc_wf_grad_positions: the conv-GNN kinds have no position reverse pass"; return 2; }
+    if (cfg.backflow_add) { err = "dqmc_wf_grad_positions: additive backflow branch has no reverse pass"; return 2; }
+    if (cfg.kind == DQMC_TRANSPSIFORMER && grad_R) {
+      err = "dqmc_wf_grad_positions: the TransPsiformer's nuclear tokens and envelope exponents depend on R through the host-side "
+            "nuclear stream; only grad_r is available (out_grad_R must be null)";
+      return 2;
+    }
+    if (B == 0) return 0;
+    const T* r = (const T*)r_;
+    const T* R = (const T*)R_;
+    const bool fermi = cfg.kind == DQMC_FERMINET;
+    int64_t Bc = largest_fit(B, wsb, [&](int64_t n) { return vjp_chunk_bytes((int)n, true); });
+    if (Bc < 1) { err = "workspace too small for a single walker (grad_positions)"; return 3; }
+    if (!fermi) DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
+    {  // the warps-per-block rule of the launch sites
+      const size_t pw = slater_bwd_smem_per_warp<T>(N);
+      int wpb = (int)((96 * 1024) / pw);
+      wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
+      if (pw * wpb > 227 * 1024) { err = "system too large for the shared-memory tiling of the reverse pass (N)"; return 2; }
+      DQ_CHECK(raise_dyn_smem(slater_bwd_kernel<T>, (int)(pw * wpb)));
+    }
+    for (int b0 = 0; b0 < B; b0 += (int)Bc) {
+      const int nb = (int)std::min<int64_t>(Bc, B - b0);
+      const T* rc_ = r + (size_t)b0 * 3 * N;
+      const T* Rc_ = R + (Rb ? (size_t)b0 * 3 * M : 0);
+      const PosOut po{grad_r ? (T*)grad_r + (size_t)b0 * 3 * N : nullptr, grad_R ? (T*)grad_R + (size_t)b0 * 3 * M : nullptr};
+      const Arena a(this, ws, wsb);
+      int rc = fermi ? vjp_chunk_ferminet(rc_, Rc_, Rb, nb, nullptr, (T*)sign + b0, (T*)logp + b0, nullptr, a, st, &po)
+                     : vjp_chunk(rc_, Rc_, Rb, nb, nullptr, (T*)sign + b0, (T*)logp + b0, nullptr, a, st, &po);
+      if (rc) return rc;
+      rc = check_guards();
+      if (rc) return rc;
+      if (dry) break;  // planning pass: the first chunk is the largest
+    }
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
+  // closed-form force terms per walker (force_terms_kernel); all-electron Hamiltonians only
+  int force_terms(const void* r, const void* R, int Rb, int B, const void* grad_r, void* bare, void* zvq, void* Q,
+                  cudaStream_t st) override {
+    if (J > 0 || cfg.ecp_loc_terms > 0 || d_ph_tabs) {
+      err = "dqmc_force_terms: effective core potentials and pseudo-Hamiltonians are not supported (all-electron only)";
+      return 2;
+    }
+    if (zvq && !grad_r) { err = "dqmc_force_terms: out_zvq needs grad_r"; return 2; }
+    if (B == 0) return 0;
+    DQ_LAUNCH(force_terms_kernel<T>, dim3(B), dim3(32), 0, st, (const T*)r, (const T*)R, Rb, N, M, (const T*)d_zval,
+              (const T*)grad_r, (T*)bare, (T*)zvq, (T*)Q);
     DQ_CHECK(cudaGetLastError());
     return 0;
   }
@@ -2778,6 +2890,24 @@ int dqmc_spin(dqmc_handle h, const void* r, const void* R, int32_t R_batched, in
   if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
   return h->e->spin(r, R, R_batched, n_walkers, sign, log, down_idx, out_s2, out_ratio, workspace, workspace_bytes,
                     (cudaStream_t)stream);
+}
+int dqmc_wf_grad_positions(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, void* out_sign,
+                           void* out_log, void* out_grad_r, void* out_grad_R, void* workspace, int64_t workspace_bytes,
+                           void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
+  if (n_walkers > 0 && (!r || !R || !out_sign || !out_log)) { h->e->err = "dqmc_wf_grad_positions: null array"; return 2; }
+  return h->e->grad_positions(r, R, R_batched, n_walkers, out_sign, out_log, out_grad_r, out_grad_R, workspace, workspace_bytes,
+                              (cudaStream_t)stream);
+}
+int dqmc_force_terms(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, const void* grad_r,
+                     void* out_bare, void* out_zvq, void* out_Q, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
+  if (n_walkers > 0 && (!r || !R)) { h->e->err = "dqmc_force_terms: null array"; return 2; }
+  return h->e->force_terms(r, R, R_batched, n_walkers, grad_r, out_bare, out_zvq, out_Q, (cudaStream_t)stream);
 }
 int dqmc_set_pseudo_hamiltonian(dqmc_handle h, int32_t n_tab, int32_t n_grid, double r_max, const double* tables,
                                 const int32_t* tab_of_nuc) {

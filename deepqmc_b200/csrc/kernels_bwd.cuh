@@ -196,7 +196,7 @@ __global__ void attn_bwd_kernel(const T* __restrict__ QKV, int ldq, const T* __r
     T* dst = dQKV + (row0 + i) * ldq + h * dh + e;
     dst[0] = dq; dst[dmodel] = dk; dst[2 * dmodel] = dv;
   }
-  for (int idx = tid; idx < Mn * dh; idx += nt) {
+  for (int idx = tid; dKn && idx < Mn * dh; idx += nt) {  // dKn / dVn null: parameter cotangents not wanted
     const int m = idx / dh, e = idx - m * dh;
     T dk = T(0), dv = T(0);
     for (int j = 0; j < N; ++j) {
@@ -229,7 +229,7 @@ __global__ void finalize_bwd_kernel(const T* __restrict__ r, int N, int n_up, in
                                     T* __restrict__ dconf_w) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  const T w = weights[b];
+  const T w = weights ? weights[b] : T(1);  // null: per-walker cotangent 1 (position gradients)
   const T* ds = det_sign + (size_t)b * K;
   const T* dl = det_log + (size_t)b * K;
   T shift = dl[0];
@@ -280,6 +280,10 @@ __global__ void finalize_bwd_kernel(const T* __restrict__ r, int N, int n_up, in
 // Slater backward, one warp per (walker, determinant): rebuild A = env * bf, invert it (Gauss-Jordan with partial
 // pivoting), G = dlogdet A^-T;  dBF[b][i][k N + mu] = G[i][mu] env[i][mu];  envelope parameters:
 //   dpi[o][m] += G bf e^{-|zeta| rho},  dzeta[o][m] += G bf pi e^{-|zeta| rho} (-rho sign(zeta))   (o = k N + mu).
+// dpi_up null: no envelope-parameter gradients.  cpart (nullable) [B K][N][M][3]: this determinant's share of the pair
+// cotangent d log|psi| / d d_im (d_im = r_i - R_m) through the envelopes,
+//   sum_mu G bf sum_t pi e^{-|zeta| rho} (-|zeta|) d_im / rho,
+// summed over mu in a fixed order by one lane per (i, m) (no atomics: callers reduce over k in order).
 // dynamic smem per warp: sizeof(T) * (N (2N + 1) + 2 N (N + 1)).
 // ------------------------------------------------------------------------------------------
 template <class T>
@@ -288,7 +292,7 @@ __global__ void slater_bwd_kernel(const T* __restrict__ r, const T* __restrict__
                                   const T* __restrict__ zeta_up, const T* __restrict__ zeta_dn,
                                   const T* __restrict__ BF, int ldb, const T* __restrict__ dlogdet, T* __restrict__ dBF,
                                   T* __restrict__ dpi_up, T* __restrict__ dpi_dn, T* __restrict__ dzeta_up,
-                                  T* __restrict__ dzeta_dn, int rep, int full_det) {
+                                  T* __restrict__ dzeta_dn, int rep, int full_det, T* __restrict__ cpart) {
   // full_det == 0: spin-factorised determinants = block-diagonal A (off-diagonal spin blocks zero, as in slater_kernel)
   DQMC_DYN_SMEM(smem_raw);
   const int NP = N + 1, N2 = 2 * N + 1;
@@ -361,7 +365,7 @@ __global__ void slater_bwd_kernel(const T* __restrict__ r, const T* __restrict__
     const bool blocked = !full_det && ((i < n_up) != (mu < n_up));
     const T G = blocked ? T(0) : dl * aug[mu * N2 + N + i];
     dBF[((size_t)b * N + i) * ldb + k * N + mu] = G * env[i * NP + mu];
-    if (blocked) continue;
+    if (blocked || !dpi_up) continue;
     const T gb = G * bfv[i * NP + mu];  // d / d env[i][mu]
     const bool up = i < n_up;
     const T* pi = (up ? pi_up : pi_dn) + (size_t)(k * N + mu) * M * rep;
@@ -377,6 +381,29 @@ __global__ void slater_bwd_kernel(const T* __restrict__ r, const T* __restrict__
         atomic_add(dze + m * rep + et, gb * pi[m * rep + et] * ex * (-rho) * (z > T(0) ? T(1) : (z < T(0) ? T(-1) : T(0))));
       }
     }
+  }
+  if (!cpart) return;
+  for (int idx = lane; idx < N * M; idx += 32) {
+    const int i = idx / M, m = idx - i * M;
+    const bool up = i < n_up;
+    const T dx0 = rb[3 * i] - Rb[3 * m], dx1 = rb[3 * i + 1] - Rb[3 * m + 1], dx2 = rb[3 * i + 2] - Rb[3 * m + 2];
+    const T rho = m_sqrt(Num<T>::eps() + dx0 * dx0 + dx1 * dx1 + dx2 * dx2);
+    T acc = T(0);
+    for (int mu = 0; mu < N; ++mu) {
+      if (!full_det && (up != (mu < n_up))) continue;
+      const T gb = dl * aug[mu * N2 + N + i] * bfv[i * NP + mu];
+      const T* pi = (up ? pi_up : pi_dn) + ((size_t)(k * N + mu) * M + m) * rep;
+      const T* ze = (up ? zeta_up : zeta_dn) + ((size_t)(k * N + mu) * M + m) * rep;
+      T de = T(0);  // d env[i][mu] / d rho_im
+      for (int et = 0; et < rep; ++et) {
+        const T az = m_abs(ze[et]);
+        de -= pi[et] * az * m_exp(-az * rho);
+      }
+      acc += gb * de;
+    }
+    const T s = acc / rho;
+    T* c = cpart + (((size_t)gw * N + i) * M + m) * 3;
+    c[0] = s * dx0; c[1] = s * dx1; c[2] = s * dx2;
   }
 }
 
@@ -401,6 +428,146 @@ __global__ void embed_feat_kernel(const T* __restrict__ r, const T* __restrict__
   if (m == 0) f[F - 1] = i < n_up ? T(1) : T(-1);
 }
 
+
+// ------------------------------------------------------------------------------------------
+// Position gradients of log|psi| from the reverse pass (reference: jax.grad of wf(...).log with respect to r and R,
+// force.py:96-118 make_grad_nuc_log_wf / make_grad_log_wf).  One block per walker, every sum in a fixed order.
+// Phase 1, thread per (i, m): the pair cotangent c_im = d log|psi| / d d_im (d_im = r_i - R_m) into cbuf[B][N][M][3]:
+//   envelopes  sum_k cpart[b][k][i][m]  (slater_bwd_kernel),
+//   features   dFeat[b i][4 m .. 4 m + 3] through the Jacobian of [f(rho), d s(rho)], rho = sqrt(eps + |d|^2):
+//              log_rescale 1 (Psiformer, embed_feat_kernel) f = log1p rho, s = f / rho; 0 (FermiNet) f = rho, s = 1,
+//   nuclear cusp (finalize_kernel, plain distance): -sc / (den0 + |d|).
+// Phase 2: grad_r[b][i] = sum_m c_im + the e-e cusp + the e-e edge features dE[b][j][i][4] (FermiNet: sender j,
+// receiver i, [rho, r_i - r_j]);  grad_R[b][m] = -sum_i c_im.  grad_r / grad_R nullable.
+// ------------------------------------------------------------------------------------------
+template <class T>
+__global__ void pos_grad_reduce_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M, int n_up,
+                                       int K, const T* __restrict__ cpart, const T* __restrict__ dFeat, int ldf, int log_rescale,
+                                       const T* __restrict__ dE, int cusp_kind, T same_scale, T anti_scale,
+                                       const T* __restrict__ cusp_alpha, int nuc_cusp_kind, const T* __restrict__ nuc_cusp,
+                                       T* __restrict__ cbuf, T* __restrict__ grad_r, T* __restrict__ grad_R) {
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const T* rb = r + (size_t)b * N * 3;
+  const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
+  T* cb = cbuf + (size_t)b * N * M * 3;
+  for (int idx = tid; idx < N * M; idx += nt) {
+    const int i = idx / M, m = idx - i * M;
+    const T d[3] = {rb[3 * i] - Rb[3 * m], rb[3 * i + 1] - Rb[3 * m + 1], rb[3 * i + 2] - Rb[3 * m + 2]};
+    const T d2 = d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
+    T c[3] = {T(0), T(0), T(0)};
+    for (int k = 0; k < K; ++k) {
+      const T* p = cpart + ((((size_t)b * K + k) * N + i) * M + m) * 3;
+      c[0] += p[0]; c[1] += p[1]; c[2] += p[2];
+    }
+    if (dFeat) {
+      const T rho = m_sqrt(Num<T>::eps() + d2);
+      const T* f = dFeat + ((size_t)b * N + i) * ldf + 4 * m;
+      T fp, s, sp;  // f'(rho), s(rho), s'(rho)
+      if (log_rescale) {
+        const T g = m_log1p(rho);
+        fp = T(1) / (T(1) + rho); s = g / rho; sp = fp / rho - g / (rho * rho);
+      } else {
+        fp = T(1); s = T(1); sp = T(0);
+      }
+      const T fd = f[1] * d[0] + f[2] * d[1] + f[3] * d[2];
+      const T rad = (f[0] * fp + fd * sp) / rho;
+      for (int a = 0; a < 3; ++a) c[a] += rad * d[a] + f[1 + a] * s;
+    }
+    if (nuc_cusp_kind != 0) {
+      const T dist = m_sqrt(d2), al = nuc_cusp[0];
+      const T sc = nuc_cusp[1 + m] * (nuc_cusp_kind == 1 ? al * al : T(1) / (al * al));
+      const T den = (nuc_cusp_kind == 1 ? al : T(1) / al) + dist;
+      const T cc = sc / (den * den) / dist;
+      for (int a = 0; a < 3; ++a) c[a] += cc * d[a];
+    }
+    T* o = cb + ((size_t)i * M + m) * 3;
+    o[0] = c[0]; o[1] = c[1]; o[2] = c[2];
+  }
+  __syncthreads();
+  T as_ = T(1), aa_ = T(1);
+  if (cusp_kind != 0) { as_ = cusp_alpha[0]; aa_ = cusp_alpha[1]; }
+  for (int i = tid; grad_r && i < N; i += nt) {
+    T g[3] = {T(0), T(0), T(0)};
+    for (int m = 0; m < M; ++m)
+      for (int a = 0; a < 3; ++a) g[a] += cb[((size_t)i * M + m) * 3 + a];
+    for (int j = 0; j < N; ++j) {
+      if (j == i) continue;
+      const T d[3] = {rb[3 * i] - rb[3 * j], rb[3 * i + 1] - rb[3 * j + 1], rb[3 * i + 2] - rb[3 * j + 2]};
+      const T rho = m_sqrt(Num<T>::eps() + d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+      if (cusp_kind != 0) {  // both cusp forms are -sc / (den0 + rho), counted once per unordered pair
+        const bool same = (i < n_up) == (j < n_up);
+        const T al = same ? as_ : aa_;
+        const T sc = (same ? same_scale : anti_scale) * (cusp_kind == 1 ? al * al : T(1) / (al * al));
+        const T den = (cusp_kind == 1 ? al : T(1) / al) + rho;
+        const T cc = sc / (den * den) / rho;
+        for (int a = 0; a < 3; ++a) g[a] += cc * d[a];
+      }
+      if (dE) {  // edge (sender j -> receiver i) carries [rho, d], edge (i -> j) [rho, -d]: rho is shared
+        const T* e1 = dE + (((size_t)b * N + j) * N + i) * 4;
+        const T* e2 = dE + (((size_t)b * N + i) * N + j) * 4;
+        const T rr = (e1[0] + e2[0]) / rho;
+        for (int a = 0; a < 3; ++a) g[a] += rr * d[a] + e1[1 + a] - e2[1 + a];
+      }
+    }
+    T* o = grad_r + ((size_t)b * N + i) * 3;
+    o[0] = g[0]; o[1] = g[1]; o[2] = g[2];
+  }
+  for (int m = tid; grad_R && m < M; m += nt) {
+    T g[3] = {T(0), T(0), T(0)};
+    for (int i = 0; i < N; ++i)
+      for (int a = 0; a < 3; ++a) g[a] -= cb[((size_t)i * M + m) * 3 + a];
+    T* o = grad_R + ((size_t)b * M + m) * 3;
+    o[0] = g[0]; o[1] = g[1]; o[2] = g[2];
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// Closed-form force terms per walker (reference force.py:30-38 nuclear_force, :122-132 Q, :172-194 bare + ZVQ,
+// :252-301 bare, all-electron part), one block per walker, nucleus m per thread, sums in a fixed order:
+//   F_nuc[m]  = sum_{n != m} Z_m Z_n (R_m - R_n) / rho_mn^3   (eps-safe norm, physics.py:112-116)
+//   bare[m]   = F_nuc[m] + Z_m sum_i d_im / |d_im|^3          (-grad_R of the Coulomb attraction, plain norm)
+//   Q[m]      = Z_m sum_i d_im / |d_im|
+//   zvq[m]    = F_nuc[m] + Z_m sum_i (g_i / |d| - d (d . g_i) / |d|^3),  g_i = grad_{r_i} log|psi|
+// d_im = r_i - R_m.  Every output nullable.
+// ------------------------------------------------------------------------------------------
+template <class T>
+__global__ void force_terms_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M,
+                                   const T* __restrict__ Z, const T* __restrict__ grad_r, T* __restrict__ bare,
+                                   T* __restrict__ zvq, T* __restrict__ Qo) {
+  const int b = blockIdx.x;
+  const T* rb = r + (size_t)b * N * 3;
+  const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
+  const T* gb = grad_r ? grad_r + (size_t)b * N * 3 : nullptr;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) {
+    const T zm = Z[m];
+    T fn[3] = {T(0), T(0), T(0)};
+    for (int n = 0; n < M; ++n) {
+      if (n == m) continue;
+      const T d[3] = {Rb[3 * m] - Rb[3 * n], Rb[3 * m + 1] - Rb[3 * n + 1], Rb[3 * m + 2] - Rb[3 * n + 2]};
+      const T rho = m_sqrt(Num<T>::eps() + d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+      const T s = zm * Z[n] / (rho * rho * rho);
+      for (int a = 0; a < 3; ++a) fn[a] += s * d[a];
+    }
+    T fb[3] = {T(0), T(0), T(0)}, q[3] = {T(0), T(0), T(0)}, fz[3] = {T(0), T(0), T(0)};
+    for (int i = 0; i < N; ++i) {
+      const T d[3] = {rb[3 * i] - Rb[3 * m], rb[3 * i + 1] - Rb[3 * m + 1], rb[3 * i + 2] - Rb[3 * m + 2]};
+      const T dist = m_sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), inv = T(1) / dist, inv3 = inv * inv * inv;
+      T dg = T(0);
+      if (gb) dg = d[0] * gb[3 * i] + d[1] * gb[3 * i + 1] + d[2] * gb[3 * i + 2];
+      for (int a = 0; a < 3; ++a) {
+        fb[a] += d[a] * inv3;
+        q[a] += d[a] * inv;
+        if (gb) fz[a] += gb[3 * i + a] * inv - d[a] * dg * inv3;
+      }
+    }
+    const size_t o = ((size_t)b * M + m) * 3;
+    for (int a = 0; a < 3; ++a) {
+      if (bare) bare[o + a] = fn[a] + zm * fb[a];
+      if (Qo) Qo[o + a] = zm * q[a];
+      if (zvq) zvq[o + a] = fn[a] + zm * fz[a];
+    }
+  }
+}
 
 // ==========================================================================================
 // conv-GNN ("PauliNet" test ansatz, tests/conf/ansatz.yaml) reverse pass, plain-forward VALUE layouts:

@@ -14,7 +14,7 @@ from . import _lib
 from . import params as PN
 from .spec import AnsatzSpec
 
-MODE_FORWARD, MODE_LOCAL_ENERGY, MODE_VJP, MODE_MCMC, MODE_LANGEVIN, MODE_SPIN = 0, 1, 2, 3, 4, 5
+MODE_FORWARD, MODE_LOCAL_ENERGY, MODE_VJP, MODE_MCMC, MODE_LANGEVIN, MODE_SPIN, MODE_GRAD_POS = 0, 1, 2, 3, 4, 5, 6
 _TORCH_DTYPE = {0: torch.float64, 1: torch.float32}
 
 
@@ -598,6 +598,41 @@ class Engine:
                                 ptr(ratio), ws.data_ptr(), ws.numel(), self._stream())
         self._check(rc, 'dqmc_spin')
         return s2, ratio
+
+    def grad_positions(self, r, R, want_r=True, want_R=True, max_ws_bytes=None):
+        """-> (sign[B], log[B], grad_r[B, N, 3] or None, grad_R[B, M, 3] or None): gradients of log|psi| with respect to the
+        electron and nuclear positions by the reverse pass (dqmc_wf_grad_positions; reference force.py:96-118).  Psiformer and
+        FermiNet: both; TransPsiformer: grad_r only; conv-GNN kinds and the additive backflow branch: not available."""
+        r = self._prep(r)
+        B, N = r.shape[0], r.shape[1]
+        R, Rb = self._R(R, B)
+        mk = lambda *s: torch.empty(*s, dtype=self.dtype, device=self.device)
+        sign, log = mk(B), mk(B)
+        gr = mk(B, N, 3) if want_r else None
+        gR = mk(B, self.spec.n_nuc, 3) if want_R else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        ws = self.workspace(B, MODE_GRAD_POS, max_ws_bytes)
+        rc = self.lib.dqmc_wf_grad_positions(self.h, r.data_ptr(), R.data_ptr(), Rb, B, sign.data_ptr(), log.data_ptr(), ptr(gr),
+                                             ptr(gR), ws.data_ptr(), ws.numel(), self._stream())
+        self._check(rc, 'dqmc_wf_grad_positions')
+        return sign, log, gr, gR
+
+    def force_terms(self, r, R, grad_r=None):
+        """-> (bare[B, M, 3], zvq[B, M, 3] or None, Q[B, M, 3]): the closed-form per-walker force terms of dqmc_force_terms
+        (all-electron Hamiltonians); zvq needs ``grad_r`` [B, N, 3] = grad_r log|psi|."""
+        r = self._prep(r)
+        B = r.shape[0]
+        R, Rb = self._R(R, B)
+        mk = lambda *s: torch.empty(*s, dtype=self.dtype, device=self.device)
+        M = self.spec.n_nuc
+        bare, Q = mk(B, M, 3), mk(B, M, 3)
+        g = self._prep(grad_r).reshape(B, -1) if grad_r is not None else None
+        zvq = mk(B, M, 3) if g is not None else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        rc = self.lib.dqmc_force_terms(self.h, r.data_ptr(), R.data_ptr(), Rb, B, ptr(g), bare.data_ptr(), ptr(zvq), Q.data_ptr(),
+                                       self._stream())
+        self._check(rc, 'dqmc_force_terms')
+        return bare, zvq, Q
 
     def mcmc_sweep(self, state, R, n_sub, target_acceptance=0.57, max_age=None, seed=0, step0=0, walker_offset=0,
                    noise_normal=None, noise_uniform=None, max_ws_bytes=None, exchange_probability=0.0, exchange_flags=None,

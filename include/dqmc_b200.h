@@ -31,7 +31,7 @@ enum { DQMC_PSIFORMER = 0, DQMC_FERMINET = 1, DQMC_TRANSPSIFORMER = 2, DQMC_PAUL
 enum { DQMC_F64 = 0, DQMC_F32 = 1 };
 enum { DQMC_GEMM_SIMT = 0, DQMC_GEMM_TCGEN05 = 1 };
 enum { DQMC_MODE_FORWARD = 0, DQMC_MODE_LOCAL_ENERGY = 1, DQMC_MODE_VJP = 2, DQMC_MODE_MCMC = 3, DQMC_MODE_LANGEVIN = 4,
-       DQMC_MODE_SPIN = 5 };
+       DQMC_MODE_SPIN = 5, DQMC_MODE_GRAD_POS = 6 };
 
 /* Ansatz + Hamiltonian constants that fix the kernel shapes.
  * reference: src/deepqmc/conf/ansatz/psiformer.yaml, ferminet.yaml (SURVEY.md 8(a0));
@@ -208,6 +208,31 @@ int dqmc_wf_vjp_params(dqmc_handle h, const void* r, const void* R, int32_t R_ba
 int dqmc_spin(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, const void* sign,
               const void* log, int32_t down_idx, void* out_s2, void* out_ratio, void* workspace, int64_t workspace_bytes,
               void* stream);
+
+/* Position gradients of log|psi| per walker: out_grad_r[B][N][3] = grad_r log|psi|, out_grad_R[B][M][3] = grad_R log|psi|
+ * (either nullable), plus sign / log [B] (required).  The reverse pass of dqmc_wf_vjp_params with cotangent 1 per walker and no
+ * parameter gradients, carried on through the electron-nucleus features, the envelopes and the cusps into the pair cotangent
+ * c_im = d log|psi| / d(r_i - R_m); grad_{r_i} = sum_m c_im + the e-e terms, grad_{R_m} = -sum_i c_im.  No atomics: every sum
+ * runs in a fixed order, a repeated call is bitwise identical.  Psiformer and FermiNet: both outputs; TransPsiformer: grad_r
+ * only (its nuclear tokens and envelope exponents depend on R through the host-side nuclear stream; a non-null out_grad_R is
+ * status 2); conv-GNN kinds and the additive backflow branch: status 2.  n_walkers = 0 is a no-op.
+ * Workspace: dqmc_workspace_bytes(h, B, DQMC_MODE_GRAD_POS) (walkers are chunked to fit).
+ * replaces: force.py:96-118 make_grad_nuc_log_wf / make_grad_log_wf (jax.grad of wf(...).log with respect to R and r). */
+int dqmc_wf_grad_positions(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers,
+                           void* out_sign, void* out_log, void* out_grad_r, void* out_grad_R,
+                           void* workspace, int64_t workspace_bytes, void* stream);
+
+/* Closed-form force terms per walker [B][M][3] (device, every output nullable), d_im = r_i - R_m, Z = the nuclear charges:
+ *   out_bare = F_nuc + Z_m sum_i d_im / |d_im|^3                    (bare Hellmann-Feynman force, all-electron)
+ *   out_zvq  = F_nuc + sum_i (dQ_m / dr_i)^T grad_i log|psi|        (needs grad_r[B][N][3]; otherwise status 2)
+ *   out_Q    = Q_m = Z_m sum_i d_im / |d_im|
+ * F_nuc = -grad_R E_nuc (eps-safe nucleus-nucleus distances); dQ_ma / dr_ib = Z_m (delta_ab / |d| - d_a d_b / |d|^3).
+ * Engines with an effective core potential (local or non-local) or a pseudo-Hamiltonian return status 2.  One block per
+ * walker, sums in a fixed order.
+ * replaces: force.py:30-38 nuclear_force, :122-132 Q, :172-194 make_bare_plus_zvq_term, :252-301 evaluate_hf_force_bare
+ *           (all-electron part). */
+int dqmc_force_terms(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers,
+                     const void* grad_r, void* out_bare, void* out_zvq, void* out_Q, void* stream);
 
 /* Switch the handle's Hamiltonian to a pseudo-Hamiltonian (fully local replacement of the semi-local ECP):
  * tables[n_tab][2][n_grid] (host, fp64) = r V_loc(r) and r V_L2(r) per tabulated element on the uniform grid
