@@ -941,12 +941,9 @@ struct Engine : EngineBase {
   // (pos: the position mode of dqmc_wf_grad_positions, Psiformer kinds and FermiNet)
   int64_t vjp_chunk_bytes(int Bc, bool pos = false) {
     DryPass dp(this);
-    const Arena a(this, plan_base());
     const PosOut none{nullptr, nullptr};
-    const PosOut* po = pos ? &none : nullptr;
-    if (gnn) vjp_chunk_paulinet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr);
-    else if (cfg.kind == DQMC_FERMINET) vjp_chunk_ferminet(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr, po);
-    else vjp_chunk(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, a, nullptr, po);
+    reverse_chunk(nullptr, nullptr, 0, Bc, nullptr, nullptr, nullptr, nullptr, Arena(this, plan_base()), nullptr,
+                  pos ? &none : nullptr);
     return dp.bytes();
   }
   bool has_pos_pass() const { return !gnn && !cfg.backflow_add; }
@@ -1862,6 +1859,8 @@ struct Engine : EngineBase {
 
   // ---- parameter VJP of the plain forward (Psiformer): SURVEY.md 8(f) N1 ------------------------
   const T* PT(const std::string& n) const { return d_params_t + off(n); }
+  // entry n's slot in the parameter cotangent G; null when G is (the position mode accumulates no parameter gradients)
+  T* PG(T* G, const std::string& n) const { return G ? G + off(n) : nullptr; }
   // C = (Res) + A @ W with a raw weight pointer (CUDA-core kernel; used by the reverse pass with transposed weights)
   int gemm_raw(const T* A, int lda, const T* W0, const T* W1, int zsplit, int ldw, const T* Res, int ldr, T* C, int ldc,
                int Mr, int Nc, int Kc, int sliced, cudaStream_t st) {
@@ -1873,8 +1872,10 @@ struct Engine : EngineBase {
     DQ_LAUNCH((gemm_kernel<T, BM, BN, BK, TM, TN>), grid, dim3(256), 0, st, g);
     return 0;
   }
-  // dW += A^T dY over `rows` rows (optionally only electrons lo <= i < hi of every walker), db += column sums
+  // dW += A^T dY over `rows` rows (optionally only electrons lo <= i < hi of every walker), db += column sums; a null dW / db
+  // (PG in the position mode) accumulates nothing
   void wgrad(const T* A, int lda, const T* dY, int ldy, int rows, int Kc, int Nc, T* dW, int lo, int hi, cudaStream_t st) {
+    if (!dW) return;
     int nz = (rows + 4095) / 4096;
     if (nz > 256) nz = 256;
     if (nz < 1) nz = 1;
@@ -1883,6 +1884,7 @@ struct Engine : EngineBase {
               rows, Kc, Nc, rpb, hi > lo ? N : 0, lo, hi, dW, Nc);
   }
   void bgrad(const T* dZ, int ld, int rows, int Nc, T* db, cudaStream_t st, int lo = 0, int hi = 0) {
+    if (!db) return;
     int ny = (rows + 2047) / 2048;
     if (ny > 128) ny = 128;
     if (ny < 1) ny = 1;
@@ -1909,15 +1911,66 @@ struct Engine : EngineBase {
               cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr, pb.cbuf, po->gr, po->gR);
   }
 
+  // slater_bwd_kernel's launch: as many warps per block (1 ... 4) as fit 96 KiB of dynamic shared memory.  The launch and
+  // the shared-memory opt-in both take it from here, so the opt-in always covers the launch (DESIGN §8).
+  int slater_bwd_shape(int& wpb, size_t& smem) {
+    const size_t pw = slater_bwd_smem_per_warp<T>(N);
+    wpb = (int)((96 * 1024) / pw);
+    wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
+    smem = pw * wpb;
+    if (smem > 227 * 1024) { err = "system too large for the shared-memory tiling of the reverse pass (N)"; return 2; }
+    return 0;
+  }
+
+  // Determinant head of the reverse passes, from the backflow output BF [Bc N][KN] to its cotangent dBF: determinants and
+  // their sum (sign, logp), then back through both.  The conv-GNN kinds' spin-factorised determinants, hk.Linear determinant
+  // weights and Jastrow (jastrow: the Jastrow tape's output, null without one) follow from cfg.  G null: position mode, no
+  // parameter gradients; cpart: its pair-cotangent buffer (null otherwise).
+  int det_head_bwd(const T* r, const T* R, int Rb, int Bc, const T* BF, T* dBF, const T* wts, T* sign, T* logp, T* G,
+                   const T* jastrow, T* cpart, Arena& a, cudaStream_t st) {
+    T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
+    if (a.left() < 0) { err = "internal: reverse-pass buffers exceed the planned workspace"; return 3; }
+    int wpb;
+    size_t smem;
+    int rc = slater_bwd_shape(wpb, smem);
+    if (rc) return rc;
+    const int full_det = cfg.factorized_det ? 0 : 1;
+    const T* conf = cfg.conf_linear ? P("conf.w") : nullptr;
+    const T* nuc = cfg.nuc_cusp_kind ? P("cusp.nuc") : nullptr;
+    const int sl_wpb = slater_warps_per_block<T>(N);
+    DQ_LAUNCH(slater_kernel<T>, dim3((Bc * K + sl_wpb - 1) / sl_wpb), dim3(32 * sl_wpb), slater_smem_bytes<T>(N), st, r, R, Rb, N,
+              M, cfg.n_up, K, 1, Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), BF, KN, dsign, dlog,
+              (T*)nullptr, (T*)nullptr, env_rep, full_det, (const T*)nullptr, (const T*)nullptr, 0, 1);
+    FinalizeCfg fc = finalize_cfg(1);
+    fc.ecp_terms = 0;  // sign and log only: no local energy, no ECP table
+    DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb, (const T*)dsign,
+              (const T*)dlog, (const T*)nullptr, (const T*)nullptr, P("cusp.alpha"), (const T*)d_zval, (const T*)nullptr,
+              (const int*)d_ecp_mask, Bc, sign, logp, (T*)nullptr, (T*)nullptr, (T*)nullptr, conf, jastrow, nuc, PhArgs<T>());
+    // ---- reverse ------------------------------------------------------------------------------------------------
+    // the conv-GNN kinds pass cusp kind 0 (fixed cusp exponent: no gradient)
+    DQ_LAUNCH(finalize_bwd_kernel<T>, dim3((Bc + 127) / 128), dim3(128), 0, st, r, N, cfg.n_up, K, Bc, (const T*)dsign,
+              (const T*)dlog, wts, gnn ? 0 : cfg.cusp_kind, (T)cfg.cusp_same_scale, (T)cfg.cusp_anti_scale, P("cusp.alpha"), dld,
+              gnn ? (T*)nullptr : PG(G, "cusp.alpha"), R, Rb, M, cfg.nuc_cusp_kind, nuc,
+              cfg.nuc_cusp_kind ? PG(G, "cusp.nuc") : (T*)nullptr, conf, cfg.conf_linear ? PG(G, "conf.w") : (T*)nullptr);
+    DQ_LAUNCH(slater_bwd_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), smem, st, r, R, Rb, N, M, cfg.n_up, K, Bc * K,
+              P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), BF, KN, (const T*)dld, dBF, PG(G, "env.pi_up"),
+              PG(G, "env.pi_dn"), PG(G, "env.zeta_up"), PG(G, "env.zeta_dn"), env_rep, full_det, cpart);
+    return 0;
+  }
+  // linear backflow heads of the Psiformer kinds and FermiNet: dX_L = dBF W_spin^T, dW_spin += X_L[spin rows]^T dBF[spin rows]
+  void bf_head_bwd(const T* XL, const T* dBF, T* dXL, int Bc, T* G, cudaStream_t st) {
+    gemm_raw(dBF, KN, PT("bf.up"), PT("bf.dn"), cfg.n_up, d, nullptr, 0, dXL, d, Bc, d, KN, 1, st);
+    wgrad(XL, d, dBF, KN, Bc * N, d, KN, PG(G, "bf.up"), 0, cfg.n_up, st);
+    wgrad(XL, d, dBF, KN, Bc * N, d, KN, PG(G, "bf.dn"), cfg.n_up, N, st);
+  }
+
   int vjp_chunk(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a, cudaStream_t st,
-                const PosOut* po = nullptr) {
+                const PosOut* po) {
     const int L = cfg.n_layers, rows = Bc * N, F = 4 * M + 1;
-    auto gp = [&](const std::string& n) { return po ? (T*)nullptr : G + off(n); };  // parameter cotangent (none in position mode)
     std::vector<T*> X(L + 1), QKV(L), O(L), A(L), M1(L);
     for (int l = 0; l <= L; ++l) X[l] = a.take<T>((size_t)rows * d);
     for (int l = 0; l < L; ++l) { QKV[l] = a.take<T>((size_t)rows * 3 * d); O[l] = a.take<T>((size_t)rows * d); A[l] = a.take<T>((size_t)rows * d); M1[l] = a.take<T>((size_t)rows * d); }
     T* BF = a.take<T>((size_t)rows * KN); T* dBF = a.take<T>((size_t)rows * KN);
-    T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
     T* dXn = a.take<T>((size_t)rows * d); T* dZ = a.take<T>((size_t)rows * d); T* dM1 = a.take<T>((size_t)rows * d);
     T* dA = a.take<T>((size_t)rows * d); T* dO = a.take<T>((size_t)rows * d); T* dQKV = a.take<T>((size_t)rows * 3 * d);
     T* dX = a.take<T>((size_t)rows * d); T* Feat = a.take<T>((size_t)rows * F);
@@ -1941,64 +1994,32 @@ struct Engine : EngineBase {
       DQ_LAUNCH(tanh_fl_kernel<T>, dim3(rows, (d + 127) / 128), dim3(128), 0, st, X[l + 1], d, (const T*)A[l], d, 1, d, T(1));
     }
     gemm(X[L], d, "bf.up", "bf.dn", cfg.n_up, KN, nullptr, nullptr, 0, BF, KN, Bc, KN, d, 1, 1, N, st);
-    const int sl_wpb = slater_warps_per_block<T>(N);
-    DQ_LAUNCH(slater_kernel<T>, dim3((Bc * K + sl_wpb - 1) / sl_wpb), dim3(32 * sl_wpb), slater_smem_bytes<T>(N), st, r, R, Rb, N,
-              M, cfg.n_up, K, 1, Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN,
-              dsign, dlog, (T*)nullptr, (T*)nullptr, env_rep, 1, (const T*)nullptr, (const T*)nullptr, 0, 1);
-    FinalizeCfg fc;
-    fc.N = N; fc.M = M; fc.n_up = cfg.n_up; fc.K = K; fc.S = 1; fc.cusp_kind = cfg.cusp_kind;
-    fc.cusp_same_scale = cfg.cusp_same_scale; fc.cusp_anti_scale = cfg.cusp_anti_scale; fc.ecp_terms = 0;
-    fc.nuc_cusp_kind = cfg.nuc_cusp_kind;
-    DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb, (const T*)dsign,
-              (const T*)dlog, (const T*)nullptr, (const T*)nullptr, P("cusp.alpha"), (const T*)d_zval, (const T*)nullptr,
-              (const int*)d_ecp_mask, Bc, sign, logp, (T*)nullptr, (T*)nullptr, (T*)nullptr, (const T*)nullptr, (const T*)nullptr,
-              cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr, PhArgs<T>());
-    // ---- reverse ------------------------------------------------------------------------------------------------
-    DQ_LAUNCH(finalize_bwd_kernel<T>, dim3((Bc + 127) / 128), dim3(128), 0, st, r, N, cfg.n_up, K, Bc, (const T*)dsign,
-              (const T*)dlog, wts, cfg.cusp_kind, (T)cfg.cusp_same_scale, (T)cfg.cusp_anti_scale, P("cusp.alpha"), dld,
-              gp("cusp.alpha"), R, Rb, M, cfg.nuc_cusp_kind, cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr,
-              cfg.nuc_cusp_kind ? gp("cusp.nuc") : (T*)nullptr, (const T*)nullptr, (T*)nullptr);
-    {
-      const size_t pw = slater_bwd_smem_per_warp<T>(N);
-      int wpb = (int)((96 * 1024) / pw);
-      wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
-      DQ_LAUNCH(slater_bwd_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), pw * wpb, st, r, R, Rb, N, M, cfg.n_up, K,
-                Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, (const T*)dld, dBF,
-                gp("env.pi_up"), gp("env.pi_dn"), gp("env.zeta_up"), gp("env.zeta_dn"), env_rep, 1, pb.cpart);
-    }
-    // backflow heads: dX_L = dBF W_spin^T, dW_spin += X_L[spin rows]^T dBF[spin rows]
-    gemm_raw(dBF, KN, PT("bf.up"), PT("bf.dn"), cfg.n_up, d, nullptr, 0, dXn, d, Bc, d, KN, 1, st);
-    if (!po) {
-      wgrad(X[L], d, dBF, KN, rows, d, KN, G + off("bf.up"), 0, cfg.n_up, st);
-      wgrad(X[L], d, dBF, KN, rows, d, KN, G + off("bf.dn"), cfg.n_up, N, st);
-    }
+    int rc = det_head_bwd(r, R, Rb, Bc, BF, dBF, wts, sign, logp, G, nullptr, pb.cpart, a, st);
+    if (rc) return rc;
+    bf_head_bwd(X[L], dBF, dXn, Bc, G, st);
     const size_t nel = (size_t)rows * d;
     for (int l = L - 1; l >= 0; --l) {
       const std::string q = "L" + std::to_string(l) + ".";
       // X_{l+1} = A + tanh(M1 W2 + b2)
       DQ_LAUNCH(tanh_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dXn, (const T*)X[l + 1],
                 (const T*)A[l], dZ, nel);
-      if (!po) {
-        bgrad(dZ, d, rows, d, G + off(q + "b2"), st);
-        wgrad(M1[l], d, dZ, d, rows, d, d, G + off(q + "w2"), 0, 0, st);
-      }
+      bgrad(dZ, d, rows, d, PG(G, q + "b2"), st);
+      wgrad(M1[l], d, dZ, d, rows, d, d, PG(G, q + "w2"), 0, 0, st);
       gemm_raw(dZ, d, PT(q + "w2"), nullptr, 0, d, nullptr, 0, dM1, d, rows, d, d, 0, st);
       // M1 = tanh(A W1 + b1)
       DQ_LAUNCH(tanh_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dM1, (const T*)M1[l],
                 (const T*)nullptr, dZ, nel);
-      if (!po) {
-        bgrad(dZ, d, rows, d, G + off(q + "b1"), st);
-        wgrad(A[l], d, dZ, d, rows, d, d, G + off(q + "w1"), 0, 0, st);
-      }
+      bgrad(dZ, d, rows, d, PG(G, q + "b1"), st);
+      wgrad(A[l], d, dZ, d, rows, d, d, PG(G, q + "w1"), 0, 0, st);
       gemm_raw(dZ, d, PT(q + "w1"), nullptr, 0, d, dXn, d, dA, d, rows, d, d, 0, st);  // dA = dX_{l+1} + dZ1 W1^T
       // A = X + O Wo
-      if (!po) wgrad(O[l], d, dA, d, rows, d, d, G + off(q + "wo"), 0, 0, st);
+      wgrad(O[l], d, dA, d, rows, d, d, PG(G, q + "wo"), 0, 0, st);
       gemm_raw(dA, d, PT(q + "wo"), nullptr, 0, d, nullptr, 0, dO, d, rows, d, d, 0, st);
       DQ_LAUNCH(attn_bwd_kernel<T>, dim3(Bc, H), dim3(128), attn_bwd_smem_bytes<T>(N, dh, Mn), st, (const T*)QKV[l], 3 * d,
                 (const T*)dO, d, N, dh, d, scale, dQKV, Mn > 0 ? P(q + "kn") : (const T*)nullptr,
-                Mn > 0 ? P(q + "vn") : (const T*)nullptr, Mn, Mn > 0 ? gp(q + "kn") : (T*)nullptr,
-                Mn > 0 ? gp(q + "vn") : (T*)nullptr);
-      if (!po) wgrad(X[l], d, dQKV, 3 * d, rows, d, 3 * d, G + off(q + "wqkv"), 0, 0, st);
+                Mn > 0 ? P(q + "vn") : (const T*)nullptr, Mn, Mn > 0 ? PG(G, q + "kn") : (T*)nullptr,
+                Mn > 0 ? PG(G, q + "vn") : (T*)nullptr);
+      wgrad(X[l], d, dQKV, 3 * d, rows, d, 3 * d, PG(G, q + "wqkv"), 0, 0, st);
       gemm_raw(dQKV, 3 * d, PT(q + "wqkv"), nullptr, 0, d, dA, d, dX, d, rows, d, 3 * d, 0, st);  // dX_l = dA + dQKV Wqkv^T
       T* t = dXn; dXn = dX; dX = t;
     }
@@ -2016,8 +2037,7 @@ struct Engine : EngineBase {
   // incoming edges], shared edge MLP u, residuals / sqrt(2).  The raw input features carry no parameters, so the
   // parameter chain stops at the first layer's weights; the position mode carries it on to the raw node and edge features.
   int vjp_chunk_ferminet(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a,
-                         cudaStream_t st, const PosOut* po = nullptr) {
-    auto gp = [&](const std::string& n) { return po ? (T*)nullptr : G + off(n); };
+                         cudaStream_t st, const PosOut* po) {
     const int L = cfg.n_layers, rows = Bc * N, rowsE = Bc * N * N, de = cfg.edge_dim, d0 = 4 * M;
     const T isq2 = (T)0.70710678118654752440;
     std::vector<T*> Hs(L + 1), Es(L), Fs(L);
@@ -2029,7 +2049,6 @@ struct Engine : EngineBase {
     for (int l = 0; l < L; ++l) { Es[l] = a.take<T>((size_t)rowsE * dEd[l]); Fs[l] = a.take<T>((size_t)rows * (3 * dH[l] + 2 * dEd[l])); }
     const int fmax = 3 * (d > d0 ? d : d0) + 2 * (de > 4 ? de : 4);
     T* BF = a.take<T>((size_t)rows * KN); T* dBF = a.take<T>((size_t)rows * KN);
-    T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
     const int dx = po ? std::max(d, d0) : d, dex = po ? std::max(de, 4) : de;  // the position mode reaches layer 0's inputs
     T* dXa = a.take<T>((size_t)rows * dx); T* dXb = a.take<T>((size_t)rows * dx); T* dZ = a.take<T>((size_t)rows * d);
     T* dF = a.take<T>((size_t)rows * fmax);
@@ -2056,40 +2075,13 @@ struct Engine : EngineBase {
       }
     }
     gemm(Hs[L], d, "bf.up", "bf.dn", cfg.n_up, KN, nullptr, nullptr, 0, BF, KN, Bc, KN, d, 1, 1, N, st);
-    const int sl_wpb = slater_warps_per_block<T>(N);
-    DQ_LAUNCH(slater_kernel<T>, dim3((Bc * K + sl_wpb - 1) / sl_wpb), dim3(32 * sl_wpb), slater_smem_bytes<T>(N), st, r, R, Rb, N,
-              M, cfg.n_up, K, 1, Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN,
-              dsign, dlog, (T*)nullptr, (T*)nullptr, env_rep, 1, (const T*)nullptr, (const T*)nullptr, 0, 1);
-    FinalizeCfg fc;
-    fc.N = N; fc.M = M; fc.n_up = cfg.n_up; fc.K = K; fc.S = 1; fc.cusp_kind = cfg.cusp_kind;
-    fc.cusp_same_scale = cfg.cusp_same_scale; fc.cusp_anti_scale = cfg.cusp_anti_scale; fc.ecp_terms = 0;
-    fc.nuc_cusp_kind = cfg.nuc_cusp_kind;
-    DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb, (const T*)dsign,
-              (const T*)dlog, (const T*)nullptr, (const T*)nullptr, P("cusp.alpha"), (const T*)d_zval, (const T*)nullptr,
-              (const int*)d_ecp_mask, Bc, sign, logp, (T*)nullptr, (T*)nullptr, (T*)nullptr, (const T*)nullptr, (const T*)nullptr,
-              cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr, PhArgs<T>());
-    // ---- reverse -------------------------------------------------------------------------------------------------
-    DQ_LAUNCH(finalize_bwd_kernel<T>, dim3((Bc + 127) / 128), dim3(128), 0, st, r, N, cfg.n_up, K, Bc, (const T*)dsign,
-              (const T*)dlog, wts, cfg.cusp_kind, (T)cfg.cusp_same_scale, (T)cfg.cusp_anti_scale, P("cusp.alpha"), dld,
-              gp("cusp.alpha"), R, Rb, M, cfg.nuc_cusp_kind, cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr,
-              cfg.nuc_cusp_kind ? gp("cusp.nuc") : (T*)nullptr, (const T*)nullptr, (T*)nullptr);
-    {
-      const size_t pw = slater_bwd_smem_per_warp<T>(N);
-      int wpb = (int)((96 * 1024) / pw);
-      wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
-      DQ_LAUNCH(slater_bwd_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), pw * wpb, st, r, R, Rb, N, M, cfg.n_up, K,
-                Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, (const T*)dld, dBF,
-                gp("env.pi_up"), gp("env.pi_dn"), gp("env.zeta_up"), gp("env.zeta_dn"), env_rep, 1, pb.cpart);
-    }
+    int rc = det_head_bwd(r, R, Rb, Bc, BF, dBF, wts, sign, logp, G, nullptr, pb.cpart, a, st);
+    if (rc) return rc;
     T* dHn = dXa;   // gradient w.r.t. H_{l+1}
     T* dHc = dXb;   // gradient w.r.t. H_l (being built)
     T* dEn = dEa;   // gradient w.r.t. E_{l+1} (valid for l < L - 1)
     T* dEc = dEb;
-    gemm_raw(dBF, KN, PT("bf.up"), PT("bf.dn"), cfg.n_up, d, nullptr, 0, dHn, d, Bc, d, KN, 1, st);
-    if (!po) {
-      wgrad(Hs[L], d, dBF, KN, rows, d, KN, G + off("bf.up"), 0, cfg.n_up, st);
-      wgrad(Hs[L], d, dBF, KN, rows, d, KN, G + off("bf.dn"), cfg.n_up, N, st);
-    }
+    bf_head_bwd(Hs[L], dBF, dHn, Bc, G, st);
     for (int l = L - 1; l >= 0; --l) {
       const std::string q = "F" + std::to_string(l) + ".";
       const int dc = dH[l], ec = dEd[l], fin = 3 * dc + 2 * ec;
@@ -2098,10 +2090,8 @@ struct Engine : EngineBase {
       // H_{l+1} = s (H_l + tanh(F Wg + bg))  |  tanh(F Wg + bg)
       DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dHn, (const T*)Hs[l + 1],
                 (const T*)(res_h ? Hs[l] : nullptr), res_h ? isq2 : T(1), dZ, nel);
-      if (!po) {
-        bgrad(dZ, d, rows, d, G + off(q + "bg"), st);
-        wgrad(Fs[l], fin, dZ, d, rows, fin, d, G + off(q + "wg"), 0, 0, st);
-      }
+      bgrad(dZ, d, rows, d, PG(G, q + "bg"), st);
+      wgrad(Fs[l], fin, dZ, d, rows, fin, d, PG(G, q + "wg"), 0, 0, st);
       if (l > 0 || po) {
         gemm_raw(dZ, d, PT(q + "wg"), nullptr, 0, fin, nullptr, 0, dF, fin, rows, fin, d, 0, st);
         DQ_LAUNCH(fermi_agg_bwd_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)dF, dc, ec, N, cfg.n_up,
@@ -2112,10 +2102,8 @@ struct Engine : EngineBase {
         const size_t nee = (size_t)rowsE * de;
         DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nee + 255) / 256)), dim3(256), 0, st, (const T*)dEn, (const T*)Es[l + 1],
                   (const T*)(res_e ? Es[l] : nullptr), res_e ? isq2 : T(1), dZe, nee);
-        if (!po) {
-          bgrad(dZe, de, rowsE, de, G + off(q + "bu"), st);
-          wgrad(Es[l], ec, dZe, de, rowsE, ec, de, G + off(q + "wu"), 0, 0, st);
-        }
+        bgrad(dZe, de, rowsE, de, PG(G, q + "bu"), st);
+        wgrad(Es[l], ec, dZe, de, rowsE, ec, de, PG(G, q + "wu"), 0, 0, st);
         if (l > 0 || po) {
           gemm_raw(dZe, de, PT(q + "wu"), nullptr, 0, ec, dEc, ec, dEc, ec, rowsE, ec, de, 0, st);  // dE_l += dZe Wu^T
           if (res_e) {
@@ -2288,36 +2276,9 @@ struct Engine : EngineBase {
     if (rc) return rc;
     if (cfg.mult_act == 1)
       DQ_LAUNCH(act_fl_kernel<T>, dim3(rows, (KN + 127) / 128), dim3(128), 0, st, BF, KN, (const T*)nullptr, 0, 1, KN, T(1), 2);
-    T* dsign = a.take<T>((size_t)Bc * K); T* dlog = a.take<T>((size_t)Bc * K); T* dld = a.take<T>((size_t)Bc * K);
-    const int full_det = cfg.factorized_det ? 0 : 1;
-    const int sl_wpb = slater_warps_per_block<T>(N);
-    DQ_LAUNCH(slater_kernel<T>, dim3((Bc * K + sl_wpb - 1) / sl_wpb), dim3(32 * sl_wpb), slater_smem_bytes<T>(N), st, r, R, Rb, N,
-              M, cfg.n_up, K, 1, Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN,
-              dsign, dlog, (T*)nullptr, (T*)nullptr, env_rep, full_det, (const T*)nullptr, (const T*)nullptr, 0, 1);
-    FinalizeCfg fc;
-    fc.N = N; fc.M = M; fc.n_up = cfg.n_up; fc.K = K; fc.S = 1; fc.cusp_kind = cfg.cusp_kind;
-    fc.cusp_same_scale = cfg.cusp_same_scale; fc.cusp_anti_scale = cfg.cusp_anti_scale; fc.ecp_terms = 0;
-    fc.nuc_cusp_kind = cfg.nuc_cusp_kind;
-    DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb, (const T*)dsign,
-              (const T*)dlog, (const T*)nullptr, (const T*)nullptr, P("cusp.alpha"), (const T*)d_zval, (const T*)nullptr,
-              (const int*)d_ecp_mask, Bc, sign, logp, (T*)nullptr, (T*)nullptr, (T*)nullptr,
-              cfg.conf_linear ? P("conf.w") : (const T*)nullptr, cfg.jastrow_n > 0 ? (const T*)Jt.a.back() : (const T*)nullptr,
-              cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr, PhArgs<T>());
-    // ---- reverse ---------------------------------------------------------------------------------------------------
-    DQ_LAUNCH(finalize_bwd_kernel<T>, dim3((Bc + 127) / 128), dim3(128), 0, st, r, N, cfg.n_up, K, Bc, (const T*)dsign,
-              (const T*)dlog, wts, 0 /*fixed cusp exponent: no gradient*/, (T)cfg.cusp_same_scale, (T)cfg.cusp_anti_scale,
-              P("cusp.alpha"), dld, (T*)nullptr, R, Rb, M, cfg.nuc_cusp_kind, cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr,
-              cfg.nuc_cusp_kind ? G + off("cusp.nuc") : (T*)nullptr, cfg.conf_linear ? P("conf.w") : (const T*)nullptr,
-              cfg.conf_linear ? G + off("conf.w") : (T*)nullptr);
-    {
-      const size_t pw = slater_bwd_smem_per_warp<T>(N);
-      int wpb = (int)((96 * 1024) / pw);
-      wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
-      DQ_LAUNCH(slater_bwd_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), pw * wpb, st, r, R, Rb, N, M, cfg.n_up, K,
-                Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, (const T*)dld, dBF,
-                G + off("env.pi_up"), G + off("env.pi_dn"), G + off("env.zeta_up"), G + off("env.zeta_dn"), env_rep, full_det,
-                (T*)nullptr);
-    }
+    rc = det_head_bwd(r, R, Rb, Bc, BF, dBF, wts, sign, logp, G, cfg.jastrow_n > 0 ? (const T*)Jt.a.back() : nullptr, nullptr,
+                      a, st);
+    if (rc) return rc;
     // scratch for the reverse sweep
     const int xm = std::max(d, xd[0]);
     const int hm = std::max(gnn_hmax(), xm), hn = std::max(gnn_hnode_max(), e), em = gnn_emax();
@@ -2432,37 +2393,34 @@ struct Engine : EngineBase {
     return 0;
   }
 
-  int vjp_params(const void* r_, const void* R_, int Rb, int B, const void* weights, void* sign, void* logp,
-                 void* grad_params, void* ws, int64_t wsb, cudaStream_t st) override {
+  // one reverse-pass chunk of the engine's kind; po: position mode (Psiformer kinds and FermiNet only)
+  int reverse_chunk(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, const Arena& a,
+                    cudaStream_t st, const PosOut* po) {
+    if (gnn) return vjp_chunk_paulinet(r, R, Rb, Bc, wts, sign, logp, G, a, st);
+    if (cfg.kind == DQMC_FERMINET) return vjp_chunk_ferminet(r, R, Rb, Bc, wts, sign, logp, G, a, st, po);
+    return vjp_chunk(r, R, Rb, Bc, wts, sign, logp, G, a, st, po);
+  }
 
-    if (cfg.backflow_add) { err = "dqmc_wf_vjp_params: additive backflow branch has no reverse pass"; return 2; }
-    const T* r = (const T*)r_;
-    const T* R = (const T*)R_;
-    DQ_CHECK(cudaMemsetAsync(grad_params, 0, sizeof(T) * total, st));
-    if (B == 0) return 0;  // empty batch: zero gradient
-    // walkers per chunk: activations of every layer stay resident for the reverse pass (64 buffers, 256 B alignment each)
-    const bool fermi = cfg.kind == DQMC_FERMINET;
-    // largest chunk whose buffers (measured by a dry pass of the chunk function) fit the caller's workspace
+  // The reverse pass over B walkers in chunks: activations of every layer stay resident for the reverse pass, so a chunk is
+  // the largest one whose buffers (a dry pass of the chunk function) fit the caller's workspace.  po: position mode, its
+  // outputs from walker 0 on (wts and G null there); what: the entry point the workspace refusal names.
+  int reverse_pass(const T* r, const T* R, int Rb, int B, const T* wts, T* sign, T* logp, T* G, const PosOut* po, void* ws,
+                   int64_t wsb, cudaStream_t st, const char* what) {
     // (not const: nvcc 12.9's front end aborts on a const local initialised through this lambda)
-    int64_t Bc = largest_fit(B, wsb, [&](int64_t n) { return vjp_chunk_bytes((int)n); });
-    if (Bc < 1) { err = "workspace too small for a single walker (vjp)"; return 3; }
-    if (!fermi && !gnn)
-    DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
-    {  // the same warps-per-block rule as at the launch sites (at most 4 warps, at most 96 KiB)
-      const size_t pw = slater_bwd_smem_per_warp<T>(N);
-      int wpb = (int)((96 * 1024) / pw);
-      wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
-      if (pw * wpb > 227 * 1024) { err = "system too large for the shared-memory tiling of the reverse pass (N)"; return 2; }
-      DQ_CHECK(raise_dyn_smem(slater_bwd_kernel<T>, (int)(pw * wpb)));
-    }
+    int64_t Bc = largest_fit(B, wsb, [&](int64_t n) { return vjp_chunk_bytes((int)n, po != nullptr); });
+    if (Bc < 1) { err = std::string("workspace too small for a single walker (") + what + ")"; return 3; }
+    if (!gnn && cfg.kind != DQMC_FERMINET) DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
+    int wpb;
+    size_t smem;
+    int rc = slater_bwd_shape(wpb, smem);
+    if (rc) return rc;
+    DQ_CHECK(raise_dyn_smem(slater_bwd_kernel<T>, (int)smem));
     for (int b0 = 0; b0 < B; b0 += (int)Bc) {
       const int nb = (int)std::min<int64_t>(Bc, B - b0);
-      const T* rc_ = r + (size_t)b0 * 3 * N;
-      const T* Rc_ = R + (Rb ? (size_t)b0 * 3 * M : 0);
-      const Arena a(this, ws, wsb);
-      int rc = gnn ? vjp_chunk_paulinet(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, a, st)
-             : fermi ? vjp_chunk_ferminet(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, a, st)
-                     : vjp_chunk(rc_, Rc_, Rb, nb, (const T*)weights + b0, (T*)sign + b0, (T*)logp + b0, (T*)grad_params, a, st);
+      PosOut pc{nullptr, nullptr};
+      if (po) pc = {po->gr ? po->gr + (size_t)b0 * 3 * N : nullptr, po->gR ? po->gR + (size_t)b0 * 3 * M : nullptr};
+      rc = reverse_chunk(r + (size_t)b0 * 3 * N, R + (Rb ? (size_t)b0 * 3 * M : 0), Rb, nb, wts ? wts + b0 : nullptr, sign + b0,
+                         logp + b0, G, Arena(this, ws, wsb), st, po ? &pc : nullptr);
       if (rc) return rc;
       rc = check_guards();
       if (rc) return rc;
@@ -2472,8 +2430,17 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  int vjp_params(const void* r, const void* R, int Rb, int B, const void* weights, void* sign, void* logp,
+                 void* grad_params, void* ws, int64_t wsb, cudaStream_t st) override {
+    if (cfg.backflow_add) { err = "dqmc_wf_vjp_params: additive backflow branch has no reverse pass"; return 2; }
+    DQ_CHECK(cudaMemsetAsync(grad_params, 0, sizeof(T) * total, st));
+    if (B == 0) return 0;  // empty batch: zero gradient
+    return reverse_pass((const T*)r, (const T*)R, Rb, B, (const T*)weights, (T*)sign, (T*)logp, (T*)grad_params, nullptr, ws,
+                        wsb, st, "vjp");
+  }
+
   // d log|psi| / d r and / d R per walker: the parameter reverse pass in its position mode, chunked like vjp_params
-  int grad_positions(const void* r_, const void* R_, int Rb, int B, void* sign, void* logp, void* grad_r, void* grad_R, void* ws,
+  int grad_positions(const void* r, const void* R, int Rb, int B, void* sign, void* logp, void* grad_r, void* grad_R, void* ws,
                      int64_t wsb, cudaStream_t st) override {
     if (gnn) { err = "dqmc_wf_grad_positions: the conv-GNN kinds have no position reverse pass"; return 2; }
     if (cfg.backflow_add) { err = "dqmc_wf_grad_positions: additive backflow branch has no reverse pass"; return 2; }
@@ -2483,34 +2450,8 @@ struct Engine : EngineBase {
       return 2;
     }
     if (B == 0) return 0;
-    const T* r = (const T*)r_;
-    const T* R = (const T*)R_;
-    const bool fermi = cfg.kind == DQMC_FERMINET;
-    int64_t Bc = largest_fit(B, wsb, [&](int64_t n) { return vjp_chunk_bytes((int)n, true); });
-    if (Bc < 1) { err = "workspace too small for a single walker (grad_positions)"; return 3; }
-    if (!fermi) DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
-    {  // the warps-per-block rule of the launch sites
-      const size_t pw = slater_bwd_smem_per_warp<T>(N);
-      int wpb = (int)((96 * 1024) / pw);
-      wpb = wpb < 1 ? 1 : (wpb > 4 ? 4 : wpb);
-      if (pw * wpb > 227 * 1024) { err = "system too large for the shared-memory tiling of the reverse pass (N)"; return 2; }
-      DQ_CHECK(raise_dyn_smem(slater_bwd_kernel<T>, (int)(pw * wpb)));
-    }
-    for (int b0 = 0; b0 < B; b0 += (int)Bc) {
-      const int nb = (int)std::min<int64_t>(Bc, B - b0);
-      const T* rc_ = r + (size_t)b0 * 3 * N;
-      const T* Rc_ = R + (Rb ? (size_t)b0 * 3 * M : 0);
-      const PosOut po{grad_r ? (T*)grad_r + (size_t)b0 * 3 * N : nullptr, grad_R ? (T*)grad_R + (size_t)b0 * 3 * M : nullptr};
-      const Arena a(this, ws, wsb);
-      int rc = fermi ? vjp_chunk_ferminet(rc_, Rc_, Rb, nb, nullptr, (T*)sign + b0, (T*)logp + b0, nullptr, a, st, &po)
-                     : vjp_chunk(rc_, Rc_, Rb, nb, nullptr, (T*)sign + b0, (T*)logp + b0, nullptr, a, st, &po);
-      if (rc) return rc;
-      rc = check_guards();
-      if (rc) return rc;
-      if (dry) break;  // planning pass: the first chunk is the largest
-    }
-    DQ_CHECK(cudaGetLastError());
-    return 0;
+    const PosOut po{(T*)grad_r, (T*)grad_R};
+    return reverse_pass((const T*)r, (const T*)R, Rb, B, nullptr, (T*)sign, (T*)logp, nullptr, &po, ws, wsb, st, "grad_positions");
   }
 
   // closed-form force terms per walker (force_terms_kernel); all-electron Hamiltonians only
