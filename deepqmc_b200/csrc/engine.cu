@@ -37,6 +37,19 @@ struct ParamEntry {
 
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
+// largest d2 >= lo with w(d2) >= eps, for w falling on [lo, inf) with w(lo) >= eps: doubling, then bisection to adjacent doubles
+template <class W>
+static double last_above(W w, double lo, double eps) {
+  double hi = lo > 0.0 ? 2 * lo : 1.0;
+  while (w(hi) >= eps) { lo = hi; hi *= 2; }
+  for (;;) {
+    const double mid = lo + 0.5 * (hi - lo);
+    if (mid <= lo || mid >= hi) break;
+    (w(mid) >= eps ? lo : hi) = mid;
+  }
+  return lo;
+}
+
 // Squared cutoff radius of one non-local ECP nucleus, nl[l][alpha | beta][t] as the accumulator reads it: the largest d2 with
 // w(d2) = sum_l (2l+1) sum_t |beta_lt| exp(-alpha_lt d2) >= 2^-100.  A pair's term in V_nl is at most w(d2) max_q |psi ratio|
 // (sum_q |P_l(cos th_q)| <= 12), so the pairs beyond it are skipped (common.cuh ecp_pair_active).  w falls monotonically
@@ -57,14 +70,32 @@ static double ecp_cutoff_rc2(const T* nl, int L, int Tn, bool on) {
     return s;
   };
   if (w(0.0) < eps) return -inf;  // no pair is ever active
-  double lo = 0.0, hi = 1.0;
-  while (w(hi) >= eps) { lo = hi; hi *= 2; }
-  for (;;) {
-    const double mid = lo + 0.5 * (hi - lo);
-    if (mid <= lo || mid >= hi) break;
-    (w(mid) >= eps ? lo : hi) = mid;
-  }
-  return lo;
+  return last_above(w, 0.0, eps);
+}
+
+// Squared cutoff radius of the non-local ECP force (dqmc_ecp_force): a pair's share of grad_R V_nl is bounded by the weight w
+// above and by its radial derivative w'(rho) = sum_l (2l+1) sum_t 2 alpha_lt |beta_lt| rho exp(-alpha_lt rho^2) times the
+// ratios and their gradients, so the radius bounds both by 2^-100.  Each term of w' rises up to rho^2 = 1 / (2 alpha) and falls
+// beyond, so w' falls from the largest of those points on and the bisection starts there; a radius inside it keeps that whole
+// ball.  Never smaller than the energy's radius; +inf wherever that one is.
+template <class T>
+static double ecp_force_cutoff_rc2(const T* nl, int L, int Tn, bool on) {
+  const double rc2 = ecp_cutoff_rc2(nl, L, Tn, on), eps = std::ldexp(1.0, -100);
+  if (rc2 == std::numeric_limits<double>::infinity()) return rc2;
+  double peak = 0.0;
+  for (int l = 0; l < L; ++l)
+    for (int t = 0; t < Tn; ++t)
+      if ((double)nl[(l * 2 + 1) * Tn + t] != 0.0) peak = std::max(peak, 0.5 / (double)nl[(l * 2) * Tn + t]);
+  auto wd = [&](double d2) {
+    double s = 0.0;
+    for (int l = 0; l < L; ++l)
+      for (int t = 0; t < Tn; ++t) {
+        const double a = (double)nl[(l * 2) * Tn + t];
+        s += (2 * l + 1) * 2 * a * std::fabs((double)nl[(l * 2 + 1) * Tn + t]) * std::sqrt(d2) * std::exp(-a * d2);
+      }
+    return s;
+  };
+  return std::max(rc2, wd(peak) >= eps ? last_above(wd, peak, eps) : peak);
 }
 
 // The A/B switches (DESIGN §9), read from the environment once, when an engine is created.  A flag switch is on when its
@@ -172,6 +203,8 @@ struct EngineBase {
                              void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int force_terms(const void* r, const void* R, int Rb, int B, const void* grad_r, void* bare, void* zvq, void* Q,
                           cudaStream_t st) = 0;
+  virtual int ecp_force(const void* r, const void* R, int Rb, int B, uint64_t seed, const void* twist, void* bare, void* nl,
+                        void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int orbitals(const void* r, const void* R, int Rb, int B, void* out, void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int set_ph(int n_tab, int n_grid, double r_max, const double* tables, const int32_t* tab_of_nuc) = 0;
   virtual int debug_gemm(const char* wname, const char* bname, const void* A, const void* Res, void* C, int Mr, int S,
@@ -436,6 +469,7 @@ struct Engine : EngineBase {
   T* d_nl_params = nullptr;
   int* d_nl_nuc = nullptr;
   double* d_nl_rc2 = nullptr;  // [J] squared cutoff radius of each non-local nucleus slot (ecp_cutoff_rc2)
+  double* d_nl_rc2f = nullptr;  // [J] ... of the non-local force (ecp_force_cutoff_rc2)
   int J = 0;  // nuclei with a non-local channel
   // pseudo-Hamiltonian (reference ecp/pseudo_hamiltonian.py): tables r V_loc / r V_L2 per element on a uniform grid
   T* d_ph_tabs = nullptr;
@@ -613,10 +647,15 @@ struct Engine : EngineBase {
         DQ_CHECK(cudaMemcpy(d_nl_params, np.data(), sizeof(T) * np.size(), cudaMemcpyHostToDevice));
         DQ_CHECK(cudaMalloc((void**)&d_nl_nuc, sizeof(int) * J));
         DQ_CHECK(cudaMemcpy(d_nl_nuc, nuc.data(), sizeof(int) * J, cudaMemcpyHostToDevice));
-        std::vector<double> rc2(J);
-        for (int j = 0; j < J; ++j) rc2[j] = ecp_cutoff_rc2(np.data() + (size_t)nuc[j] * L * 2 * Tn, L, Tn, sw.ecp_cutoff);
+        std::vector<double> rc2(J), rc2f(J);
+        for (int j = 0; j < J; ++j) {
+          rc2[j] = ecp_cutoff_rc2(np.data() + (size_t)nuc[j] * L * 2 * Tn, L, Tn, sw.ecp_cutoff);
+          rc2f[j] = ecp_force_cutoff_rc2(np.data() + (size_t)nuc[j] * L * 2 * Tn, L, Tn, sw.ecp_cutoff);
+        }
         DQ_CHECK(cudaMalloc((void**)&d_nl_rc2, sizeof(double) * J));
         DQ_CHECK(cudaMemcpy(d_nl_rc2, rc2.data(), sizeof(double) * J, cudaMemcpyHostToDevice));
+        DQ_CHECK(cudaMalloc((void**)&d_nl_rc2f, sizeof(double) * J));
+        DQ_CHECK(cudaMemcpy(d_nl_rc2f, rc2f.data(), sizeof(double) * J, cudaMemcpyHostToDevice));
       }
     }
 #ifndef DQMC_EMU
@@ -705,6 +744,7 @@ struct Engine : EngineBase {
     if (d_nl_params) cudaFree(d_nl_params);
     if (d_nl_nuc) cudaFree(d_nl_nuc);
     if (d_nl_rc2) cudaFree(d_nl_rc2);
+    if (d_nl_rc2f) cudaFree(d_nl_rc2f);
     if (d_ph_tabs) cudaFree(d_ph_tabs);
     if (d_ph_nuc) cudaFree(d_ph_nuc);
 #if !defined(DQMC_NO_TCGEN05)
@@ -888,8 +928,9 @@ struct Engine : EngineBase {
   // offsets into it int[nb + 1] (the last entry is the group's pair count), the spin group the base walkers' sign[nb] and
   // log[nb].
   struct VirtGroup {
-    T *r, *sign, *logp, *env, *emb, *sign0 = nullptr, *logp0 = nullptr;
+    T *r, *sign, *logp, *env = nullptr, *emb = nullptr, *sign0 = nullptr, *logp0 = nullptr;
     int *pairs = nullptr, *offs = nullptr;
+    T *gr = nullptr, *gR = nullptr, *gR0 = nullptr;  // ECP force group: grad_r / grad_R of the virtual walkers, grad_R of the base walkers
   };
   VirtGroup carve_virt_group(Arena& a, int64_t nb, int64_t V) const {
     VirtGroup g;
@@ -904,6 +945,18 @@ struct Engine : EngineBase {
     g.pairs = a.take<int>(nb * J * N); g.offs = a.take<int>(nb + 1);
     return g;
   }
+  // ECP force group (dqmc_ecp_force): the virtual walkers are materialised (no base-walker tables) and the position reverse
+  // pass writes their sign, log, grad_r [V][N][3] and grad_R [V][M][3]; the base walkers' sign, log and grad_R [nb][M][3].
+  // Sized for every pair active, like carve_ecp_group.
+  VirtGroup carve_ecp_force_group(Arena& a, int64_t nb) const {
+    const int64_t V = nb * J * N * 12;
+    VirtGroup g;
+    g.r = a.take<T>(V * 3 * N); g.sign = a.take<T>(V); g.logp = a.take<T>(V);
+    g.gr = a.take<T>(V * 3 * N); g.gR = a.take<T>(V * 3 * M);
+    g.pairs = a.take<int>(nb * J * N); g.offs = a.take<int>(nb + 1);
+    g.sign0 = a.take<T>(nb); g.logp0 = a.take<T>(nb); g.gR0 = a.take<T>(nb * 3 * M);
+    return g;
+  }
   VirtGroup carve_spin_group(Arena& a, int64_t nb, int64_t P) const {  // P swapped pairs per walker
     VirtGroup g = carve_virt_group(a, nb, nb * P);
     g.sign0 = a.take<T>(nb); g.logp0 = a.take<T>(nb);
@@ -914,6 +967,23 @@ struct Engine : EngineBase {
   int64_t group_cap(int64_t vper) const { return std::max<int64_t>(1, kRowCap / ((int64_t)N * 3 * d) / vper); }
   // bytes of an ECP / spin group of nb walkers + a plain-forward chunk of Vc virtual walkers
   int64_t ecp_bytes(int64_t nb, int64_t Vc) const { return prefixed_bytes([&](Arena& a) { carve_ecp_group(a, nb); }, Vc, 1); }
+  // what one chunk of Vc virtual walkers carves after a group's prefix: a plain forward (ECP energy, spin), or a position
+  // reverse pass (ECP force); the chunk-size functions of virtual_groups
+  void fwd_chunk_carve(Arena& a, int64_t Vc) const { carve(a.top, (int)Vc, 1); }
+  void pos_chunk_carve(Arena& a, int64_t Vc) {
+    const PosOut none{nullptr, nullptr};
+    reverse_chunk(nullptr, nullptr, 0, (int)Vc, nullptr, nullptr, nullptr, nullptr, Arena(this, a.top), nullptr, &none);
+  }
+  // bytes of an ECP force group of nb walkers + a position reverse-pass chunk of Vc virtual walkers
+  int64_t ecp_force_bytes(int64_t nb, int64_t Vc) {
+    DryPass dp(this);
+    Arena a(this, plan_base());
+    carve_ecp_force_group(a, nb);
+    pos_chunk_carve(a, Vc);
+    return dp.bytes();
+  }
+  // the non-local ECP force needs grad_r and grad_R of log|psi| by the reverse pass (TransPsiformer: grad_r only)
+  bool has_nl_force() const { return has_pos_pass() && !trans; }
   int64_t spin_bytes(int64_t nb, int64_t P, int64_t Vc) const {
     return prefixed_bytes([&](Arena& a) { carve_spin_group(a, nb, P); }, Vc, 1);
   }
@@ -953,6 +1023,11 @@ struct Engine : EngineBase {
     if (mode == DQMC_MODE_GRAD_POS) return has_pos_pass() ? vjp_chunk_bytes(B, true) : 0;
     if (mode == DQMC_MODE_MCMC) return sweep_bytes(B, false, B);
     if (mode == DQMC_MODE_LANGEVIN) return sweep_bytes(B, true, B);
+    if (mode == DQMC_MODE_ECP_FORCE) {  // out_nl; out_bare alone needs no workspace
+      if (!J || !has_nl_force()) return 0;
+      const int64_t vper = (int64_t)J * N * 12, nb = std::min<int64_t>(B, group_cap(vper));
+      return ecp_force_bytes(nb, nb * vper);
+    }
     if (mode == DQMC_MODE_SPIN) {  // sized for the exact estimator, the larger of the two; no down electrons: no forwards
       const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
       if (!P) return 0;
@@ -977,6 +1052,7 @@ struct Engine : EngineBase {
       case DQMC_MODE_MCMC: return sweep_bytes(B, false, 1);
       case DQMC_MODE_LANGEVIN: return sweep_bytes(B, true, 1);
       case DQMC_MODE_LOCAL_ENERGY: return std::max<int64_t>(chunk_bytes(1, S), J > 0 ? ecp_bytes(1, 1) : 0);
+      case DQMC_MODE_ECP_FORCE: return J > 0 && has_nl_force() ? ecp_force_bytes(1, 1) : 0;
       case DQMC_MODE_SPIN: {
         const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
         return P ? spin_bytes(1, P, 1) : 0;
@@ -1010,6 +1086,9 @@ struct Engine : EngineBase {
       case DQMC_MODE_SPIN: rc = spin(nullptr, nullptr, 0, B, nullptr, nullptr, -1, nullptr, nullptr, ws, wsb, nullptr); break;
       case DQMC_MODE_GRAD_POS:
         rc = grad_positions(nullptr, nullptr, 0, B, nullptr, nullptr, nullptr, nullptr, ws, wsb, nullptr);
+        break;
+      case DQMC_MODE_ECP_FORCE:
+        rc = ecp_force(nullptr, nullptr, 0, B, 0, nullptr, nullptr, has_nl_force() ? ws : nullptr, ws, wsb, nullptr);
         break;
       default: err = "unknown mode"; rc = 2;
     }
@@ -2409,7 +2488,12 @@ struct Engine : EngineBase {
     // (not const: nvcc 12.9's front end aborts on a const local initialised through this lambda)
     int64_t Bc = largest_fit(B, wsb, [&](int64_t n) { return vjp_chunk_bytes((int)n, po != nullptr); });
     if (Bc < 1) { err = std::string("workspace too small for a single walker (") + what + ")"; return 3; }
-    if (!gnn && cfg.kind != DQMC_FERMINET) DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
+    if (!gnn && cfg.kind != DQMC_FERMINET) {
+      DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
+      // the chunk's forward runs the generic attention with one slot, which fp32 engines on the specialised kernels never
+      // opted in at creation (benzene, N = 30, dh = 64: 69 KB)
+      DQ_CHECK(raise_dyn_smem(attn_fl_kernel<T>, (int)attn_smem_bytes<T>(N, dh, 1, Mn)));
+    }
     int wpb;
     size_t smem;
     int rc = slater_bwd_shape(wpb, smem);
@@ -2464,7 +2548,7 @@ struct Engine : EngineBase {
     if (zvq && !grad_r) { err = "dqmc_force_terms: out_zvq needs grad_r"; return 2; }
     if (B == 0) return 0;
     DQ_LAUNCH(force_terms_kernel<T>, dim3(B), dim3(32), 0, st, (const T*)r, (const T*)R, Rb, N, M, (const T*)d_zval,
-              (const T*)grad_r, (T*)bare, (T*)zvq, (T*)Q);
+              (const T*)grad_r, (T*)bare, (T*)zvq, (T*)Q, (const T*)nullptr, 0);
     DQ_CHECK(cudaGetLastError());
     return 0;
   }
@@ -2502,17 +2586,26 @@ struct Engine : EngineBase {
     return 0;
   }
 
-  // Virtual walkers (vper per base walker: ECP quadrature points, spin swaps) through the plain forward in groups of nb base
-  // walkers: the largest group whose prefix (carve_group) + one forward chunk of all its virtual walkers fits wsb, else one
-  // walker (run_batched chunks its virtual walkers).  Per group, setup() launches the kind's work before the forwards and sets
-  // V, the virtual walkers to run, and finish() reduces their results.  With `tables` (and slater_fwd2, N <= 32) the forwards
-  // take the unmoved electrons' envelopes and, with `emb_table`, embedding rows from tables of the base walkers.
-  template <class CarveGroup, class Setup, class Finish>
+  // Virtual walkers (vper per base walker: ECP quadrature points, spin swaps) through a per-group pass in groups of nb base
+  // walkers: the largest group whose prefix (carve_group) + one pass chunk of all its virtual walkers (chunk_carve, a dry carve
+  // after the prefix) fits wsb, else one walker (the pass chunks its virtual walkers).  Per group, setup() launches the kind's
+  // work before the pass and sets V, the virtual walkers to run, pass(g, V, rest) runs them in the workspace after the prefix
+  // (run_batched: plain forwards; reverse_pass: position gradients), and finish() reduces their results.  With `tables` (and
+  // slater_fwd2, N <= 32) the forwards take the unmoved electrons' envelopes and, with `emb_table`, embedding rows from tables
+  // of the base walkers.
+  template <class CarveGroup, class Setup, class Pass, class ChunkCarve, class Finish>
   int virtual_groups(const T* r, const T* R, int B, int64_t vper, int layout, bool tables, bool emb_table, void* ws,
-                     int64_t wsb, const char* too_small, CarveGroup carve_group, Setup setup, Finish finish, cudaStream_t st) {
-    auto bytes = [&](int64_t nb, int64_t Vc) { return prefixed_bytes([&](Arena& a) { carve_group(a, nb); }, Vc, 1); };
+                     int64_t wsb, const char* too_small, CarveGroup carve_group, Setup setup, Pass pass, ChunkCarve chunk_carve,
+                     Finish finish, cudaStream_t st) {
+    auto bytes = [&](int64_t nb, int64_t Vc) {
+      DryPass dp(this);
+      Arena a(this, plan_base());
+      carve_group(a, nb);
+      chunk_carve(a, Vc);
+      return dp.bytes();
+    };
     int64_t Be = largest_fit(std::min<int64_t>(B, group_cap(vper)), wsb, [&](int64_t nb) { return bytes(nb, nb * vper); });
-    if (Be < 1) Be = 1;  // one walker's virtual walkers do not fit at once: the plain-forward pass chunks them
+    if (Be < 1) Be = 1;  // one walker's virtual walkers do not fit at once: the pass chunks them
     if (bytes(Be, 1) > wsb) { err = too_small; return 3; }
     tables = tables && slater_fwd2_ok && N <= 32 && !dry;
     emb_table = tables && emb_table && embed_fwd_ok && can_trunk(1);
@@ -2534,7 +2627,7 @@ struct Engine : EngineBase {
           ecp_emb = g.emb;
         }
       }
-      if (V > 0) rc = run_batched(g.r, R, 0, (int)V, 1, g.sign, g.logp, nullptr, nullptr, nullptr, a.top, a.left(), st);
+      if (V > 0) rc = pass(g, V, a);
       ecp_env = nullptr; ecp_emb = nullptr; ecp_pairs = nullptr; virt_layout = kVirtEcp;
       if (rc) return rc;
       rc = finish(b0, nb, g);
@@ -2542,6 +2635,73 @@ struct Engine : EngineBase {
       if (rc) return rc;
       if (dry) break;  // planning pass: the first group is the largest
     }
+    return 0;
+  }
+
+  // the plain-forward pass of a virtual-walker group (ECP energy, spin), in the workspace after the group's prefix
+  int virt_forwards(const VirtGroup& g, const T* R, int64_t V, const Arena& rest, cudaStream_t st) {
+    return run_batched(g.r, R, 0, (int)V, 1, g.sign, g.logp, nullptr, nullptr, nullptr, rest.top, rest.left(), st);
+  }
+
+  // Hellmann-Feynman force terms with effective core potentials (reference force.py:252-301): bare = F_nuc(Z_eff) - grad_R V_loc
+  // (force_terms_kernel with the local ECP table), nl = -grad_R V_nl per walker.  The non-local part runs in groups of base
+  // walkers (virtual_groups): a position reverse pass of the base walkers (sign, log, grad_R), the active pairs inside the
+  // force's cutoff radius with their quadrature points (the energy pass's twists for the same seed / ecp_twist), a position
+  // reverse pass over those virtual walkers, and ecp_force_accumulate_kernel.
+  int ecp_force(const void* r_, const void* R_, int Rb, int B, uint64_t seed, const void* twist, void* bare, void* nl, void* ws,
+                int64_t wsb, cudaStream_t st) override {
+    const T* r = (const T*)r_;
+    const T* R = (const T*)R_;
+    if (d_ph_tabs) { err = "dqmc_ecp_force: pseudo-Hamiltonians are not supported"; return 2; }
+    if (nl && !has_nl_force()) {
+      err = "dqmc_ecp_force: the non-local force needs grad_r and grad_R of log|psi| by the reverse pass (Psiformer and FermiNet "
+            "with multiplicative backflow); out_nl must be null";
+      return 2;
+    }
+    if (nl && Rb) { err = "non-local ECP with per-walker nuclei is not supported"; return 2; }
+    if (B == 0) return 0;
+    if (bare)
+      DQ_LAUNCH(force_terms_kernel<T>, dim3(B), dim3(32), 0, st, r, R, Rb, N, M, (const T*)d_zval, (const T*)nullptr, (T*)bare,
+                (T*)nullptr, (T*)nullptr, (const T*)d_ecp_loc, cfg.ecp_loc_terms);
+    if (nl && !J && !dry) DQ_CHECK(cudaMemsetAsync(nl, 0, sizeof(T) * (size_t)B * M * 3, st));
+    if (nl && J) {
+      auto setup = [&](int b0, int nb, const VirtGroup& g, const Arena& rest, int64_t& V) {
+        const T* rb = r + (size_t)b0 * 3 * N;
+        const PosOut p0{nullptr, g.gR0};
+        int rc = reverse_pass(rb, R, 0, nb, nullptr, g.sign0, g.logp0, nullptr, &p0, rest.top, rest.left(), st, "ecp_force");
+        if (rc) return rc;
+        DQ_LAUNCH(ecp_pairs_kernel<T>, dim3(1), dim3(1024), 0, st, rb, R, 0, N, M, J, (const int*)d_nl_nuc,
+                  (const double*)d_nl_rc2f, nb, g.offs, g.pairs, g.offs + nb);
+        int n_act = nb * J * N;  // the planning pass sizes every buffer for all pairs
+        if (!dry) {
+          DQ_CHECK(cudaMemcpyAsync(&n_act, g.offs + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+          DQ_CHECK(cudaStreamSynchronize(st));
+          ecp_forwards += (int64_t)n_act * 12;
+        }
+        V = (int64_t)n_act * 12;
+        if (n_act > 0)
+          DQ_LAUNCH(ecp_points_kernel<T>, dim3(n_act), dim3(64), 0, st, rb, R, 0, N, M, J, (const int*)d_nl_nuc,
+                    twist ? (const T*)twist + (size_t)b0 * J * N : nullptr, seed, (uint64_t)b0, (const int*)g.pairs, g.r);
+        return 0;
+      };
+      auto pass = [&](const VirtGroup& g, int64_t V, const Arena& rest) {
+        const PosOut pv{g.gr, g.gR};
+        return reverse_pass(g.r, R, 0, (int)V, nullptr, g.sign, g.logp, nullptr, &pv, rest.top, rest.left(), st, "ecp_force");
+      };
+      auto finish = [&](int b0, int nb, const VirtGroup& g) {
+        DQ_LAUNCH(ecp_force_accumulate_kernel<T>, dim3((nb + 3) / 4), dim3(128), 0, st, r + (size_t)b0 * 3 * N, R, N, M, J,
+                  (const int*)d_nl_nuc, (const T*)d_nl_params, (const double*)d_nl_rc2f, (const int*)g.offs, cfg.ecp_nl_lmax_p1,
+                  cfg.ecp_nl_terms, twist ? (const T*)twist + (size_t)b0 * J * N : nullptr, seed, (uint64_t)b0,
+                  (const T*)g.sign0, (const T*)g.logp0, (const T*)g.gR0, (const T*)g.sign, (const T*)g.logp, (const T*)g.gr,
+                  (const T*)g.gR, nb, (T*)nl + (size_t)b0 * M * 3);
+        return 0;
+      };
+      int rc = virtual_groups(r, R, B, (int64_t)J * N * 12, kVirtEcp, false, false, ws, wsb,
+                              "workspace too small for the non-local ECP force", [&](Arena& a, int64_t nb) { return carve_ecp_force_group(a, nb); },
+                              setup, pass, [&](Arena& a, int64_t Vc) { pos_chunk_carve(a, Vc); }, finish, st);
+      if (rc) return rc;
+    }
+    DQ_CHECK(cudaGetLastError());
     return 0;
   }
 
@@ -2583,7 +2743,9 @@ struct Engine : EngineBase {
         return 0;
       };
       rc = virtual_groups(r, R, B, (int64_t)J * N * 12, kVirtEcp, sw.ecp_env_table, sw.ecp_emb_table, ws, wsb,
-                          "workspace too small for the non-local ECP pass", [&](Arena& a, int64_t nb) { return carve_ecp_group(a, nb); }, setup, finish, st);
+                          "workspace too small for the non-local ECP pass", [&](Arena& a, int64_t nb) { return carve_ecp_group(a, nb); }, setup,
+                          [&](const VirtGroup& g, int64_t V, const Arena& a) { return virt_forwards(g, R, V, a, st); },
+                          [&](Arena& a, int64_t Vc) { fwd_chunk_carve(a, Vc); }, finish, st);
       if (rc) return rc;
     }
     DQ_CHECK(cudaGetLastError());
@@ -2631,7 +2793,9 @@ struct Engine : EngineBase {
     // a swapped walker differs from its base walker in two electrons: the forwards take every other electron's envelopes and
     // embedding rows from tables of the base walkers
     int rc = virtual_groups(r, R, B, Pn, down_idx, cfg.kind == DQMC_PSIFORMER, true, ws, wsb, "workspace too small for the spin pass",
-                            [&](Arena& a, int64_t nb) { return carve_spin_group(a, nb, Pn); }, setup, finish, st);
+                            [&](Arena& a, int64_t nb) { return carve_spin_group(a, nb, Pn); }, setup,
+                            [&](const VirtGroup& g, int64_t V, const Arena& a) { return virt_forwards(g, R, V, a, st); },
+                            [&](Arena& a, int64_t Vc) { fwd_chunk_carve(a, Vc); }, finish, st);
     if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
     return 0;
@@ -2849,6 +3013,15 @@ int dqmc_force_terms(dqmc_handle h, const void* r, const void* R, int32_t R_batc
   if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
   if (n_walkers > 0 && (!r || !R)) { h->e->err = "dqmc_force_terms: null array"; return 2; }
   return h->e->force_terms(r, R, R_batched, n_walkers, grad_r, out_bare, out_zvq, out_Q, (cudaStream_t)stream);
+}
+int dqmc_ecp_force(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, uint64_t seed,
+                   const void* ecp_twist, void* out_bare, void* out_nl, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
+  if (n_walkers > 0 && (!r || !R)) { h->e->err = "dqmc_ecp_force: null array"; return 2; }
+  return h->e->ecp_force(r, R, R_batched, n_walkers, seed, ecp_twist, out_bare, out_nl, workspace, workspace_bytes,
+                         (cudaStream_t)stream);
 }
 int dqmc_set_pseudo_hamiltonian(dqmc_handle h, int32_t n_tab, int32_t n_grid, double r_max, const double* tables,
                                 const int32_t* tab_of_nuc) {

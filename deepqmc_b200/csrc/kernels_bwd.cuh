@@ -528,12 +528,14 @@ __global__ void pos_grad_reduce_kernel(const T* __restrict__ r, const T* __restr
 //   bare[m]   = F_nuc[m] + Z_m sum_i d_im / |d_im|^3          (-grad_R of the Coulomb attraction, plain norm)
 //   Q[m]      = Z_m sum_i d_im / |d_im|
 //   zvq[m]    = F_nuc[m] + Z_m sum_i (g_i / |d| - d (d . g_i) / |d|^3),  g_i = grad_{r_i} log|psi|
-// d_im = r_i - R_m.  Every output nullable.
+// d_im = r_i - R_m.  Every output nullable.  loc[M][3][2][Tm] (nullable; dqmc_ecp_force): bare also takes -grad_R of the
+// local ECP, sum_t beta_0 e^{-alpha_0 rho^2} / rho + beta_1 e^{-alpha_1 rho^2} + beta_2 rho e^{-alpha_2 rho^2} per electron
+// (gaussian_type_ecp.py:127-159): -grad_{R_m} = V'(rho) d_im / rho.
 // ------------------------------------------------------------------------------------------
 template <class T>
 __global__ void force_terms_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M,
                                    const T* __restrict__ Z, const T* __restrict__ grad_r, T* __restrict__ bare,
-                                   T* __restrict__ zvq, T* __restrict__ Qo) {
+                                   T* __restrict__ zvq, T* __restrict__ Qo, const T* __restrict__ loc, int Tm) {
   const int b = blockIdx.x;
   const T* rb = r + (size_t)b * N * 3;
   const T* Rb = R + (R_batched ? (size_t)b * M * 3 : 0);
@@ -548,7 +550,7 @@ __global__ void force_terms_kernel(const T* __restrict__ r, const T* __restrict_
       const T s = zm * Z[n] / (rho * rho * rho);
       for (int a = 0; a < 3; ++a) fn[a] += s * d[a];
     }
-    T fb[3] = {T(0), T(0), T(0)}, q[3] = {T(0), T(0), T(0)}, fz[3] = {T(0), T(0), T(0)};
+    T fb[3] = {T(0), T(0), T(0)}, q[3] = {T(0), T(0), T(0)}, fz[3] = {T(0), T(0), T(0)}, fl[3] = {T(0), T(0), T(0)};
     for (int i = 0; i < N; ++i) {
       const T d[3] = {rb[3 * i] - Rb[3 * m], rb[3 * i + 1] - Rb[3 * m + 1], rb[3 * i + 2] - Rb[3 * m + 2]};
       const T dist = m_sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), inv = T(1) / dist, inv3 = inv * inv * inv;
@@ -559,10 +561,21 @@ __global__ void force_terms_kernel(const T* __restrict__ r, const T* __restrict_
         q[a] += d[a] * inv;
         if (gb) fz[a] += gb[3 * i + a] * inv - d[a] * dg * inv3;
       }
+      if (loc) {
+        const T* lp = loc + (size_t)m * 6 * Tm;  // [r^-1, r^0, r^1][alpha, beta][t]
+        T dv = T(0);
+        for (int t = 0; t < Tm; ++t) {
+          const T a0 = lp[t], b0 = lp[Tm + t], a1 = lp[2 * Tm + t], b1 = lp[3 * Tm + t], a2 = lp[4 * Tm + t], b2 = lp[5 * Tm + t];
+          const T d2 = dist * dist;
+          dv += b0 * m_exp(-a0 * d2) * (-inv * inv - T(2) * a0) - T(2) * a1 * dist * b1 * m_exp(-a1 * d2) +
+                b2 * m_exp(-a2 * d2) * (T(1) - T(2) * a2 * d2);
+        }
+        for (int a = 0; a < 3; ++a) fl[a] += dv * inv * d[a];
+      }
     }
     const size_t o = ((size_t)b * M + m) * 3;
     for (int a = 0; a < 3; ++a) {
-      if (bare) bare[o + a] = fn[a] + zm * fb[a];
+      if (bare) bare[o + a] = loc ? fn[a] + zm * fb[a] + fl[a] : fn[a] + zm * fb[a];
       if (Qo) Qo[o + a] = zm * q[a];
       if (zvq) zvq[o + a] = fn[a] + zm * fz[a];
     }

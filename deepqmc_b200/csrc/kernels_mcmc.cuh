@@ -323,6 +323,17 @@ __device__ __forceinline__ void ico_vertex(int q, double& th, double& ph) {
   }
 }
 
+// The twist of pair (walker b of the group, nucleus slot j, electron i): injected phi[B][J][N] or Philox(seed) keyed by the
+// pair's global index (ecp_points_kernel and ecp_force_accumulate_kernel draw the same one).
+template <class T>
+__device__ __forceinline__ double ecp_pair_twist(const T* __restrict__ phi, uint64_t seed, uint64_t walker_offset, int b, int j,
+                                                 int i, int J, int N) {
+  if (phi) return (double)phi[((size_t)b * J + j) * N + i];
+  uint32_t w[4];
+  Philox::gen(seed ^ 0xD1B54A32D192ED03ull, (walker_offset + (uint64_t)b) * (uint64_t)(J * N) + (uint64_t)(j * N + i), 0, w);
+  return Philox::u01(w[0], w[1]) * (3.141592653589793 / 5);
+}
+
 template <class T>
 __global__ void ecp_points_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M,
                                   int J, const int* __restrict__ nl_nuc, const T* __restrict__ phi, uint64_t seed,
@@ -341,13 +352,7 @@ __global__ void ecp_points_kernel(const T* __restrict__ r, const T* __restrict__
     double cz = dz / radius;
     cz = cz > 1.0 ? 1.0 : (cz < -1.0 ? -1.0 : cz);
     double theta = ::acos(cz), ph0 = ::atan2(dy, dx);
-    double pr;
-    if (phi) pr = (double)phi[((size_t)b * J + j) * N + i];
-    else {
-      uint32_t w[4];
-      Philox::gen(seed ^ 0xD1B54A32D192ED03ull, (walker_offset + (uint64_t)b) * (uint64_t)(J * N) + (uint64_t)(j * N + i), 0, w);
-      pr = Philox::u01(w[0], w[1]) * (3.141592653589793 / 5);
-    }
+    const double pr = ecp_pair_twist(phi, seed, walker_offset, b, j, i, J, N);
     double th, ph;
     ico_vertex(q, th, ph);
     double ux = ::sin(th) * ::cos(ph), uy = ::sin(th) * ::sin(ph), uz = ::cos(th);
@@ -483,6 +488,103 @@ __global__ void ecp_accumulate_kernel(const T* __restrict__ r, const T* __restri
   if (lane == 0) {
     out_E[b] += (T)total;
     out_stats[3 * (size_t)Bstat + b] = (T)total;
+  }
+}
+
+// Non-local ECP force (reference: ecp/gaussian_type_ecp.py:257-328, ecp_force_utils.py): out[b][I] = -grad_{R_I} of
+// nucleus I's share of V_nl, sum_i sum_l (2l+1)/12 v_l(rho) sum_q P_l(cos th_q) psi(r_q(R), R) / psi(r, R), rho = |r_i - R_I|;
+// rows of nuclei without a non-local term are zero.  With d = r_i - R_I, r_q = R_I + f_q(d), f_q = rho Rz(phi) Ry(theta) w_q,
+// w_q = Rz(twist) u_q (ecp_points_kernel):
+//   d ratio_q / d R_I = ratio_q [g_R(r_q)[I] + (1 - df_q/dd)^T g_r(r_q)[i] - g_R(r)[I]],
+//   df_q/dd = (f_q / rho) d^T / rho + rho Rz(phi) Ry'(theta) w_q (dtheta/dd)^T + rho Rz'(phi) Ry(theta) w_q (dphi/dd)^T,
+//   dtheta/dd = (d_z d / rho^2 - e_z) / s, dphi/dd = (-d_y, d_x, 0) / s^2, s = sqrt(d_x^2 + d_y^2),
+//   d v_l / d R_I = 2 d sum_t alpha beta exp(-alpha rho^2).
+// g_r, g_R = grad_r, grad_R log|psi| from the position reverse pass: of the base walkers (gR0[nb][M][3], sign0, log0) and of
+// the virtual walkers of the active pairs (gr_v[V][N][3], gR_v[V][M][3], sign_v, log_v, v = 12 a + q for the pair's entry a in
+// the group's list, ecp_pairs_kernel with the force's cutoff rc2).  One WARP per walker: nucleus slot by nucleus slot, lanes
+// stride over the electrons, everything in double, a fixed shuffle tree per slot -- no atomics.
+template <class T>
+__global__ void ecp_force_accumulate_kernel(const T* __restrict__ r, const T* __restrict__ R, int N, int M, int J,
+                                            const int* __restrict__ nl_nuc, const T* __restrict__ nl_params,
+                                            const double* __restrict__ rc2, const int* __restrict__ offs, int L, int Tm,
+                                            const T* __restrict__ phi, uint64_t seed, uint64_t walker_offset,
+                                            const T* __restrict__ sign0, const T* __restrict__ log0, const T* __restrict__ gR0,
+                                            const T* __restrict__ sign_v, const T* __restrict__ log_v,
+                                            const T* __restrict__ gr_v, const T* __restrict__ gR_v, int B, T* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;  // warp-uniform
+  const T* rb = r + (size_t)b * 3 * N;
+  T* ob = out + (size_t)b * M * 3;
+  for (int k = lane; k < 3 * M; k += 32) ob[k] = T(0);
+  __syncwarp();
+  const double l0 = (double)log0[b], s0 = (double)sign0[b];
+  int slot = offs[b];
+  for (int j = 0; j < J; ++j) {
+    const int I = nl_nuc[j];
+    const T* nl = nl_params + (size_t)I * L * 2 * Tm;
+    const double g0[3] = {(double)gR0[((size_t)b * M + I) * 3], (double)gR0[((size_t)b * M + I) * 3 + 1],
+                          (double)gR0[((size_t)b * M + I) * 3 + 2]};
+    double acc[3] = {0.0, 0.0, 0.0};
+    for (int i0 = 0; i0 < N; i0 += 32) {  // warp-uniform trip count: every lane takes part in the ballot
+      const int i = i0 + lane;
+      double d2 = 0.0;
+      const bool act = i < N && ecp_pair_active(rb + 3 * i, R + 3 * I, rc2[j], d2);
+      const unsigned m = __ballot_sync(0xffffffffu, act);
+      const int a = slot + __popc(m & ((1u << lane) - 1u));
+      slot += __popc(m);
+      if (!act) continue;
+      const double d[3] = {(double)rb[3 * i] - (double)R[3 * I], (double)rb[3 * i + 1] - (double)R[3 * I + 1],
+                           (double)rb[3 * i + 2] - (double)R[3 * I + 2]};
+      const double rho = ::sqrt(d2), s2 = d[0] * d[0] + d[1] * d[1], s = ::sqrt(s2);
+      double cz = d[2] / rho;
+      cz = cz > 1.0 ? 1.0 : (cz < -1.0 ? -1.0 : cz);
+      const double th = ::acos(cz), ph = ::atan2(d[1], d[0]), tw = ecp_pair_twist(phi, seed, walker_offset, b, j, i, J, N);
+      const double ct = ::cos(th), st = ::sin(th), cp = ::cos(ph), sp = ::sin(ph), cw = ::cos(tw), sw = ::sin(tw);
+      const double dth[3] = {(d[2] * d[0] / d2) / s, (d[2] * d[1] / d2) / s, (d[2] * d[2] / d2 - 1.0) / s};
+      const double dph[3] = {-d[1] / s2, d[0] / s2, 0.0};
+      double integ[4] = {0, 0, 0, 0}, dinteg[4][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
+      for (int q = 0; q < 12; ++q) {
+        const size_t v = (size_t)a * 12 + q;
+        const double ratio = ::exp((double)log_v[v] - l0) * (double)sign_v[v] * s0;
+        double qt, qp;
+        ico_vertex(q, qt, qp);
+        const double ux = ::sin(qt) * ::cos(qp), uy = ::sin(qt) * ::sin(qp), uz = ::cos(qt);
+        const double wx = cw * ux - sw * uy, wy = sw * ux + cw * uy, wz = uz;               // Rz(twist) u
+        const double A[3] = {ct * wx + st * wz, wy, -st * wx + ct * wz};                     // Ry(theta) w
+        const double Ad[3] = {-st * wx + ct * wz, 0.0, -ct * wx - st * wz};                  // Ry'(theta) w
+        const double f[3] = {rho * (cp * A[0] - sp * A[1]), rho * (sp * A[0] + cp * A[1]), rho * A[2]};
+        const double t1[3] = {rho * (cp * Ad[0] - sp * Ad[1]), rho * (sp * Ad[0] + cp * Ad[1]), rho * Ad[2]};
+        const double t2[3] = {rho * (-sp * A[0] - cp * A[1]), rho * (cp * A[0] - sp * A[1]), 0.0};
+        const T* gr = gr_v + (v * N + i) * 3;
+        const T* gR = gR_v + (v * M + I) * 3;
+        const double g[3] = {(double)gr[0], (double)gr[1], (double)gr[2]};
+        const double fg = (f[0] * g[0] + f[1] * g[1] + f[2] * g[2]) / d2, t1g = t1[0] * g[0] + t1[1] * g[1] + t1[2] * g[2],
+                     t2g = t2[0] * g[0] + t2[1] * g[1] + t2[2] * g[2];
+        double dr[3];
+        for (int c = 0; c < 3; ++c)  // ratio_q [g_R(r_q) + g_r(r_q) - J^T g_r(r_q) - g_R(r)]
+          dr[c] = ratio * ((double)gR[c] + g[c] - (d[c] * fg + dth[c] * t1g + dph[c] * t2g) - g0[c]);
+        const double x = ::cos(qt);
+        const double pl[4] = {1.0, x, 0.5 * (3 * x * x - 1), 0.5 * (5 * x * x * x - 3 * x)};
+        for (int l = 0; l < L; ++l) {
+          integ[l] += ratio * pl[l];
+          for (int c = 0; c < 3; ++c) dinteg[l][c] += dr[c] * pl[l];
+        }
+      }
+      for (int l = 0; l < L; ++l) {
+        double vl = 0.0, dvl = 0.0;
+        for (int t = 0; t < Tm; ++t) {
+          const double al = (double)nl[(l * 2 + 0) * Tm + t], be = (double)nl[(l * 2 + 1) * Tm + t], e = ::exp(-al * d2);
+          vl += be * e;
+          dvl += al * be * e;
+        }
+        const double c = (2 * l + 1) / 12.0;
+        for (int k = 0; k < 3; ++k) acc[k] += c * (2 * d[k] * dvl * integ[l] + vl * dinteg[l][k]);
+      }
+    }
+    for (int k = 0; k < 3; ++k) acc[k] = warp_sum(acc[k]);
+    if (lane == 0)
+      for (int k = 0; k < 3; ++k) ob[(size_t)I * 3 + k] = (T)(-acc[k]);
   }
 }
 

@@ -14,7 +14,7 @@ from . import _lib
 from . import params as PN
 from .spec import AnsatzSpec
 
-MODE_FORWARD, MODE_LOCAL_ENERGY, MODE_VJP, MODE_MCMC, MODE_LANGEVIN, MODE_SPIN, MODE_GRAD_POS = 0, 1, 2, 3, 4, 5, 6
+MODE_FORWARD, MODE_LOCAL_ENERGY, MODE_VJP, MODE_MCMC, MODE_LANGEVIN, MODE_SPIN, MODE_GRAD_POS, MODE_ECP_FORCE = 0, 1, 2, 3, 4, 5, 6, 7
 _TORCH_DTYPE = {0: torch.float64, 1: torch.float32}
 
 
@@ -633,6 +633,26 @@ class Engine:
                                        self._stream())
         self._check(rc, 'dqmc_force_terms')
         return bare, zvq, Q
+
+    def ecp_force(self, r, R, seed=0, ecp_twist=None, want_nl=True, max_ws_bytes=None):
+        """-> (bare[B, M, 3], nl[B, M, 3] or None): the Hellmann-Feynman force terms with an effective core potential
+        (dqmc_ecp_force): bare = F_nuc(Z_eff) - grad_R V_loc, nl = -grad_R V_nl (reference force.py:295-297,
+        gaussian_type_ecp.py:257-328), nl in the nucleus' own row.  ``seed`` / ``ecp_twist`` [B, J, N] choose the quadrature
+        twists as in ``local_energy``.  nl: Psiformer and FermiNet with multiplicative backflow, unbatched R."""
+        r = self._prep(r)
+        B = r.shape[0]
+        R, Rb = self._R(R, B)
+        mk = lambda *s: torch.empty(*s, dtype=self.dtype, device=self.device)
+        M = self.spec.n_nuc
+        bare = mk(B, M, 3)
+        nl = mk(B, M, 3) if want_nl else None
+        tw = self._prep(ecp_twist) if ecp_twist is not None else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        ws = self.workspace(B, MODE_ECP_FORCE, max_ws_bytes) if want_nl else None
+        rc = self.lib.dqmc_ecp_force(self.h, r.data_ptr(), R.data_ptr(), Rb, B, seed, ptr(tw), bare.data_ptr(), ptr(nl), ptr(ws),
+                                     ws.numel() if ws is not None else 0, self._stream())
+        self._check(rc, 'dqmc_ecp_force')
+        return bare, nl
 
     def mcmc_sweep(self, state, R, n_sub, target_acceptance=0.57, max_age=None, seed=0, step0=0, walker_offset=0,
                    noise_normal=None, noise_uniform=None, max_ws_bytes=None, exchange_probability=0.0, exchange_flags=None,

@@ -1,5 +1,5 @@
 """Hellmann-Feynman force estimators on top of the engine's position gradients (``dqmc_wf_grad_positions``) and closed-form
-force terms (``dqmc_force_terms``).
+force terms (``dqmc_force_terms``, and ``dqmc_ecp_force`` with an effective core potential).
 
 Mirror of the reference's ``force.py`` (Cartesian nuclear coordinates) with its names and argument order.  Every estimator
 factory takes ``(hamil, ansatz.apply)`` and returns a batched callable: ``phys_conf`` carries r [B, N, 3] and R [M, 3] or
@@ -7,8 +7,15 @@ factory takes ``(hamil, ansatz.apply)`` and returns a batched callable: ``phys_c
 
 grad_r log|psi| comes from the reverse pass where the ansatz kind has one and from the forward-Laplacian pass of
 ``dqmc_local_energy`` otherwise, so the ZVQ family runs on every kind; grad_R log|psi| (the zero-bias estimators) needs the
-reverse pass into the nuclear coordinates: Psiformer and FermiNet.  Not built: AC-ZV / AC-ZVZB (the local energy of the
-nuclear-JVP wave function) and the ECP part of the bare force (``grad_nonloc_potential``); see DESIGN.md.
+reverse pass into the nuclear coordinates: Psiformer and FermiNet.
+
+With a Gaussian-type ECP the bare force (and so AC-ZB and the antithetic wrapper around bare) adds -grad_R of the local ECP
+and the non-local part -grad_nonloc_potential (``dqmc_ecp_force``; Psiformer and FermiNet).  As in the reference, every
+(nucleus, electron) pair of a walker shares one quadrature twist, drawn per walker from ``rng`` (the energy pass draws one per
+pair); unlike the reference, nucleus I's non-local force lands in row I, not in row j (its index among the non-local nuclei):
+the two agree when the ECP nuclei come first, as in every molecule the reference ships.  The ZVQ family refuses ECP engines,
+which the reference documents as incompatible.  Not built: AC-ZV / AC-ZVZB (the local energy of the nuclear-JVP wave
+function); see DESIGN.md.
 """
 from __future__ import annotations
 
@@ -122,13 +129,38 @@ def make_grad_nuc_log_wf(hamil, wf):
     return grad_nuc_log_wf
 
 
+def _has_ecp(hamil):
+    return getattr(hamil, 'loc_params', None) is not None
+
+
+def ecp_force_twist(hamil, rng, B, N):
+    """-> [B, J, N] quadrature twists of the ECP force: one per walker, uniform in [0, pi/5) from a generator seeded with
+    ``rng`` as ``evaluate_finite_difference_force`` seeds its twists, shared by every (nucleus, electron) pair of the walker
+    (reference ecp_force_utils.py:55-57 passes the un-folded rng to every pair); None without non-local nuclei."""
+    n_nl = 0 if hamil.nl_params is None else len(hamil.pot.nuc_with_nl_pot)
+    if not n_nl:
+        return None
+    g = torch.Generator(device='cpu').manual_seed(0 if rng is None else int(rng))
+    return (torch.rand(B, generator=g, dtype=torch.float64) * (torch.pi / 5))[:, None, None].expand(B, n_nl, N)
+
+
+def _bare(hamil, eng, rng, r, R):
+    """F_nuc - grad_R V_loc (- grad_R V_nl with an ECP) [B, M, 3]."""
+    if not _has_ecp(hamil):
+        return eng.force_terms(r, R)[0]
+    tw = ecp_force_twist(hamil, rng, r.shape[0], r.shape[1])
+    bare, nl = eng.ecp_force(r, R, seed=0 if rng is None else int(rng), ecp_twist=tw, want_nl=tw is not None)
+    return bare if nl is None else bare + nl
+
+
 def evaluate_hf_force_bare(hamil, wf):
-    """-> f(rng, params, phys_conf) -> F_nuc + Z_m sum_i d_im / |d_im|^3 [B, M, 3] (reference force.py:250-301, all-electron;
-    the ECP part is not built: engines with an ECP refuse)."""
+    """-> f(rng, params, phys_conf) -> F_nuc - grad_R V_loc - grad_R V_nl [B, M, 3] (reference force.py:250-301): all-electron
+    F_nuc + Z_m sum_i d_im / |d_im|^3; with a Gaussian-type ECP the local ECP terms and -grad_nonloc_potential added
+    (dqmc_ecp_force, twists drawn from ``rng``: see the module docstring)."""
 
     def evaluate_hf_force_bare_(rng, params, phys_conf: PhysicalConfiguration):
         r, R, single = _batched(phys_conf)
-        return _unbatch(_engine(hamil, wf, params).force_terms(r, R)[0], single)
+        return _unbatch(_bare(hamil, _engine(hamil, wf, params), rng, r, R), single)
 
     return evaluate_hf_force_bare_
 
@@ -167,13 +199,13 @@ def evaluate_hf_force_ac_zvzbq(hamil, wf):
 
 def evaluate_hf_force_ac_zb(hamil, wf):
     """-> f(rng, params, phys_conf, e_loc, energy) -> bare - 2 (E_loc - energy) grad_R log|psi| [B, M, 3]
-    (reference force.py:412-447)."""
+    (reference force.py:412-447; with an ECP, bare as in ``evaluate_hf_force_bare``)."""
 
     def evaluate_hf_force_ac_zb_(rng, params, phys_conf: PhysicalConfiguration, e_loc, energy):
         r, R, single = _batched(phys_conf)
         eng = _engine(hamil, wf, params)
         gR = _grad_R(eng, r, R)
-        f = eng.force_terms(r, R)[0] + _zb_factor(e_loc, energy, gR).reshape(-1, 1, 1) * gR
+        f = _bare(hamil, eng, rng, r, R) + _zb_factor(e_loc, energy, gR).reshape(-1, 1, 1) * gR
         return _unbatch(f, single)
 
     return evaluate_hf_force_ac_zb_

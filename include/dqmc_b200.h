@@ -31,7 +31,7 @@ enum { DQMC_PSIFORMER = 0, DQMC_FERMINET = 1, DQMC_TRANSPSIFORMER = 2, DQMC_PAUL
 enum { DQMC_F64 = 0, DQMC_F32 = 1 };
 enum { DQMC_GEMM_SIMT = 0, DQMC_GEMM_TCGEN05 = 1 };
 enum { DQMC_MODE_FORWARD = 0, DQMC_MODE_LOCAL_ENERGY = 1, DQMC_MODE_VJP = 2, DQMC_MODE_MCMC = 3, DQMC_MODE_LANGEVIN = 4,
-       DQMC_MODE_SPIN = 5, DQMC_MODE_GRAD_POS = 6 };
+       DQMC_MODE_SPIN = 5, DQMC_MODE_GRAD_POS = 6, DQMC_MODE_ECP_FORCE = 7 };
 
 /* Ansatz + Hamiltonian constants that fix the kernel shapes.
  * reference: src/deepqmc/conf/ansatz/psiformer.yaml, ferminet.yaml (SURVEY.md 8(a0));
@@ -234,6 +234,28 @@ int dqmc_wf_grad_positions(dqmc_handle h, const void* r, const void* R, int32_t 
 int dqmc_force_terms(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers,
                      const void* grad_r, void* out_bare, void* out_zvq, void* out_Q, void* stream);
 
+/* Hellmann-Feynman force terms with effective core potentials, per walker [B][M][3] (device, both outputs nullable):
+ *   out_bare = F_nuc(Z_eff) - grad_R V_loc: dqmc_force_terms' out_bare with the local ECP's Gaussian terms added (equal to it
+ *              on an all-electron engine); any ansatz kind.
+ *   out_nl   = -grad_R V_nl (the reference's -grad_nonloc_potential): for every nucleus I with a non-local term and electron i,
+ *              d/dR_I of v_l(|r_i - R_I|) (2l+1)/12 sum_q P_l(cos th_q) psi(r_q(R), R) / psi(r, R), where the quadrature point
+ *              r_q moves with R_I and psi depends on R_I explicitly, in the numerator and the denominator; rows of nuclei
+ *              without a non-local term are zero.  Written into row I, the nucleus' own row (the reference writes row j, the
+ *              nucleus' index among the non-local nuclei; the two agree when those nuclei come first).  Needs grad_r and
+ *              grad_R of log|psi| by the reverse pass: Psiformer and FermiNet with multiplicative backflow; the other kinds,
+ *              R_batched = 1 and a non-null out_nl return status 2.
+ * Quadrature twists: seed / ecp_twist [B][J][N] as in dqmc_local_energy, so the same seed gives the energy pass's
+ * quadrature points.  Pairs beyond the force's cutoff radius (the weight sum_l (2l+1) sum_t |beta| exp(-alpha rho^2) and its
+ * radial derivative below 2^-100; DQMC_ECP_CUTOFF=0: none) add nothing and run no reverse pass; their quadrature walkers
+ * count in dqmc_ecp_forward_count.  Every sum runs in a fixed order without atomics: a repeated call is bitwise identical.
+ * Pseudo-Hamiltonians: status 2.  n_walkers = 0 is a no-op.
+ * Workspace: dqmc_workspace_bytes(h, B, DQMC_MODE_ECP_FORCE) (0 where out_nl has nothing to compute; walkers are grouped
+ * and the reverse passes chunked to fit).
+ * replaces: force.py:252-301 evaluate_hf_force_bare with a GaussianTypeECP (local_potential gradient,
+ *           ecp/gaussian_type_ecp.py:257-328 grad_nonloc_potential, ecp/ecp_force_utils.py). */
+int dqmc_ecp_force(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, uint64_t seed,
+                   const void* ecp_twist, void* out_bare, void* out_nl, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* Switch the handle's Hamiltonian to a pseudo-Hamiltonian (fully local replacement of the semi-local ECP):
  * tables[n_tab][2][n_grid] (host, fp64) = r V_loc(r) and r V_L2(r) per tabulated element on the uniform grid
  * [0, r_max]; tab_of_nuc[n_nuc] = table index of each nucleus or -1.  z_valence of the config carries the
@@ -264,7 +286,7 @@ int dqmc_debug_plan(dqmc_handle h, int32_t n_walkers, int32_t mode, int64_t work
 /* Number of kernels this handle has launched so far (bench.py's gpu_launches claim). */
 int64_t dqmc_launch_count(dqmc_handle h);
 /* Number of non-local ECP quadrature forwards (virtual walkers, 12 per active electron-nucleus pair) this handle has run so far
-   in local-energy calls: pairs beyond the nucleus' cutoff radius run none (DQMC_ECP_CUTOFF=0: every pair runs). */
+   in local-energy and dqmc_ecp_force calls: pairs beyond the nucleus' cutoff radius run none (DQMC_ECP_CUTOFF=0: every pair runs). */
 int64_t dqmc_ecp_forward_count(dqmc_handle h);
 
 /* Self-test hook: run ONE dense-layer row GEMM  C = (Res) + A @ W[weight] (+ bias on value rows)
