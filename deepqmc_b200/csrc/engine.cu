@@ -722,7 +722,12 @@ struct Engine : EngineBase {
       DQ_CHECK(raise_dyn_smem(tc::gemm3x_kernel<true>, tc::SmemLayout::total()));
       DQ_CHECK(raise_dyn_smem(tc::mlp_block_f16_kernel<128>, tc::MlpSmem::total()));
       DQ_CHECK(raise_dyn_smem(tc::mlp_block_f16_kernel<256>, tc::MlpSmem::total()));
-      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel, tc::TrSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<1>, tc::TrSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<2>, tc::TrSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<4>, tc::TrSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<8>, tc::TrSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<16>, tc::TrSmem::total()));
+      DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<32>, tc::TrSmem::total()));
       if (psif && !trans && d == 256 && H == 4 && N <= 32 && cfg.n_layers <= tc::kTrMaxLayers) {
         DQ_CHECK(cudaMalloc((void**)&d_trunk_maps, sizeof(CUtensorMap) * 8 * cfg.n_layers));
         DQ_CHECK(cudaMalloc((void**)&d_trunk_scratch, (size_t)n_sms * tc::kTrScratchPerCta));
@@ -1258,7 +1263,7 @@ struct Engine : EngineBase {
       p.n_up = cfg.n_up; p.vlayout = virt_layout; p.pairs = ecp_pairs; p.wspin = P("emb.w") + (size_t)(4 * M) * d;  // the +-1 spin feature's row
       int np2 = 1;
       while (np2 < N) np2 *= 2;  // walker slot of the tile: electrons rounded up to a power of two (<= 32)
-      p.walkers = rows / N; p.N = N; p.NP = np2; p.L = cfg.n_layers; p.a_scale = kActScale;
+      p.walkers = rows / N; p.N = N; p.L = cfg.n_layers; p.a_scale = kActScale;
       p.attn_scale = (float)(1.0 / std::sqrt((double)dh)); p.err_flag = nullptr; p.phase = d_trunk_phase;
       for (int l = 0; l < cfg.n_layers; ++l) {
         const std::string pfx = "L" + std::to_string(l) + ".";
@@ -1272,7 +1277,15 @@ struct Engine : EngineBase {
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       if (prof) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
 #endif
-      DQ_LAUNCH(tc::trunk_f16_kernel, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p);
+      switch (np2) {  // one kernel instance per walker slot
+        case 1: DQ_LAUNCH(tc::trunk_f16_kernel<1>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p); break;
+        case 2: DQ_LAUNCH(tc::trunk_f16_kernel<2>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p); break;
+        case 4: DQ_LAUNCH(tc::trunk_f16_kernel<4>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p); break;
+        case 8: DQ_LAUNCH(tc::trunk_f16_kernel<8>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p); break;
+        case 16: DQ_LAUNCH(tc::trunk_f16_kernel<16>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p); break;
+        case 32: DQ_LAUNCH(tc::trunk_f16_kernel<32>, dim3(grid), dim3(tc::kTrThreads), tc::TrSmem::total(), st, p); break;
+        default: err = "internal: fused trunk walker slot above 32"; return 5;
+      }
 #ifndef DQMC_EMU
       if (prof) {
         cudaEventRecord(e1, st);

@@ -71,7 +71,9 @@ __device__ __forceinline__ void start_pingpong(unsigned char* smem) {
 // Phase timers of the whole-trunk kernel (TrunkParams::phase): clock64() cycles summed over the consumer warpgroups of all
 // CTAs, in this order; kPhWait (waiting for weight slots to land) and kPhTurn (waiting for the other warpgroup to hand over
 // the MMA token) are not part of the mainloop phases.
-enum Phase { kPhLoad, kPhQkv, kPhQkvEpi, kPhAttn, kPhWo, kPhW1, kPhW2, kPhMlpEpi, kPhWait, kPhTurn, kPhPairs, kPhases };
+enum Phase {
+  kPhLoad, kPhQkv, kPhQkvEpi, kPhAttn, kPhWo, kPhWoEpi, kPhW1, kPhW1Epi, kPhW2, kPhW2Epi, kPhWait, kPhTurn, kPhPairs, kPhases
+};
 static_assert(kPhases <= 16, "MlpSmem::phases() holds 16 counters per warpgroup");
 struct PhaseClock {
   unsigned long long* acc;  // this warpgroup's shared-memory counters on its timing thread, nullptr: not timing
@@ -247,85 +249,102 @@ struct Frag {
   }
 };
 
+// The epilogues of the MLP block's three GEMMs (mlp3), per accumulator pair (acc0, acc1) = columns c, c + 1 of tile row `row`
+// with its row r of the residual input (A for kEpiW2, X for kEpiWo):
+//   kEpiWo: A = X + acc us -> gout (parked A), operand
+//   kEpiW1: M1 = tanh(acc us + b) -> operand
+//   kEpiW2: X' = A + tanh(acc us + b) -> gout (X'), operand if `operand`
+enum MlpEpi { kEpiWo, kEpiW1, kEpiW2 };
+template <int E>
+__device__ __forceinline__ void mlp_epi_pair(unsigned char* smem, int row, int c, float acc0, float acc1, float2 r, float us,
+                                             const float* bias, float a_scale, float* gout, bool operand) {
+  float v0, v1;
+  if constexpr (E == kEpiWo) {
+    v0 = r.x + acc0 * us;
+    v1 = r.y + acc1 * us;
+  } else {
+    const float2 b = make_float2(__ldg(bias + c), __ldg(bias + c + 1));  // (the parameter table gives no 8-byte alignment)
+    if constexpr (E == kEpiW1) {
+      v0 = mlp_tanh(acc0 * us + b.x);
+      v1 = mlp_tanh(acc1 * us + b.y);
+    } else {
+      v0 = r.x + mlp_tanh(acc0 * us + b.x);
+      v1 = r.y + mlp_tanh(acc1 * us + b.y);
+    }
+  }
+  if (E != kEpiW1 && gout) *(float2*)(gout + c) = make_float2(v0, v1);
+  if (operand) store_operand_pair(smem, row, c, v0 * a_scale, v1 * a_scale);
+}
+
+// Epilogue E of the MLP block on this warpgroup's accumulator: per fragment row h (tile rows fr, fr + 8) the residual input
+// rin[h] (nullptr: zero for kEpiWo, row skipped for kEpiW2) and the row output gout[h] (nullptr: not stored).  A rolled loop
+// over column quarters keeps the code to one quarter: the quarter's values are always acc[0 .. D / 8 - 1] (static register
+// indices), the next quarter's move down after each.  This clobbers acc, dead after the epilogue.
+template <int D, int E>
+__device__ __forceinline__ void mlp_epilogue(float (&acc)[D / 2], unsigned char* smem, float us, const float* bias,
+                                             float a_scale, const float* const (&rin)[2], float* const (&gout)[2], bool operand) {
+  const Frag f;
+  constexpr int QJ = D / 32;  // fragment columns of 8 per quarter
+  // Row loads are issued in batches of kJ fragment columns ahead of the stores: rin / gout may alias, so the compiler would
+  // otherwise wait for every load behind the previous store.
+  constexpr int kJ = 4;
+#pragma unroll 1
+  for (int q = 0; q < 4; ++q) {
+#pragma unroll
+    for (int jb = 0; jb < QJ; jb += kJ) {
+      float2 r[kJ][2];
+#pragma unroll
+      for (int j = 0; j < kJ; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          r[j][h] = E != kEpiW1 && rin[h] ? *(const float2*)(rin[h] + 8 * (QJ * q + jb + j) + f.fc) : make_float2(0.f, 0.f);
+#pragma unroll
+      for (int j = 0; j < kJ; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (E == kEpiW2 && !rin[h]) continue;
+          mlp_epi_pair<E>(smem, f.fr + 8 * h, 8 * (QJ * q + jb + j) + f.fc, acc[4 * (jb + j) + 2 * h],
+                          acc[4 * (jb + j) + 2 * h + 1], r[j][h], us, bias, a_scale, gout[h], E != kEpiW2 || operand);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < D / 2 - D / 8; ++i) acc[i] = acc[i + D / 8];
+  }
+}
+
 // The three GEMMs of the MLP block with their epilogues, run by one warpgroup on its 64 rows, its operand rows holding O
 // (scaled, split) on entry.  Per fragment row h (tile rows fr, fr + 8): xin[h] residual X (nullptr: zero), aout[h] where A is
 // parked (nullptr: row not stored), xout[h] where X' goes (nullptr: not stored); operand_out: X' also becomes the operand
-// rows (next layer of the trunk).  b1, b2: the biases in global memory (read through the read-only cache).
+// rows (next layer of the trunk).  wmaps: (Wo, W1, W2) x (hi, lo) tensor maps; b1, b2: the biases in global memory (read
+// through the read-only cache).  One call site of the GEMM for all three (a rolled loop): the kernel's code stays small.
 template <int D>
-__device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const CUtensorMap* wo_hi,
-                                     const CUtensorMap* wo_lo, const CUtensorMap* w1_hi, const CUtensorMap* w1_lo,
-                                     const CUtensorMap* w2_hi, const CUtensorMap* w2_lo, float us0, float us1, float us2,
-                                     float a_scale, const float* b1, const float* b2, const float* const (&xin)[2],
-                                     float* const (&aout)[2], float* const (&xout)[2], bool operand_out, int* err,
-                                     PhaseClock& pc) {
-  const Frag f;
+__device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const CUtensorMap* const (&wmaps)[6],
+                                     float us0, float us1, float us2, float a_scale, const float* b1, const float* b2,
+                                     const float* const (&xin)[2], float* const (&aout)[2], float* const (&xout)[2],
+                                     bool operand_out, int* err, PhaseClock& pc) {
   const int wg = threadIdx.x >> 7;
-  // Row loads are issued in batches of kJ fragment columns ahead of the stores: xin / aout / xout may alias, so the compiler
-  // would otherwise wait for every load behind the previous store.
-  constexpr int kJ = 4;
-  // ---- A = X + O Wo -> parked rows and the operand buffer
-  gemm_abuf<D>(acc, smem, ring, wo_hi, wo_lo, 0, kTurnOwn, err, pc);
-  pc.mark(kPhWo);
-#pragma unroll
-  for (int jb = 0; jb < D / 8; jb += kJ) {
-    float2 x[kJ][2];
-#pragma unroll
-    for (int j = 0; j < kJ; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) x[j][h] = xin[h] ? *(const float2*)(xin[h] + 8 * (jb + j) + f.fc) : make_float2(0.f, 0.f);
-#pragma unroll
-    for (int j = 0; j < kJ; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c = 8 * (jb + j) + f.fc;
-        const float a0 = x[j][h].x + acc[4 * (jb + j) + 2 * h] * us0, a1 = x[j][h].y + acc[4 * (jb + j) + 2 * h + 1] * us0;
-        if (aout[h]) *(float2*)(aout[h] + c) = make_float2(a0, a1);
-        store_operand_pair(smem, f.fr + 8 * h, c, a0 * a_scale, a1 * a_scale);
-      }
-  }
-  fence_proxy_async();
-  wg_sync(wg);
-  pc.mark(kPhMlpEpi);
-  // ---- M1 = tanh(A W1 + b1) -> operand buffer
-  gemm_abuf<D>(acc, smem, ring, w1_hi, w1_lo, 0, kTurnOwn, err, pc);
-  pc.mark(kPhW1);
-#pragma unroll
-  for (int j = 0; j < D / 8; ++j) {
-    const int c = 8 * j + f.fc;
-    const float2 b = make_float2(__ldg(b1 + c), __ldg(b1 + c + 1));  // (the parameter table gives no 8-byte alignment)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const float m0 = mlp_tanh(acc[4 * j + 2 * h] * us1 + b.x), m1 = mlp_tanh(acc[4 * j + 2 * h + 1] * us1 + b.y);
-      store_operand_pair(smem, f.fr + 8 * h, c, m0 * a_scale, m1 * a_scale);
+#pragma unroll 1
+  for (int g = 0; g < 3; ++g) {
+    const CUtensorMap* mh = g == 0 ? wmaps[0] : (g == 1 ? wmaps[2] : wmaps[4]);
+    const CUtensorMap* ml = g == 0 ? wmaps[1] : (g == 1 ? wmaps[3] : wmaps[5]);
+    gemm_abuf<D>(acc, smem, ring, mh, ml, 0, kTurnOwn, err, pc);
+    pc.mark(kPhWo + 2 * g);
+    if (g == 0) {  // ---- A = X + O Wo -> parked rows and the operand buffer
+      mlp_epilogue<D, kEpiWo>(acc, smem, us0, nullptr, a_scale, xin, aout, true);
+      fence_proxy_async();
+      wg_sync(wg);
+      pc.mark(kPhWoEpi);
+    } else if (g == 1) {  // ---- M1 = tanh(A W1 + b1) -> operand buffer
+      mlp_epilogue<D, kEpiW1>(acc, smem, us1, b1, a_scale, xin, aout, true);
+      fence_proxy_async();
+      wg_sync(wg);
+      pc.mark(kPhW1Epi);
+    } else {  // ---- X' = A + tanh(M1 W2 + b2)
+      const float* const ain[2] = {aout[0], aout[1]};
+      mlp_epilogue<D, kEpiW2>(acc, smem, us2, b2, a_scale, ain, xout, operand_out);
+      pc.mark(kPhW2Epi);
     }
   }
-  fence_proxy_async();
-  wg_sync(wg);
-  pc.mark(kPhMlpEpi);
-  // ---- X' = A + tanh(M1 W2 + b2)
-  gemm_abuf<D>(acc, smem, ring, w2_hi, w2_lo, 0, kTurnOwn, err, pc);
-  pc.mark(kPhW2);
-#pragma unroll
-  for (int jb = 0; jb < D / 8; jb += kJ) {
-    float2 a[kJ][2];
-#pragma unroll
-    for (int j = 0; j < kJ; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) a[j][h] = aout[h] ? *(const float2*)(aout[h] + 8 * (jb + j) + f.fc) : make_float2(0.f, 0.f);
-#pragma unroll
-    for (int j = 0; j < kJ; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c = 8 * (jb + j) + f.fc;
-        if (!aout[h]) continue;
-        const float2 b = make_float2(__ldg(b2 + c), __ldg(b2 + c + 1));
-        const float x0 = a[j][h].x + mlp_tanh(acc[4 * (jb + j) + 2 * h] * us2 + b.x);
-        const float x1 = a[j][h].y + mlp_tanh(acc[4 * (jb + j) + 2 * h + 1] * us2 + b.y);
-        if (xout[h]) *(float2*)(xout[h] + c) = make_float2(x0, x1);
-        if (operand_out) store_operand_pair(smem, f.fr + 8 * h, c, x0 * a_scale, x1 * a_scale);
-      }
-  }
-  pc.mark(kPhMlpEpi);
 }
 
 template <int D>
@@ -372,8 +391,8 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
       xin[h] = valid ? p.X + (size_t)grow * p.ldx : nullptr;
       aout[h] = valid ? p.Out + (size_t)grow * p.ldout : nullptr;
     }
-    mlp3<D>(acc, smem, ring, &wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo, p.us0, p.us1, p.us2, p.a_scale, p.b1, p.b2,
-            xin, aout, aout, false, p.err_flag, pc);
+    const CUtensorMap* const wmaps[6] = {&wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo};
+    mlp3<D>(acc, smem, ring, wmaps, p.us0, p.us1, p.us2, p.a_scale, p.b1, p.b2, xin, aout, aout, false, p.err_flag, pc);
   }
 }
 

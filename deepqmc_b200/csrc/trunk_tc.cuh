@@ -51,22 +51,26 @@ struct TrunkParams {
   const float* b2[kTrMaxLayers];
   float us[kTrMaxLayers][4];     // accumulator unscale of the four GEMMs of a layer: 1 / (a_scale * weight scale)
   unsigned char* scratch;        // gridDim.x * kTrScratchPerCta bytes
-  int walkers, N, NP, L;         // walkers, electrons per walker, walker slot size (power of two >= N, <= 32), layers
+  int walkers, N, L;             // walkers, electrons per walker, layers
   float a_scale;                 // power of two applied to activations before the hi / lo split
   float attn_scale;              // 1 / sqrt(dh)
   int* err_flag;
   unsigned long long* phase;     // kPhases cycle / pair counters (fused_tc.cuh Phase), accumulated; nullptr: timers off
 };
 
+// NP: the walker slot (electrons rounded up to a power of two, <= 32), one instance each: an instance carries only the
+// attention variant of its slot size.
+template <int NP>
 __global__ void __launch_bounds__(kTrThreads, 1)
 trunk_f16_kernel(TrunkParams p) {
+  static_assert(NP >= 1 && NP <= 32 && (NP & (NP - 1)) == 0, "walker slot: a power of two <= 32");
   DQMC_TC_SMEM(smem);
   if ((smem_u32(smem) & 1023u) != 0u) tc_trap();
 
   const int tid = threadIdx.x, wg = tid >> 7;
-  const int N = p.N, NP = p.NP, L = p.L;
-  const int lnp = 31 - __clz(NP);                // NP is a power of two
-  const int G = 128 / NP;                        // walker slots per tile
+  const int N = p.N, L = p.L;
+  constexpr int lnp = NP == 1 ? 0 : NP == 2 ? 1 : NP == 4 ? 2 : NP == 8 ? 3 : NP == 16 ? 4 : 5;
+  constexpr int G = 128 / NP;                    // walker slots per tile
   const int MT = (p.walkers + G - 1) / G;
   float* qkv = (float*)(p.scratch + (size_t)blockIdx.x * kTrScratchPerCta);  // [128][768]
   float* resid = qkv + 128 * 768;                                            // [128][256]
@@ -98,6 +102,7 @@ trunk_f16_kernel(TrunkParams p) {
     };
     // ---- tile load: the warpgroup's embedding rows -> residual stream and the operand buffer (loads in batches of 8 ahead
     // of the stores)
+#pragma unroll 1
     for (int i0 = 0; i0 < 64 * 64 / 128; i0 += 8) {
       float4 x[8];
 #pragma unroll
@@ -142,6 +147,7 @@ trunk_f16_kernel(TrunkParams p) {
       const bool last = l == L - 1;
       const CUtensorMap* lm = p.maps + 8 * l;
       // ---- Q | K | V = X Wqkv, 256 columns at a time -> scratch (true values)
+#pragma unroll 1
       for (int j = 0; j < 3; ++j) {
         // one MMA token for the three column blocks: their epilogues are much shorter than a GEMM
         const int turn = j == 0 ? kTurnTake : (j == 2 ? kTurnPass : kTurnKeep);
@@ -171,7 +177,7 @@ trunk_f16_kernel(TrunkParams p) {
           const int r = r0 + ag + 8 * i;
           if ((r & (NP - 1)) < N) store_operand_pair(smem, r, 64 * h + c, o0 * p.a_scale, o1 * p.a_scale);
         };
-        if (NP > 16) attn_task_mma<4, true>(p.attn_scale, qrow, krow, vrow, valid, store);
+        if constexpr (NP > 16) attn_task_mma<4, true>(p.attn_scale, qrow, krow, vrow, valid, store);
         else attn_task_mma<2, true>(p.attn_scale, qrow, krow, vrow, valid, store, NP < 16 ? NP : 0);
       }
       fence_proxy_async();
@@ -189,11 +195,12 @@ trunk_f16_kernel(TrunkParams p) {
         const long long row = grow_of(r);
         xout[h] = !last ? resid + r * 256 : (row >= 0 ? p.Out + (size_t)row * p.ldout : nullptr);
       }
-      mlp3<256>(acc, smem, ring, lm + 2, lm + 3, lm + 4, lm + 5, lm + 6, lm + 7, p.us[l][1], p.us[l][2], p.us[l][3],
-                p.a_scale, p.b1[l], p.b2[l], xin, aout, xout, !last, p.err_flag, pc);
+      const CUtensorMap* const wmaps[6] = {lm + 2, lm + 3, lm + 4, lm + 5, lm + 6, lm + 7};
+      mlp3<256>(acc, smem, ring, wmaps, p.us[l][1], p.us[l][2], p.us[l][3], p.a_scale, p.b1[l], p.b2[l], xin, aout, xout,
+                !last, p.err_flag, pc);
       fence_proxy_async();
       wg_sync(wg);  // next layer's operand rows complete / next tile's load may overwrite the residual rows
-      pc.mark(kPhMlpEpi);
+      pc.mark(kPhW2Epi);
       if (tid < 128) pc.count(kPhPairs);
     }
   }

@@ -854,8 +854,8 @@ class Engine:
         self._check(rc, 'dqmc_debug_det_sum')
         return sign, log, grad, stats
 
-    TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'w1_mainloop', 'w2_mainloop',
-                    'mlp_epilogues', 'weight_wait', 'mma_turn', 'tile_layer_pairs')
+    TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'wo_epilogue', 'w1_mainloop',
+                    'w1_epilogue', 'w2_mainloop', 'w2_epilogue', 'weight_wait', 'mma_turn', 'tile_layer_pairs')
 
     def debug_trunk_phases(self):
         """{phase: cycles} of the whole-trunk kernel's timers (engine created with DQMC_TRUNK_PHASES=1) since the last call;

@@ -381,9 +381,10 @@ int dqmc_debug_det_sum(dqmc_handle h, const void* r, const void* R, const void* 
                        void* stats, void* stream);
 
 /* Measurement aid: the phase timers of the whole-trunk kernel, summed over every launch since the last call, then reset.  On
- * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 10.  out[0..9]: clock64()
- * cycles of the consumer warpgroups in tile load, QKV mainloop, QKV epilogue, attention, Wo / W1 / W2 mainloops, MLP
- * epilogues, waiting for weight slots (not part of the mainloops), then the number of (tile, layer) pairs processed. */
+ * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 13.  out[0..11]: clock64()
+ * cycles of the consumer warpgroups in tile load, QKV mainloop, QKV epilogue, attention, Wo mainloop, Wo epilogue, W1
+ * mainloop, W1 epilogue, W2 mainloop, W2 epilogue, waiting for weight slots (not part of the mainloops), waiting for the MMA
+ * token; out[12]: the number of (tile, layer) pairs processed. */
 int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n);
 
 /* Measurement aid (bench.py roofline): between begin/end every dense-layer GEMM launch is

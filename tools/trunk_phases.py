@@ -11,10 +11,18 @@ profiler counts the trunk class: 2 rows (6 d^2 + 2 N d) per layer), each phase's
 and the card's name, power limit and SM clocks (read-only nvidia-smi query).  The two warpgroups of a CTA hand an MMA token
 back and forth: 'mma_turn' is the time a warpgroup waited for the other one's MMAs (the part of its own non-MMA work that
 did not cover them), 'weight_wait' the time it waited for weight slots to land.
+
+'sass_bytes' is the machine code of the trunk instance the run launched (cuobjdump -sass of the built library), split at the
+phase timers in address order: the code between two timer marks belongs to the phase the later mark books, a mark whose
+counter index is only known at run time books to 'shared', and code after the last mark to 'other'.  Where the compiler lays
+out the code of several phases before one mark (the rolled loop over the MLP GEMMs with its three epilogues), that mark's
+phase gets all of it; 'total' is exact.  Code size matters because a (tile, layer) runs the kernel's body once per warp as straight-line code.
 """
 import argparse
 import json
 import os
+import re
+import shutil
 import subprocess
 import sys
 
@@ -34,6 +42,55 @@ def card():
     out = subprocess.run(['nvidia-smi', f'--query-gpu={q}', '--format=csv,noheader'], capture_output=True, text=True,
                          check=True).stdout.strip().splitlines()[0]
     return dict(zip(q.split(','), (x.strip() for x in out.split(','))))
+
+
+def cuobjdump():
+    for c in (os.path.join(os.environ.get('CUDA_HOME', '/usr/local/cuda'), 'bin', 'cuobjdump'), shutil.which('cuobjdump')):
+        if c and os.access(c, os.X_OK):
+            return c
+    return None
+
+
+def sass_bytes(lib, np2, names):
+    """{phase: bytes} of the trunk instance for walker slot np2 in `lib`, split at the phase timer marks (see the module
+    docstring); None without cuobjdump.  A mark is a predicated clock read followed by the same-predicate read of its
+    counter `[R + 8 k]`; reads of the weight_wait / mma_turn counters (waits inside a phase) do not split."""
+    tool = cuobjdump()
+    if tool is None:
+        return None
+    out = ''
+    for fn in (f'_ZN2dq2tc16trunk_f16_kernelILi{np2}EEEvNS0_11TrunkParamsE', '_ZN2dq2tc16trunk_f16_kernelENS0_11TrunkParamsE'):
+        r = subprocess.run([tool, '-sass', '-fun', fn, lib], capture_output=True, text=True)
+        if r.returncode == 0 and 'Function : ' in r.stdout:
+            out = r.stdout
+            break
+    ins = [t.strip() for t in re.findall(r'/\*[0-9a-f]{4,}\*/\s+([^;]*);', out)]
+    assert ins, f'no trunk kernel in {lib}'
+    waits = {names.index('weight_wait'), names.index('mma_turn')}
+    res = {k: 0 for k in names if k != 'tile_layer_pairs'}
+    res.update(shared=0, other=0)
+    start = 0
+    for i, txt in enumerate(ins):
+        if not (txt.startswith('@') and 'SR_CLOCKLO' in txt):
+            continue
+        pred = txt.split()[0]
+        for nxt in ins[i + 1:i + 4]:
+            m = re.match(re.escape(pred) + r'\s+LDS\.64\s+\S+,\s+\[(.*)\]', nxt)
+            if m is None:
+                continue
+            addr = re.fullmatch(r'R\d+(?:\+(0x[0-9a-f]+))?', m.group(1))
+            if addr is None:
+                key = 'shared'
+            else:
+                k = int(addr.group(1) or '0', 16) // 8
+                key = None if k in waits else names[k]
+            if key is not None:
+                res[key] += 16 * (i - start)
+                start = i
+            break
+    res['other'] += 16 * (len(ins) - start)
+    res['total'] = 16 * len(ins)
+    return res
 
 
 def engine(hamil, params, phases):
@@ -95,7 +152,8 @@ def main():
         kernel='tc::trunk_f16_kernel', mol=a.mol, ecp=hamil.ecp_type, walkers=a.walkers, N=N, slot=np2, walkers_per_tile=128 // np2,
         launches=a.launches, grid=grid, ms_per_launch=ms, us_per_tile_layer=ms * 1e3 * grid / pairs,
         algorithmic_tflops=flops / (ms * 1e-3) / 1e12, phase_share={k: v / total for k, v in ph.items()},
-        phase_cycles={k: int(v) for k, v in ph.items()}, card=card())
+        phase_cycles={k: int(v) for k, v in ph.items()},
+        sass_bytes=sass_bytes(os.path.join(ROOT, 'deepqmc_b200', 'libdqmc_b200.so'), np2, timed.TRUNK_PHASES), card=card())
     os.makedirs(a.out_dir, exist_ok=True)
     with open(os.path.join(a.out_dir, f'trunk_phases_{a.mol}.json'), 'w') as f:
         json.dump(res, f, indent=1)
@@ -105,6 +163,8 @@ def main():
           f'{res["algorithmic_tflops"]:.1f} algorithmic TFLOP/s')
     for k, v in res['phase_share'].items():
         print(f'  {k:14s} {100 * v:5.1f} %')
+    if res['sass_bytes']:
+        print('SASS bytes: ' + ', '.join(f'{k} {v}' for k, v in res['sass_bytes'].items() if v))
 
 
 if __name__ == '__main__':
