@@ -486,14 +486,11 @@ struct Engine : EngineBase {
     return 0;
   }
   bool ph_on = false;      // tables uploaded
-  bool ph_active = false;  // set around the forward-Laplacian pass of local_energy only
-  T* mos_out = nullptr;    // set by orbitals(): the tail writes the orbital matrices of the chunk here and stops
   int attn_tb = 1, attn_tb1 = 1;
   bool attn_gen_mma = false;  // ... same for the generic kernel (TransPsiformer: extra key / value tokens)
   bool attn_fl_mma = false;   // fp32 forward-Laplacian attention: tangent chunks as warp-level 3xTF32 mma.sync products
   int attn_fl_threads = 128;  // block size of the fp32 forward-Laplacian attention (large molecules: one block per SM fits -> more warps)
   bool attn_f32 = false;
-  bool gemm_ran_tc = false;   // the last gemm() call ran the tensor-core kernel (not the CUDA-core gemm_kernel)
   bool embed_fwd_ok = false;
   bool attn_mma_ok = false;  // plain-forward attention on mma.sync (attn_mma.cuh)
   bool slater_fwd2_ok = false;
@@ -507,15 +504,20 @@ struct Engine : EngineBase {
   size_t max_smem = 0;
   int n_sms = 132;
   Switches sw;  // read_switches() at the start of init()
-  // compact virtual-walker group in flight (non-local ECP quadrature or spin swaps): envelope table of its base walkers
-  // [nb][N][K N] (null outside those forwards), index of the current chunk's first virtual walker, virtual walkers per base
-  // walker (J N 12, or the swapped pairs), and the layout of virtual_move (common.cuh)
-  const T* ecp_env = nullptr;
-  const T* ecp_emb = nullptr;  // ... and their embedding rows [nb][N][d] (whole-trunk kernel only)
-  int64_t ecp_v0 = 0;
-  int ecp_vper = 0;
-  int virt_layout = kVirtEcp;
-  const int* ecp_pairs = nullptr;  // the ECP group's active-pair list (ecp_pairs_kernel) of virtual_move's ECP layout
+  // What a plain forward (run_batched) takes besides positions and outputs; the default value is an ordinary forward.
+  struct FwdIn {
+    // compact virtual-walker group (non-local ECP quadrature or spin swaps, virtual_groups): envelope table of its base
+    // walkers [nb][N][K N], their embedding rows [nb][N][d] (whole-trunk kernel only), the ECP group's active-pair list
+    // (ecp_pairs_kernel), virtual walkers per base walker (J N 12, or the swapped pairs) and the layout of virtual_move
+    // (common.cuh)
+    const T* env = nullptr;
+    const T* emb = nullptr;
+    const int* pairs = nullptr;
+    int vper = 0;
+    int layout = kVirtEcp;
+    T* mos = nullptr;  // orbitals(): the tail writes the orbital matrices [B][K][N][N] here and stops
+    bool ph = false;   // the pseudo-Hamiltonian metric applies to the forward-Laplacian pass (needs ph_on)
+  };
 #if !defined(DQMC_NO_TCGEN05)
   struct TcWeight {
     float* hi = nullptr; float* lo = nullptr; CUtensorMap mh, ml; int N = 0, K = 0;
@@ -1109,17 +1111,23 @@ struct Engine : EngineBase {
     if (S == 1) return true;
     return S <= 128 && (128 / S) * S >= 112;
   }
+  // gemm() runs the tensor-core kernel for these operands (else the CUDA-core gemm_kernel)
+  bool gemm_on_tc(const char* w0, const char* w1, int lda, int ldc, int Kc, const T* bias1) const {
+#if !defined(DQMC_NO_TCGEN05)
+    return use_tc() && !bias1 && Kc % 32 == 0 && lda % 4 == 0 && ldc % 4 == 0 && tcw.count(w0) && (!w1 || tcw.count(w1));
+#else
+    return false;
+#endif
+  }
   int gemm(const T* A, int lda, const char* w0, const char* w1, int zsplit, int ldw, const T* bias, const T* Res,
            int ldr, T* C, int ldc, int Mr, int Nc, int Kc, int S, int sliced, int Nel, cudaStream_t st, int act = 0,
            const T* bias1 = nullptr) {
     if (dry) return 0;  // planning pass
     const T* W0 = P(w0);
     const T* W1 = w1 ? P(w1) : nullptr;
-    gemm_ran_tc = false;
 #if !defined(DQMC_NO_TCGEN05)
     if constexpr (std::is_same<T, float>::value) {
-      if (use_tc() && !bias1 && Kc % 32 == 0 && lda % 4 == 0 && ldc % 4 == 0 && tcw.count(w0) && (!w1 || tcw.count(w1))) {
-        gemm_ran_tc = true;
+      if (gemm_on_tc(w0, w1, lda, ldc, Kc, bias1)) {
         const TcWeight& t0 = tcw.at(w0);
         const TcWeight& t1 = w1 ? tcw.at(w1) : t0;
         tc::Params p;
@@ -1253,14 +1261,15 @@ struct Engine : EngineBase {
     return false;
 #endif
   }
-  int trunk_block(const T* X0, T* Out, int rows, cudaStream_t st, const T* Xbase = nullptr) {
+  // in.emb set: compact virtual-walker forwards, walker w of the launch is virtual walker v0 + w
+  int trunk_block(const T* X0, T* Out, int rows, cudaStream_t st, const FwdIn& in, int64_t v0) {
     if (dry) return 0;
 #if !defined(DQMC_NO_TCGEN05)
     if constexpr (std::is_same<T, float>::value) {
       tc::TrunkParams p;
       p.X0 = X0; p.ldx = d; p.Out = Out; p.ldout = d; p.maps = d_trunk_maps; p.scratch = d_trunk_scratch;
-      p.Xbase = Xbase; p.v0 = Xbase ? (long long)ecp_v0 : 0; p.vper = Xbase ? ecp_vper : 0;
-      p.n_up = cfg.n_up; p.vlayout = virt_layout; p.pairs = ecp_pairs; p.wspin = P("emb.w") + (size_t)(4 * M) * d;  // the +-1 spin feature's row
+      p.Xbase = in.emb; p.v0 = in.emb ? (long long)v0 : 0; p.vper = in.emb ? in.vper : 0;
+      p.n_up = cfg.n_up; p.vlayout = in.layout; p.pairs = in.pairs; p.wspin = P("emb.w") + (size_t)(4 * M) * d;  // the +-1 spin feature's row
       int np2 = 1;
       while (np2 < N) np2 *= 2;  // walker slot of the tile: electrons rounded up to a power of two (<= 32)
       p.walkers = rows / N; p.N = N; p.L = cfg.n_layers; p.a_scale = kActScale;
@@ -1313,7 +1322,7 @@ struct Engine : EngineBase {
   int debug_trunk(const void* X0, void* Out, int rows, cudaStream_t st) override {
     if (!can_trunk(1)) { err = "fused trunk not available for this configuration"; return 2; }
     if (rows % N != 0) { err = "debug_trunk: rows must be a multiple of the electron count"; return 2; }
-    int rc = trunk_block((const T*)X0, (T*)Out, rows, st);
+    int rc = trunk_block((const T*)X0, (T*)Out, rows, st, FwdIn{}, 0);
     if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
     return 0;
@@ -1366,7 +1375,7 @@ struct Engine : EngineBase {
       rc = 1;
     }
     if (!rc) rc = slater((const T*)r, (const T*)R, 0, Bc, S, bf, gadd, (T*)dsign, (T*)dlog, (T*)dgrad, (T*)dlap, st, nullptr,
-                         nullptr, 0, 0, kVirtEcp, nullptr, kernel);
+                         FwdIn{}, 0, kernel);
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { err = "debug_slater: kernel failed"; rc = 1; }
     cudaFree(bf);
     cudaFree(gadd);
@@ -1697,7 +1706,7 @@ struct Engine : EngineBase {
         gemm(M1, d, (p + "w2").c_str(), nullptr, 0, d, P(p + "b2"), A, d, Out, d, rows, d, d, S, 0, N, st, 1);
       } else {
         gemm(A, d, (p + "w1").c_str(), nullptr, 0, d, P(p + "b1"), nullptr, 0, M1, d, rows, d, d, S, 0, N, st);
-        which = gemm_ran_tc ? DQMC_MLP_PATH_GEMM_TANH : DQMC_MLP_PATH_SIMT_TANH;
+        which = gemm_on_tc((p + "w1").c_str(), nullptr, d, d, d, nullptr) ? DQMC_MLP_PATH_GEMM_TANH : DQMC_MLP_PATH_SIMT_TANH;
         DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, (d + 127) / 128), dim3(128), 0, st, M1, d, (const T*)nullptr, 0, S, d, T(1));
         gemm(M1, d, (p + "w2").c_str(), nullptr, 0, d, P(p + "b2"), nullptr, 0, Out, d, rows, d, d, S, 0, N, st);
         DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, (d + 127) / 128), dim3(128), 0, st, Out, d, (const T*)A, d, S, d, T(1));
@@ -1707,12 +1716,13 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  // one chunk of run_batched: walkers v0 .. v0 + Bc - 1 of its batch
   int run_chunk(const T* r, const T* R, int Rb, int Bc, int S, int Bstat, T* sign, T* logp, T* E, T* stats, T* grad,
-                void* wsbase, cudaStream_t st) {
+                void* wsbase, cudaStream_t st, const FwdIn& in, int64_t v0) {
     Ws w = carve(wsbase, Bc, S);
     const int rows = Bc * N * S;
     const T* qa = nullptr;  // pseudo-Hamiltonian: per-electron metric of the forward-Laplacian pass
-    if (ph_on && ph_active && S > 1) {
+    if (in.ph && S > 1) {
       DQ_LAUNCH(ph_coeff_kernel<T>, dim3((Bc * N + 127) / 128), dim3(128), 0, st, r, R, Rb, N, M, ph_args(nullptr), w.QA,
                 Bc * N);
       qa = w.QA;
@@ -1722,17 +1732,17 @@ struct Engine : EngineBase {
       const T* jas = nullptr;
       int rc = paulinet_trunk(r, R, Rb, Bc, S, w, &Xbf, &jas, st, qa);
       if (rc) return rc;
-      return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, Xbf, st, jas, qa);
+      return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, Xbf, st, in, v0, jas, qa);
     }
     if (cfg.kind == DQMC_FERMINET) {
       T* Xf = nullptr;
       int rc = ferminet_trunk(r, R, Rb, Bc, S, w, &Xf, st, qa);
       if (rc) return rc;
-      return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, Xf, st, nullptr, qa);
+      return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, Xf, st, in, v0, nullptr, qa);
     }
     const int F = 4 * M + 1;
-    const bool compact = S == 1 && embed_fwd_ok && ecp_emb && can_trunk(S);
-    if (compact && virt_layout != kVirtEcp) {
+    const bool compact = S == 1 && embed_fwd_ok && in.emb && can_trunk(S);
+    if (compact && in.layout != kVirtEcp) {
       // spin swaps: no embedding launch -- the whole-trunk kernel's tile load forms the two swapped rows from the base walkers'
       // table (the embedding is linear in the spin feature)
     } else if (compact) {
@@ -1741,7 +1751,7 @@ struct Engine : EngineBase {
       int epb = (Bc / (2 * n_sms)) / 32 * 32;
       epb = epb < 32 ? 32 : (epb > 512 ? 512 : epb);
       DQ_LAUNCH(embed_fwd_kernel<T>, dim3((Bc + epb - 1) / epb), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, r, R, Rb, N,
-                M, cfg.n_up, 1, P("emb.w"), d, w.X, Bc, epb, (long long)ecp_v0, ecp_vper, ecp_pairs);
+                M, cfg.n_up, 1, P("emb.w"), d, w.X, Bc, epb, (long long)v0, in.vper, in.pairs);
     } else if (S == 1 && embed_fwd_ok) {
       // plain forwards (Metropolis, ECP quadrature): register-tiled projection, W staged per block
       const int tot = Bc * N;
@@ -1757,9 +1767,9 @@ struct Engine : EngineBase {
     T* X = w.X;
     T* O = w.O;
     if (can_trunk(S)) {  // plain forward: every layer in one persistent tensor-core launch
-      int rc = trunk_block(X, O, rows, st, compact ? ecp_emb : nullptr);
+      int rc = trunk_block(X, O, rows, st, in, v0);
       if (rc) return rc;
-      return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, O, st, nullptr, qa);
+      return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, O, st, in, v0, nullptr, qa);
     }
     for (int l = 0; l < cfg.n_layers; ++l) {
       std::string p = "L" + std::to_string(l) + ".";
@@ -1770,18 +1780,18 @@ struct Engine : EngineBase {
       if (rc) return rc;
       T* tmp = X; X = O; O = tmp;
     }
-    return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, X, st, nullptr, qa);
+    return tail(r, R, Rb, Bc, S, Bstat, sign, logp, E, stats, grad, w, X, st, in, v0, nullptr, qa);
   }
 
   // Backflow activation -> K signed log-determinants (+ 3N tangents, Laplacian for S > 1), the kernel picked for the shape:
   // BF [Bc N S][BFW] holds the backflow head rows before activation (row (b N + i) S + s) and is activated IN PLACE; Gadd
-  // [Bc N][5] receives the additive branch's electron factor.  env_base / v0 / vper: the non-local ECP's envelope table
-  // (slater_fwd2_kernel), qa: the pseudo-Hamiltonian metric (slater_kernel), both null outside those passes.  With mos_out
-  // set, the orbital matrices are written there instead of determinants.  *kernel (if given) = {DQMC_SLATER_KERNEL_*, the
-  // template instance NS / NM, 0 for the runtime-N kernels}.  The forward tails and dqmc_debug_slater both call this.
+  // [Bc N][5] receives the additive branch's electron factor.  in.env: the virtual-walker group's envelope table
+  // (slater_fwd2_kernel; the chunk's walkers are virtual walkers v0 ..), qa: the pseudo-Hamiltonian metric (slater_kernel),
+  // both null outside those passes.  With in.mos set, the chunk's orbital matrices are written there from walker v0 on
+  // instead of determinants.  *kernel (if given) = {DQMC_SLATER_KERNEL_*, the template instance NS / NM, 0 for the
+  // runtime-N kernels}.  The forward tails and dqmc_debug_slater both call this.
   int slater(const T* r, const T* R, int Rb, int Bc, int S, T* BF, T* Gadd, T* dsign, T* dlog, T* dgrad, T* dlap,
-             cudaStream_t st, const T* qa, const T* env_base, int64_t v0, int vper, int vlayout = kVirtEcp,
-             const int* pairs = nullptr, int32_t* kernel = nullptr) {
+             cudaStream_t st, const T* qa, const FwdIn& in, int64_t v0, int32_t* kernel = nullptr) {
     if (cfg.mult_act == 1)  // default mult_act 1 + 2 tanh(x / 4) of the BackflowOp (nn_wave_function.py:14-33)
       DQ_LAUNCH(act_fl_kernel<T>, dim3(Bc * N, (KN + 127) / 128), dim3(128), 0, st, BF, KN, (const T*)nullptr, 0, S, KN, T(1), 2);
     const int full_det = cfg.factorized_det ? 0 : 1;
@@ -1796,11 +1806,11 @@ struct Engine : EngineBase {
                 P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), env_rep, full_det, Gadd, Bc * N);
       gadd = Gadd;
     }
-    if (mos_out) {  // Ansatz.apply(..., return_mos=True): orbital matrices instead of determinants
+    if (in.mos) {  // Ansatz.apply(..., return_mos=True): orbital matrices instead of determinants
       const size_t tot = (size_t)Bc * K * N * N;
       DQ_LAUNCH(orbitals_kernel<T>, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, r, R, Rb, N, M, cfg.n_up, K,
                 P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, BFW, env_rep, full_det,
-                mos_out, tot, gadd, add_off, mult_on);
+                in.mos + (size_t)v0 * K * N * N, tot, gadd, add_off, mult_on);
       return 0;
     }
     int32_t which = DQMC_SLATER_KERNEL_GENERIC, inst = 0;
@@ -1831,7 +1841,7 @@ struct Engine : EngineBase {
   inst = NMV;                                                                                                                  \
   DQ_LAUNCH((slater_fwd2_kernel<T, NMV>), dim3(grid), dim3(nthr), slater_fwd2_smem_bytes<T>(N, M, K), st, r, R, Rb, N, M,      \
             cfg.n_up, K, Bc, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), (const T*)BF, KN, dsign,     \
-            dlog, env_rep, full_det, env_base, (long long)v0, vper, vlayout, pairs)
+            dlog, env_rep, full_det, in.env, (long long)v0, in.vper, in.layout, in.pairs)
       if (N == 14) { DQ_SL_FWD2(14); }
       else if (N <= 16) { DQ_SL_FWD2(16); }
       else if (N == 28) { DQ_SL_FWD2(28); }
@@ -1864,13 +1874,12 @@ struct Engine : EngineBase {
 
   // backflow heads -> Slater determinants -> det sum / cusp / potentials (shared by all trunks)
   int tail(const T* r, const T* R, int Rb, int Bc, int S, int Bstat, T* sign, T* logp, T* E, T* stats, T* grad, Ws& w,
-           T* X, cudaStream_t st, const T* jastrow = nullptr, const T* qa = nullptr) {
+           T* X, cudaStream_t st, const FwdIn& in, int64_t v0, const T* jastrow = nullptr, const T* qa = nullptr) {
     // per-spin backflow heads: rows of electron e across walkers, weights by spin
     gemm(X, bf_in, "bf.up", "bf.dn", cfg.n_up, BFW, gnn ? P("bfb.up") : nullptr, nullptr, 0, w.BF, BFW, Bc * S, BFW, bf_in, S, 1, N,
          st, 0, gnn ? P("bfb.dn") : nullptr);
-    int rc = slater(r, R, Rb, Bc, S, w.BF, w.Gadd, w.dsign, w.dlog, w.dgrad, w.dlap, st, qa, ecp_env, ecp_v0, ecp_vper,
-                    virt_layout, ecp_pairs);
-    if (rc || mos_out) return rc;
+    int rc = slater(r, R, Rb, Bc, S, w.BF, w.Gadd, w.dsign, w.dlog, w.dgrad, w.dlap, st, qa, in, v0);
+    if (rc || in.mos) return rc;
     const FinalizeCfg fc = finalize_cfg(S);
     DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), dim3(128), finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb,
               (const T*)w.dsign, (const T*)w.dlog, (const T*)w.dgrad, (const T*)w.dlap, P("cusp.alpha"),
@@ -1881,17 +1890,16 @@ struct Engine : EngineBase {
   }
 
   int run_batched(const T* r, const T* R, int Rb, int B, int S, T* sign, T* logp, T* E, T* stats, T* grad, void* ws,
-                  int64_t wsb, cudaStream_t st) {
+                  int64_t wsb, cudaStream_t st, const FwdIn& in = {}) {
     int Bc = max_chunk(wsb, S, B);
     if (Bc < 1) { err = "workspace too small for a single walker"; return 3; }
     if (chunk_bytes(Bc, S) > wsb) { err = "internal: carved workspace exceeds the planned size"; return 3; }
     if (dry) { carve(ws, Bc, S); return 0; }  // planning pass: record the extent of the largest chunk
     for (int b0 = 0; b0 < B; b0 += Bc) {
       int nb = std::min(Bc, B - b0);
-      ecp_v0 = b0;  // index of the chunk's first walker in the caller's batch (quadrature forwards: virtual-walker index)
-      int rc = run_chunk(r + (size_t)b0 * 3 * N, R + (Rb ? (size_t)b0 * 3 * M : 0), Rb, nb, S, B, sign + b0, logp + b0,
-                         E ? E + b0 : nullptr, stats ? stats + b0 : nullptr, grad ? grad + (size_t)b0 * T3 : nullptr, ws,
-                         st);
+      int rc = run_chunk(r + (size_t)b0 * 3 * N, R + (Rb ? (size_t)b0 * 3 * M : 0), Rb, nb, S, B, sign ? sign + b0 : nullptr,
+                         logp ? logp + b0 : nullptr, E ? E + b0 : nullptr, stats ? stats + b0 : nullptr,
+                         grad ? grad + (size_t)b0 * T3 : nullptr, ws, st, in, b0);
       if (rc) return rc;
       rc = check_guards();
       if (rc) return rc;
@@ -1906,7 +1914,9 @@ struct Engine : EngineBase {
     Arena a(this, ws, wsb);
     const ForceBufs f = carve_force(a, B);
     if (a.left() < 0) { err = "workspace too small (Langevin force buffers)"; return 3; }
-    int rc = run_batched(r, R, Rb, B, T3 + 2, sign, logp, f.E, f.stats, f.grad, a.top, a.left(), st);
+    FwdIn in;
+    in.ph = false;  // the drift is the gradient of log|psi| alone (electron_samplers.py:201-209): no pseudo-Hamiltonian metric
+    int rc = run_batched(r, R, Rb, B, T3 + 2, sign, logp, f.E, f.stats, f.grad, a.top, a.left(), st, in);
     if (rc) return rc;
     DQ_LAUNCH(langevin_force_kernel<T>, dim3((B * N + 127) / 128), dim3(128), 0, st, (const T*)f.grad, r, R, Rb, (const T*)d_znuc,
               tau, N, M, B * N, force);
@@ -2573,19 +2583,10 @@ struct Engine : EngineBase {
   }
 
   // orbital matrices out[B][K][N][N] (electron i, orbital mu) of a plain forward
-  int orbitals(const void* r_, const void* R_, int Rb, int B, void* out, void* ws, int64_t wsb, cudaStream_t st) override {
-    const T* r = (const T*)r_;
-    const T* R = (const T*)R_;
-    const int Bc = max_chunk(wsb, 1, B);
-    if (Bc < 1) { err = "workspace too small for a single walker"; return 3; }
-    int rc = 0;
-    for (int b0 = 0; b0 < B && !rc; b0 += Bc) {
-      const int nb = std::min(Bc, B - b0);
-      mos_out = (T*)out + (size_t)b0 * K * N * N;
-      rc = run_chunk(r + (size_t)b0 * 3 * N, R + (Rb ? (size_t)b0 * 3 * M : 0), Rb, nb, 1, B, nullptr, nullptr, nullptr, nullptr,
-                     nullptr, ws, st);
-    }
-    mos_out = nullptr;
+  int orbitals(const void* r, const void* R, int Rb, int B, void* out, void* ws, int64_t wsb, cudaStream_t st) override {
+    FwdIn in;
+    in.mos = (T*)out;
+    int rc = run_batched((const T*)r, (const T*)R, Rb, B, 1, nullptr, nullptr, nullptr, nullptr, nullptr, ws, wsb, st, in);
     if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
     return 0;
@@ -2602,10 +2603,10 @@ struct Engine : EngineBase {
   // Virtual walkers (vper per base walker: ECP quadrature points, spin swaps) through a per-group pass in groups of nb base
   // walkers: the largest group whose prefix (carve_group) + one pass chunk of all its virtual walkers (chunk_carve, a dry carve
   // after the prefix) fits wsb, else one walker (the pass chunks its virtual walkers).  Per group, setup() launches the kind's
-  // work before the pass and sets V, the virtual walkers to run, pass(g, V, rest) runs them in the workspace after the prefix
-  // (run_batched: plain forwards; reverse_pass: position gradients), and finish() reduces their results.  With `tables` (and
-  // slater_fwd2, N <= 32) the forwards take the unmoved electrons' envelopes and, with `emb_table`, embedding rows from tables
-  // of the base walkers.
+  // work before the pass and sets V, the virtual walkers to run, pass(g, in, V, rest) runs them in the workspace after the
+  // prefix (run_batched: plain forwards; reverse_pass: position gradients), and finish() reduces their results.  With `tables`
+  // (and slater_fwd2, N <= 32) the forwards take the unmoved electrons' envelopes and, with `emb_table`, embedding rows from
+  // tables of the base walkers: `in` describes them (default: none).
   template <class CarveGroup, class Setup, class Pass, class ChunkCarve, class Finish>
   int virtual_groups(const T* r, const T* R, int B, int64_t vper, int layout, bool tables, bool emb_table, void* ws,
                      int64_t wsb, const char* too_small, CarveGroup carve_group, Setup setup, Pass pass, ChunkCarve chunk_carve,
@@ -2630,18 +2631,18 @@ struct Engine : EngineBase {
       int64_t V = 0;
       int rc = setup(b0, nb, g, a, V);
       if (rc) return rc;
+      FwdIn in;
       if (tables) {
         DQ_LAUNCH(env_table_kernel<T>, dim3(nb), dim3(256), sizeof(T) * N * M, st, rb, R, N, M, cfg.n_up, K * N, P("env.pi_up"),
                   P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"), env_rep, g.env);
-        ecp_env = g.env; ecp_vper = (int)vper; virt_layout = layout; ecp_pairs = g.pairs;
+        in.env = g.env; in.vper = (int)vper; in.layout = layout; in.pairs = g.pairs;
         if (emb_table) {
           DQ_LAUNCH(embed_fwd_kernel<T>, dim3((nb * N + 31) / 32), dim3(256), embed_fwd_smem_bytes<T>(M, d), st, rb, R, 0, N, M,
                     cfg.n_up, 1, P("emb.w"), d, g.emb, nb * N, 32, 0LL, 0, (const int*)nullptr);
-          ecp_emb = g.emb;
+          in.emb = g.emb;
         }
       }
-      if (V > 0) rc = pass(g, V, a);
-      ecp_env = nullptr; ecp_emb = nullptr; ecp_pairs = nullptr; virt_layout = kVirtEcp;
+      if (V > 0) rc = pass(g, in, V, a);
       if (rc) return rc;
       rc = finish(b0, nb, g);
       if (!rc) rc = check_guards();  // the prefix's guards, also when no forward ran (V == 0)
@@ -2652,8 +2653,30 @@ struct Engine : EngineBase {
   }
 
   // the plain-forward pass of a virtual-walker group (ECP energy, spin), in the workspace after the group's prefix
-  int virt_forwards(const VirtGroup& g, const T* R, int64_t V, const Arena& rest, cudaStream_t st) {
-    return run_batched(g.r, R, 0, (int)V, 1, g.sign, g.logp, nullptr, nullptr, nullptr, rest.top, rest.left(), st);
+  int virt_forwards(const VirtGroup& g, const FwdIn& in, const T* R, int64_t V, const Arena& rest, cudaStream_t st) {
+    return run_batched(g.r, R, 0, (int)V, 1, g.sign, g.logp, nullptr, nullptr, nullptr, rest.top, rest.left(), st, in);
+  }
+
+  // The non-local ECP's virtual walkers of the group g of nb base walkers from walker b0 on (nuclei shared by all walkers):
+  // the electron-nucleus pairs inside the cutoff radii rc2 (ecp_pairs_kernel), whose quadrature forwards alone run, and
+  // their quadrature points (ecp_points_kernel) with the twists `twist` [B][J][N] or, if null, twists drawn from `seed`.
+  // V = the number of quadrature points.  The energy and the force pass share it, each with its own radii.
+  int ecp_group_points(const T* r, const T* R, int b0, int nb, const VirtGroup& g, const double* rc2, const T* twist,
+                       uint64_t seed, int64_t& V, cudaStream_t st) {
+    const T* rb = r + (size_t)b0 * 3 * N;
+    DQ_LAUNCH(ecp_pairs_kernel<T>, dim3(1), dim3(1024), 0, st, rb, R, 0, N, M, J, (const int*)d_nl_nuc, rc2, nb, g.offs,
+              g.pairs, g.offs + nb);
+    int n_act = nb * J * N;  // the planning pass sizes every buffer for all pairs
+    if (!dry) {
+      DQ_CHECK(cudaMemcpyAsync(&n_act, g.offs + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+      DQ_CHECK(cudaStreamSynchronize(st));
+      ecp_forwards += (int64_t)n_act * 12;
+    }
+    V = (int64_t)n_act * 12;
+    if (n_act > 0)
+      DQ_LAUNCH(ecp_points_kernel<T>, dim3(n_act), dim3(64), 0, st, rb, R, 0, N, M, J, (const int*)d_nl_nuc,
+                twist ? twist + (size_t)b0 * J * N : nullptr, seed, (uint64_t)b0, (const int*)g.pairs, g.r);
+    return 0;
   }
 
   // Hellmann-Feynman force terms with effective core potentials (reference force.py:252-301): bare = F_nuc(Z_eff) - grad_R V_loc
@@ -2683,21 +2706,9 @@ struct Engine : EngineBase {
         const PosOut p0{nullptr, g.gR0};
         int rc = reverse_pass(rb, R, 0, nb, nullptr, g.sign0, g.logp0, nullptr, &p0, rest.top, rest.left(), st, "ecp_force");
         if (rc) return rc;
-        DQ_LAUNCH(ecp_pairs_kernel<T>, dim3(1), dim3(1024), 0, st, rb, R, 0, N, M, J, (const int*)d_nl_nuc,
-                  (const double*)d_nl_rc2f, nb, g.offs, g.pairs, g.offs + nb);
-        int n_act = nb * J * N;  // the planning pass sizes every buffer for all pairs
-        if (!dry) {
-          DQ_CHECK(cudaMemcpyAsync(&n_act, g.offs + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
-          DQ_CHECK(cudaStreamSynchronize(st));
-          ecp_forwards += (int64_t)n_act * 12;
-        }
-        V = (int64_t)n_act * 12;
-        if (n_act > 0)
-          DQ_LAUNCH(ecp_points_kernel<T>, dim3(n_act), dim3(64), 0, st, rb, R, 0, N, M, J, (const int*)d_nl_nuc,
-                    twist ? (const T*)twist + (size_t)b0 * J * N : nullptr, seed, (uint64_t)b0, (const int*)g.pairs, g.r);
-        return 0;
+        return ecp_group_points(r, R, b0, nb, g, d_nl_rc2f, (const T*)twist, seed, V, st);
       };
-      auto pass = [&](const VirtGroup& g, int64_t V, const Arena& rest) {
+      auto pass = [&](const VirtGroup& g, const FwdIn&, int64_t V, const Arena& rest) {
         const PosOut pv{g.gr, g.gR};
         return reverse_pass(g.r, R, 0, (int)V, nullptr, g.sign, g.logp, nullptr, &pv, rest.top, rest.left(), st, "ecp_force");
       };
@@ -2722,30 +2733,15 @@ struct Engine : EngineBase {
                    void* stats, void* sign, void* logp, void* grad, void* ws, int64_t wsb, cudaStream_t st) override {
     const T* r = (const T*)r_;
     const T* R = (const T*)R_;
-    ph_active = ph_on;
-    int rc = run_batched(r, R, Rb, B, T3 + 2, (T*)sign, (T*)logp, (T*)E, (T*)stats, (T*)grad, ws, wsb, st);
-    ph_active = false;
+    if (J > 0 && Rb) { err = "non-local ECP with per-walker nuclei is not supported"; return 2; }
+    FwdIn in;
+    in.ph = ph_on;
+    int rc = run_batched(r, R, Rb, B, T3 + 2, (T*)sign, (T*)logp, (T*)E, (T*)stats, (T*)grad, ws, wsb, st, in);
     if (rc) return rc;
     if (J > 0) {
       // non-local ECP: virtual walkers (12 quadrature points x electrons x ECP nuclei)
       auto setup = [&](int b0, int nb, const VirtGroup& g, const Arena&, int64_t& V) {
-        if (Rb) { err = "non-local ECP with per-walker nuclei is not supported"; return 2; }
-        const T* rb = r + (size_t)b0 * 3 * N;
-        const T* tw = twist ? (const T*)twist + (size_t)b0 * J * N : nullptr;
-        // the pairs inside the cutoff radius; the group's quadrature forwards run over them alone
-        DQ_LAUNCH(ecp_pairs_kernel<T>, dim3(1), dim3(1024), 0, st, rb, R, Rb, N, M, J, (const int*)d_nl_nuc,
-                  (const double*)d_nl_rc2, nb, g.offs, g.pairs, g.offs + nb);
-        int n_act = nb * J * N;  // the planning pass sizes every buffer for all pairs
-        if (!dry) {
-          DQ_CHECK(cudaMemcpyAsync(&n_act, g.offs + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
-          DQ_CHECK(cudaStreamSynchronize(st));
-          ecp_forwards += (int64_t)n_act * 12;
-        }
-        V = (int64_t)n_act * 12;
-        if (n_act > 0)
-          DQ_LAUNCH(ecp_points_kernel<T>, dim3(n_act), dim3(64), 0, st, rb, R, Rb, N, M, J, (const int*)d_nl_nuc, tw,
-                    seed, (uint64_t)b0, (const int*)g.pairs, g.r);
-        return 0;
+        return ecp_group_points(r, R, b0, nb, g, d_nl_rc2, (const T*)twist, seed, V, st);
       };
       auto finish = [&](int b0, int nb, const VirtGroup& g) {
         DQ_LAUNCH(ecp_accumulate_kernel<T>, dim3((nb + 3) / 4), dim3(128), 0, st, r + (size_t)b0 * 3 * N, R, Rb, N, M, J,
@@ -2757,7 +2753,7 @@ struct Engine : EngineBase {
       };
       rc = virtual_groups(r, R, B, (int64_t)J * N * 12, kVirtEcp, sw.ecp_env_table, sw.ecp_emb_table, ws, wsb,
                           "workspace too small for the non-local ECP pass", [&](Arena& a, int64_t nb) { return carve_ecp_group(a, nb); }, setup,
-                          [&](const VirtGroup& g, int64_t V, const Arena& a) { return virt_forwards(g, R, V, a, st); },
+                          [&](const VirtGroup& g, const FwdIn& in, int64_t V, const Arena& a) { return virt_forwards(g, in, R, V, a, st); },
                           [&](Arena& a, int64_t Vc) { fwd_chunk_carve(a, Vc); }, finish, st);
       if (rc) return rc;
     }
@@ -2807,7 +2803,7 @@ struct Engine : EngineBase {
     // embedding rows from tables of the base walkers
     int rc = virtual_groups(r, R, B, Pn, down_idx, cfg.kind == DQMC_PSIFORMER, true, ws, wsb, "workspace too small for the spin pass",
                             [&](Arena& a, int64_t nb) { return carve_spin_group(a, nb, Pn); }, setup,
-                            [&](const VirtGroup& g, int64_t V, const Arena& a) { return virt_forwards(g, R, V, a, st); },
+                            [&](const VirtGroup& g, const FwdIn& in, int64_t V, const Arena& a) { return virt_forwards(g, in, R, V, a, st); },
                             [&](Arena& a, int64_t Vc) { fwd_chunk_carve(a, Vc); }, finish, st);
     if (rc) return rc;
     DQ_CHECK(cudaGetLastError());
