@@ -5,10 +5,11 @@
 // One warp task = 16 queries of one (walker, head) pair against all of its keys (electrons, plus the TransPsiformer's constant
 // nuclear tokens).  Scores S = Q K^T and outputs O = P V are m16n8k16 products of half operands split into hi + lo
 // (x 2^e = hi + lo, 22 significant bits; three products  hi.lo + lo.hi + hi.hi  accumulated in fp32: fp32-class accuracy, the
-// power-of-two scales are undone exactly).  No shared memory: every fragment is loaded from global memory in the layout the
-// instruction wants -- a quad of lanes reads 32 contiguous bytes of a row per instruction (full sectors) -- converted in
-// registers, and the probabilities move from the accumulator layout of S to the A-operand layout of P V without leaving the
-// register file (the C fragment of two adjacent 8-key tiles IS the A fragment of one 16-key tile).
+// power-of-two scales are undone exactly).  The task body (attn_task_frag) takes its Q / K / V fragments from the caller,
+// already split: attn_task_mma loads them from fp32 rows in global memory and splits them in registers, the whole-trunk
+// kernel (trunk_tc.cuh) splits each operand once where it is produced.  The probabilities move from the accumulator layout
+// of S to the A-operand layout of P V without leaving the register file (the C fragment of two adjacent 8-key tiles IS the
+// A fragment of one 16-key tile).
 // dh = 64 only (4 k-tiles of 16); keys <= 8 NK8.
 #pragma once
 #include <cstdint>
@@ -79,67 +80,48 @@ __device__ __forceinline__ void am_split2(float x0, float x1, uint32_t& hi, uint
   lo = am_pack_half2(x0 - am_half_to_float(hi & 0xFFFFu), x1 - am_half_to_float(hi >> 16));
 }
 
-template <bool kCoherent>
-__device__ __forceinline__ float2 am_ld2(const float* p) {
-  if constexpr (kCoherent) return *(const float2*)p;
-  else return __ldg((const float2*)p);
-}
-template <bool kCoherent>
-__device__ __forceinline__ float am_ld1(const float* p) {
-  if constexpr (kCoherent) return *p;
-  else return __ldg(p);
-}
+// Operand scales of the task: q, k, v by 2^4, probabilities by 2^10 (undone exactly).  A caller that hands over pre-split
+// fragments splits x * kAmQS with am_split2, the split of the fp32 loaders below.
+constexpr float kAmQS = 16.f, kAmPS = 1024.f;
 
-// One warp task: 16 query rows of one head against 8 NK8 keys (dh = 64).  The caller supplies the rows and the mask; lane
-// (g = lane / 4, t = lane % 4) holds query rows g (i = 0) and g + 8 (i = 1):
-//   qrow(i)            query row i (64 fp32)
-//   krow(j), vrow(j)   key / value row j < 8 NK8 (padded keys must point at readable rows: their scores are masked)
-//   valid(i, j)        key j takes part in the softmax of query row i (every row needs at least one)
-//   store(i, c, o0, o1) normalised output of query row i, head columns c, c + 1
-// kCoherent: plain global loads (rows written earlier by the same kernel) instead of the read-only path.
+// One warp task: 16 query rows of one head against 8 NK8 keys (dh = 64), from fragments the caller loads already split
+// (lane: g = lane / 4, t = lane % 4, query rows g (i = 0) and g + 8 (i = 1)):
+//   ldq(kt, qh, ql)             A fragments of Q x kAmQS, k-tile kt (hi / lo: rows g, g + 8 x columns 16 kt + 2 t (+1, +8, +9))
+//   ldk(nt, kt, kh, kl)         B fragments of K x kAmQS: key nt * 8 + g, columns 16 kt + 2 t (+1) and + 8 (+9)
+//   ldv(kk, nt, keep, vh, vl)   B fragments of V x kAmQS: keys 16 kk + 2 t (+1) and + 8 (+9), column nt * 8 + g; the pair
+//                               halves of keys j with !keep(j) are zeros (substituted, never multiplied)
+//   valid(i, j)                 key j takes part in the softmax of query row i (every row needs at least one)
+//   store(i, c, o0, o1)         normalised output of query row i, head columns c, c + 1
+// Padded keys must load finite fragments: their scores are masked, their V pairs enter P V with probability zero.
 // slot > 0 (NK8 = 2, keys = the task's own 16 rows, every key masked to the query rows of its own slot of `slot` rows): a masked
 // key's probability is an exact zero, but its V row still enters P V, and 0 x Inf = NaN, so one slot with a non-finite V row
 // (or one past the range of the scaled half split, |v| >= 65504 / 16) would make the outputs of every slot in the 16-row window
 // non-finite.  If any output of the task is non-finite, P V is therefore recomputed slot by slot with the V rows of the other
 // slots read as zeros: the other slots' outputs come out exactly as without the bad slot, the bad slot's stay non-finite.
-template <int NK8, bool kCoherent, class QRow, class KRow, class VRow, class Valid, class Store>
-__device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow, VRow vrow, Valid valid, Store store,
-                                              int slot = 0) {
+template <int NK8, class LdQ, class LdK, class LdV, class Valid, class Store>
+__device__ __forceinline__ void attn_task_frag(float scale, LdQ ldq, LdK ldk, LdV ldv, Valid valid, Store store, int slot = 0) {
   constexpr int NK16 = (NK8 + 1) / 2;
-  constexpr float kQS = 16.f, kPS = 1024.f;  // operand scales: q, k, v by 2^4, probabilities by 2^10
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   // ---- Q fragments of this query tile (rows g, g + 8), hi / lo, 4 k-tiles of 16
-  const float* qp0 = qrow(0);
-  const float* qp1 = qrow(1);
   uint32_t qh[4][4], ql[4][4];
 #pragma unroll
-  for (int kt = 0; kt < 4; ++kt) {
-    const float2 a0 = am_ld2<kCoherent>(qp0 + kt * 16 + 2 * t), a1 = am_ld2<kCoherent>(qp1 + kt * 16 + 2 * t);
-    const float2 a2 = am_ld2<kCoherent>(qp0 + kt * 16 + 8 + 2 * t), a3 = am_ld2<kCoherent>(qp1 + kt * 16 + 8 + 2 * t);
-    am_split2(a0.x * kQS, a0.y * kQS, qh[kt][0], ql[kt][0]);
-    am_split2(a1.x * kQS, a1.y * kQS, qh[kt][1], ql[kt][1]);
-    am_split2(a2.x * kQS, a2.y * kQS, qh[kt][2], ql[kt][2]);
-    am_split2(a3.x * kQS, a3.y * kQS, qh[kt][3], ql[kt][3]);
-  }
+  for (int kt = 0; kt < 4; ++kt) ldq(kt, qh[kt], ql[kt]);
   // ---- scores: S[16 x 8 NK8] = Q K^T; B fragment of key tile nt: (k = dh index, n = key nt * 8 + g)
   float s[NK8][4];
 #pragma unroll
   for (int nt = 0; nt < NK8; ++nt) {
     s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-    const float* kp = krow(nt * 8 + g);
 #pragma unroll
     for (int kt = 0; kt < 4; ++kt) {
-      const float2 b0 = am_ld2<kCoherent>(kp + kt * 16 + 2 * t), b1 = am_ld2<kCoherent>(kp + kt * 16 + 8 + 2 * t);
       uint32_t kh[2], kl[2];
-      am_split2(b0.x * kQS, b0.y * kQS, kh[0], kl[0]);
-      am_split2(b1.x * kQS, b1.y * kQS, kh[1], kl[1]);
+      ldk(nt, kt, kh, kl);
       mma16816(s[nt], qh[kt], kl);
       mma16816(s[nt], ql[kt], kh);
       mma16816(s[nt], qh[kt], kh);
     }
   }
   // ---- softmax over the keys of rows g (c0, c1) and g + 8 (c2, c3); a lane holds keys nt * 8 + 2 t, + 1
-  const float us = scale / (kQS * kQS);
+  const float us = scale / (kAmQS * kAmQS);
   float m0 = -3.0e38f, m1 = -3.0e38f;
 #pragma unroll
   for (int nt = 0; nt < NK8; ++nt) {
@@ -168,30 +150,24 @@ __device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow,
 #pragma unroll
   for (int kk = 0; kk < NK16; ++kk) {
     const int n0 = 2 * kk, n1 = 2 * kk + 1;
-    am_split2(s[n0][0] * kPS, s[n0][1] * kPS, ph[kk][0], pl[kk][0]);
-    am_split2(s[n0][2] * kPS, s[n0][3] * kPS, ph[kk][1], pl[kk][1]);
+    am_split2(s[n0][0] * kAmPS, s[n0][1] * kAmPS, ph[kk][0], pl[kk][0]);
+    am_split2(s[n0][2] * kAmPS, s[n0][3] * kAmPS, ph[kk][1], pl[kk][1]);
     if (n1 < NK8) {
-      am_split2(s[n1 < NK8 ? n1 : n0][0] * kPS, s[n1 < NK8 ? n1 : n0][1] * kPS, ph[kk][2], pl[kk][2]);
-      am_split2(s[n1 < NK8 ? n1 : n0][2] * kPS, s[n1 < NK8 ? n1 : n0][3] * kPS, ph[kk][3], pl[kk][3]);
+      am_split2(s[n1 < NK8 ? n1 : n0][0] * kAmPS, s[n1 < NK8 ? n1 : n0][1] * kAmPS, ph[kk][2], pl[kk][2]);
+      am_split2(s[n1 < NK8 ? n1 : n0][2] * kAmPS, s[n1 < NK8 ? n1 : n0][3] * kAmPS, ph[kk][3], pl[kk][3]);
     } else {
       ph[kk][2] = ph[kk][3] = pl[kk][2] = pl[kk][3] = 0u;
     }
   }
   // ---- O[16 x 64] = P V: B fragment of dh tile nt: (k = key 16 kk + 2 t (+1, +8, +9), n = dh nt * 8 + g)
-  const float uo0 = 1.f / (l0 * kPS * kQS), uo1 = 1.f / (l1 * kPS * kQS);
+  const float uo0 = 1.f / (l0 * kAmPS * kAmQS), uo1 = 1.f / (l1 * kAmPS * kAmQS);
   // dh tile nt of P V, V rows of the keys j with keep(j) (the others read as zeros)
   auto pv = [&](int nt, float (&o)[4], auto keep) {
     o[0] = o[1] = o[2] = o[3] = 0.f;
 #pragma unroll
     for (int kk = 0; kk < NK16; ++kk) {
-      const int j = kk * 16 + 2 * t;
-      const float v00 = keep(j) ? am_ld1<kCoherent>(vrow(j) + nt * 8 + g) : 0.f;
-      const float v01 = keep(j + 1) ? am_ld1<kCoherent>(vrow(j + 1) + nt * 8 + g) : 0.f;
-      const float v10 = keep(j + 8) ? am_ld1<kCoherent>(vrow(j + 8) + nt * 8 + g) : 0.f;
-      const float v11 = keep(j + 9) ? am_ld1<kCoherent>(vrow(j + 9) + nt * 8 + g) : 0.f;
       uint32_t vh[2], vl[2];
-      am_split2(v00 * kQS, v01 * kQS, vh[0], vl[0]);
-      am_split2(v10 * kQS, v11 * kQS, vh[1], vl[1]);
+      ldv(kk, nt, keep, vh, vl);
       mma16816(o, ph[kk], vl);
       mma16816(o, pl[kk], vh);
       mma16816(o, ph[kk], vh);
@@ -225,6 +201,41 @@ __device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow,
       }
     }
   }
+}
+
+// The task on fp32 rows in global memory (read-only path), split in registers: every fragment is loaded in the layout the
+// instruction wants -- a quad of lanes reads 32 contiguous bytes of a row per instruction (full sectors).
+//   qrow(i)            query row i (64 fp32)
+//   krow(j), vrow(j)   key / value row j < 8 NK8 (padded keys must point at readable rows: their scores are masked)
+template <int NK8, class QRow, class KRow, class VRow, class Valid, class Store>
+__device__ __forceinline__ void attn_task_mma(float scale, QRow qrow, KRow krow, VRow vrow, Valid valid, Store store) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const float* qp0 = qrow(0);
+  const float* qp1 = qrow(1);
+  auto ldq = [&](int kt, uint32_t (&qh)[4], uint32_t (&ql)[4]) {
+    const float2 a0 = __ldg((const float2*)(qp0 + kt * 16 + 2 * t)), a1 = __ldg((const float2*)(qp1 + kt * 16 + 2 * t));
+    const float2 a2 = __ldg((const float2*)(qp0 + kt * 16 + 8 + 2 * t)), a3 = __ldg((const float2*)(qp1 + kt * 16 + 8 + 2 * t));
+    am_split2(a0.x * kAmQS, a0.y * kAmQS, qh[0], ql[0]);
+    am_split2(a1.x * kAmQS, a1.y * kAmQS, qh[1], ql[1]);
+    am_split2(a2.x * kAmQS, a2.y * kAmQS, qh[2], ql[2]);
+    am_split2(a3.x * kAmQS, a3.y * kAmQS, qh[3], ql[3]);
+  };
+  auto ldk = [&](int nt, int kt, uint32_t (&kh)[2], uint32_t (&kl)[2]) {
+    const float* kp = krow(nt * 8 + g);
+    const float2 b0 = __ldg((const float2*)(kp + kt * 16 + 2 * t)), b1 = __ldg((const float2*)(kp + kt * 16 + 8 + 2 * t));
+    am_split2(b0.x * kAmQS, b0.y * kAmQS, kh[0], kl[0]);
+    am_split2(b1.x * kAmQS, b1.y * kAmQS, kh[1], kl[1]);
+  };
+  auto ldv = [&](int kk, int nt, auto keep, uint32_t (&vh)[2], uint32_t (&vl)[2]) {
+    const int j = kk * 16 + 2 * t;
+    const float v00 = keep(j) ? __ldg(vrow(j) + nt * 8 + g) : 0.f;
+    const float v01 = keep(j + 1) ? __ldg(vrow(j + 1) + nt * 8 + g) : 0.f;
+    const float v10 = keep(j + 8) ? __ldg(vrow(j + 8) + nt * 8 + g) : 0.f;
+    const float v11 = keep(j + 9) ? __ldg(vrow(j + 9) + nt * 8 + g) : 0.f;
+    am_split2(v00 * kAmQS, v01 * kAmQS, vh[0], vl[0]);
+    am_split2(v10 * kAmQS, v11 * kAmQS, vh[1], vl[1]);
+  };
+  attn_task_frag<NK8>(scale, ldq, ldk, ldv, valid, store);
 }
 
 // NK8 = number of 8-key tiles (keys padded to 8 NK8 <= 48); block = 4 warps, each warp walks over (pair, query tile) tasks.
@@ -261,7 +272,7 @@ attn_fwd_mma_kernel(const float* __restrict__ QKV, int ldq, float* __restrict__ 
       const int q = i ? q1 : q0;
       if (q < N) *(float2*)(O + ((size_t)b * N + q) * ldo + h * DH + c) = make_float2(o0, o1);
     };
-    attn_task_mma<NK8, false>(scale, qrow, krow, vrow, valid, store);
+    attn_task_mma<NK8>(scale, qrow, krow, vrow, valid, store);
   }
 }
 

@@ -528,7 +528,7 @@ struct Engine : EngineBase {
     CUtensorMap m16h_256, m16l_256; bool f16_256 = false;  // 256-row boxes of 32 halves: weight slots of the whole-trunk kernel (trunk_tc.cuh)
   };
   CUtensorMap* d_trunk_maps = nullptr;       // [L][4][2]
-  unsigned char* d_trunk_scratch = nullptr;  // n_sms x 512 KB: Q / K / V and residual rows of a tile
+  unsigned char* d_trunk_scratch = nullptr;  // n_sms x 384 KB: split K / V and residual rows of a tile
   unsigned long long* d_trunk_phase = nullptr;  // DQMC_TRUNK_PHASES=1: the whole-trunk kernel's phase timers (tc::kPhases)
   static constexpr float kActScale = 16.f;  // 2^4: |activation| < 4094 representable, absolute floor 2^-29
   std::map<std::string, TcWeight> tcw;

@@ -46,6 +46,12 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // barrier of the 128 threads of one warpgroup (named barrier id = 1 + warpgroup; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// four 8 x 8 matrices of halves from shared memory: lane l gives the 16-byte row (l % 8) of matrix l / 8, register i holds
+// row lane / 4, columns 2 (lane % 4), +1 of matrix i (the A fragment of mma.m16n8k16 for rows / columns ordered so)
+__device__ __forceinline__ void ldsm_x4(uint32_t saddr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr) : "memory");
+}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int x, int y) {

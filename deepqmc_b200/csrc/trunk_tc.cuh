@@ -10,14 +10,21 @@
 // into the 128-byte-swizzled K-major operand buffer in shared memory ("3xFP16" hi / lo halves, see gemm_wgmma.cuh); the
 // dense GEMMs are those of the fused MLP block (fused_tc.cuh: wgmma m64 n256, accumulators in registers, weights streamed
 // by TMA).  HBM sees the embedding rows once on the way in and the trunk output once on the way out; the residual stream
-// (128 x 256 fp32) and Q / K / V (128 x 768 fp32) of the tile live in a per-CTA scratch buffer (512 KB, re-used for every
-// tile and layer, i.e. L2 resident): the register file holds one accumulator, and shared memory (operand buffer + ring)
-// cannot park them.
+// (128 x 256 fp32) and K / V of the tile (128 x 512, as split half pairs) live in a per-CTA scratch buffer (384 KB, re-used
+// for every tile and layer, i.e. L2 resident): the register file holds one accumulator, and shared memory (operand buffer +
+// ring) cannot park them.
 //
+// The QKV projection runs its column blocks in the order K, V, Q, and each epilogue splits its block into the hi / lo half
+// pairs of the attention's operands (am_split2 of x kAmQS), once per element rather than once per reading warp:
+//   K  -> scratch [128 rows][128 column pairs] of uint2 {hi, lo}: a score B fragment is one 8-byte load;
+//   V  -> scratch [64 key pairs][256 columns] of uint2 {hi, lo} of keys (2 p, 2 p + 1): a P V B fragment is one 8-byte load
+//         (the lanes of rows 2 p and 2 p + 1 swap one value to form the pairs);
+//   Q  -> k-block h of the operand buffer for head h's 64 columns (hi / lo planes, the GEMM operand layout): once the Q
+//         GEMM has retired, the warpgroup's X rows there are dead (X is in the residual rows).  Padding rows keep X.
 // Attention on the tensor cores: warp w takes tile rows r0 = 16 w .. +15 and runs the 3xFP16 mma.sync task of attn_mma.cuh
-// (shared with attn_fwd_mma_kernel) for each head, with Q, K and V read straight from the scratch (plain, coherent loads: the
-// rows were written by this kernel) and O_h written, scaled and split, into k-block h of the operand buffer (dead once the
-// QKV GEMMs have retired).  The keys of a task are its walker slot (NP = 32: 4 key tiles of 8) or, for slots of at most 16
+// (shared with attn_fwd_mma_kernel) for each head, Q fragments by ldmatrix from the operand buffer, K / V fragments straight
+// from the scratch (plain, coherent loads: this kernel wrote them), and writes O_h, scaled and split, over Q in k-block h
+// (the rows of warp w's Q are read and overwritten by warp w only).  The keys of a task are its walker slot (NP = 32: 4 key tiles of 8) or, for slots of at most 16
 // rows, the task's own 16 rows masked to the query's slot (2 key tiles; a walker whose V rows are non-finite cannot turn the
 // other walkers of the window non-finite, see attn_task_mma's slot argument).  Padding rows (electron >= N) get no attention
 // output: their operand rows keep the finite previous operand and are never stored.
@@ -34,8 +41,8 @@ namespace tc {
 
 constexpr int kTrThreads = 256;
 constexpr int kTrMaxLayers = 8;
-constexpr int kTrQkvBytes = 128 * 768 * 4;                   // Q | K | V rows of the tile, fp32
-constexpr int kTrScratchPerCta = kTrQkvBytes + 128 * 256 * 4;  // + residual stream rows
+constexpr int kTrKvBytes = 128 * 512 * 4;                    // K | V of the tile, split half pairs (uint2 {hi, lo})
+constexpr int kTrScratchPerCta = kTrKvBytes + 128 * 256 * 4;  // + residual stream rows
 using TrSmem = MlpSmem;
 
 struct TrunkParams {
@@ -72,8 +79,9 @@ trunk_f16_kernel(TrunkParams p) {
   constexpr int lnp = NP == 1 ? 0 : NP == 2 ? 1 : NP == 4 ? 2 : NP == 8 ? 3 : NP == 16 ? 4 : 5;
   constexpr int G = 128 / NP;                    // walker slots per tile
   const int MT = (p.walkers + G - 1) / G;
-  float* qkv = (float*)(p.scratch + (size_t)blockIdx.x * kTrScratchPerCta);  // [128][768]
-  float* resid = qkv + 128 * 768;                                            // [128][256]
+  uint2* kbuf = (uint2*)(p.scratch + (size_t)blockIdx.x * kTrScratchPerCta);  // [128 rows][128 column pairs]
+  uint2* vbuf = kbuf + 128 * 128;                                              // [64 key pairs][256 columns]
+  float* resid = (float*)(vbuf + 64 * 256);                                    // [128][256]
 
   if (tid == 0) {
     init_rings(smem);
@@ -89,7 +97,7 @@ trunk_f16_kernel(TrunkParams p) {
   float acc[128];
   // attention task of this warp: tile rows r0 .. r0 + 15 (lane: rows r0 + ag, r0 + ag + 8), keys from tile row k0 (inside
   // the warpgroup's 64 rows: a walker slot is at most 32 rows and aligned)
-  const int r0 = 16 * (tid >> 5), ag = (tid & 31) >> 2;
+  const int lane = tid & 31, r0 = 16 * (tid >> 5), ag = lane >> 2;
   const int k0 = r0 & ~((NP > 16 ? NP : 16) - 1);
   // From here on the warpgroups only meet at the MMA token: warpgroup w owns tile rows 64 w .. +63 (operand rows, residual
   // and Q / K / V scratch rows, attention keys) and synchronises its own 128 threads.  Both run every tile and layer of the
@@ -146,29 +154,79 @@ trunk_f16_kernel(TrunkParams p) {
     for (int l = 0; l < L; ++l) {
       const bool last = l == L - 1;
       const CUtensorMap* lm = p.maps + 8 * l;
-      // ---- Q | K | V = X Wqkv, 256 columns at a time -> scratch (true values)
+      // ---- K | V | Q = X Wqkv, 256 columns at a time, split for the attention
 #pragma unroll 1
       for (int j = 0; j < 3; ++j) {
+        const int blk = j == 2 ? 0 : j + 1;  // column block: K, V, then Q (its epilogue overwrites the operand X)
         // one MMA token for the three column blocks: their epilogues are much shorter than a GEMM
         const int turn = j == 0 ? kTurnTake : (j == 2 ? kTurnPass : kTurnKeep);
-        gemm_abuf<256>(acc, smem, ring, lm, lm + 1, 256 * j, turn, p.err_flag, pc);
+        gemm_abuf<256>(acc, smem, ring, lm, lm + 1, 256 * blk, turn, p.err_flag, pc);
         pc.mark(kPhQkv);
         const float us = p.us[l][0];
+        const int odd = ag & 1;  // fragment rows fr, fr + 8 have the parity of ag
+        // K / V: where column pair (c, c + 1) of fragment row h goes, c = 64 q + 8 jj + fc -> gdst[h] + 32 q + 4 jj (K) or
+        // + 64 q + 8 jj (V: even rows keys (r, r + 1) of column c, odd rows keys (r - 1, r) of column c + 1)
+        uint2* gdst[2];
 #pragma unroll
-        for (int jj = 0; jj < 32; ++jj)
+        for (int h = 0; h < 2; ++h) {
+          const int r = f.fr + 8 * h;
+          gdst[h] = blk == 1 ? kbuf + r * 128 + (f.fc >> 1) : vbuf + (r >> 1) * 256 + f.fc + odd;
+        }
+        const int gq = blk == 1 ? 32 : 64;
+        // one body for the three blocks, rolled over column quarters as in mlp_epilogue: the quarter's values are always
+        // acc[0 .. 31]
+#pragma unroll 1
+        for (int q = 0; q < 4; ++q) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
-            *(float2*)(qkv + (f.fr + 8 * h) * 768 + 256 * j + 8 * jj + f.fc) =
-                make_float2(acc[4 * jj + 2 * h] * us, acc[4 * jj + 2 * h + 1] * us);
+          for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = f.fr + 8 * h, c = 64 * q + 8 * jj + f.fc;
+              // (acc us) kAmQS, two roundings: what the fp32 loaders split from a stored fp32 value
+              float x0 = acc[4 * jj + 2 * h] * us * kAmQS, x1 = acc[4 * jj + 2 * h + 1] * us * kAmQS;
+              if (blk == 2) {  // the key pair: one value from the lane of the neighbouring row
+                const float y = __shfl_xor_sync(0xffffffffu, odd ? x0 : x1, 4);
+                x0 = odd ? y : x0;
+                x1 = odd ? x1 : y;
+              }
+              uint2 v;
+              am_split2(x0, x1, v.x, v.y);
+              if (blk != 0) {
+                gdst[h][gq * q + (gq >> 3) * jj] = v;
+              } else if ((r & (NP - 1)) < N) {  // Q of head q; padding rows keep their finite X operand
+                const int off = operand_off(r, c);
+                *(uint32_t*)(smem + MlpSmem::abuf(q, 0) + off) = v.x;
+                *(uint32_t*)(smem + MlpSmem::abuf(q, 1) + off) = v.y;
+              }
+            }
+#pragma unroll
+          for (int i = 0; i < 96; ++i) acc[i] = acc[i + 32];
+        }
         pc.mark(kPhQkvEpi);
       }
-      wg_sync(wg);  // Q / K / V rows of the warpgroup are in the scratch buffer
+      wg_sync(wg);  // K / V rows of the warpgroup are in the scratch buffer, Q in the operand buffer
       // ---- attention on the tensor cores, head by head -> k-block h of the operand buffer
       for (int h = 0; h < 4; ++h) {
-        const float* qb = qkv + 64 * h;
-        auto qrow = [&](int i) -> const float* { return qb + (r0 + ag + 8 * i) * 768; };
-        auto krow = [&](int j) -> const float* { return qb + (k0 + j) * 768 + 256; };
-        auto vrow = [&](int j) -> const float* { return qb + (k0 + j) * 768 + 512; };
+        const uint32_t qhi = smem_u32(smem + MlpSmem::abuf(h, 0)), qlo = smem_u32(smem + MlpSmem::abuf(h, 1));
+        auto ldq = [&](int kt, uint32_t (&qh)[4], uint32_t (&ql)[4]) {
+          const int off = operand_off(r0 + (lane & 15), 16 * kt + 8 * (lane >> 4));
+          ldsm_x4(qhi + off, qh);
+          ldsm_x4(qlo + off, ql);
+        };
+        auto ldk = [&](int nt, int kt, uint32_t (&kh)[2], uint32_t (&kl)[2]) {
+          const uint2* kp = kbuf + (k0 + nt * 8 + ag) * 128 + 32 * h + 8 * kt + (lane & 3);
+          const uint2 a = kp[0], b = kp[4];
+          kh[0] = a.x; kl[0] = a.y; kh[1] = b.x; kl[1] = b.y;
+        };
+        auto ldv = [&](int kk, int nt, auto keep, uint32_t (&vh)[2], uint32_t (&vl)[2]) {
+          const int j = 16 * kk + 2 * (lane & 3);
+          const uint2* vp = vbuf + ((k0 + j) >> 1) * 256 + 64 * h + 8 * nt + ag;
+          const uint2 a = vp[0], b = vp[4 * 256];
+          // halves of keys outside keep() are zeros: the split of a zero is a zero pair
+          auto sel = [](uint32_t x, bool lo, bool hi) { return (lo ? x & 0xFFFFu : 0u) | (hi ? x & 0xFFFF0000u : 0u); };
+          vh[0] = sel(a.x, keep(j), keep(j + 1)); vl[0] = sel(a.y, keep(j), keep(j + 1));
+          vh[1] = sel(b.x, keep(j + 8), keep(j + 9)); vl[1] = sel(b.y, keep(j + 8), keep(j + 9));
+        };
         auto valid = [&](int i, int j) {
           const int r = r0 + ag + 8 * i, k = k0 + j;
           return (k >> lnp) == (r >> lnp) && (k & (NP - 1)) < N;
@@ -177,8 +235,7 @@ trunk_f16_kernel(TrunkParams p) {
           const int r = r0 + ag + 8 * i;
           if ((r & (NP - 1)) < N) store_operand_pair(smem, r, 64 * h + c, o0 * p.a_scale, o1 * p.a_scale);
         };
-        if constexpr (NP > 16) attn_task_mma<4, true>(p.attn_scale, qrow, krow, vrow, valid, store);
-        else attn_task_mma<2, true>(p.attn_scale, qrow, krow, vrow, valid, store, NP < 16 ? NP : 0);
+        attn_task_frag<(NP > 16 ? 4 : 2)>(p.attn_scale, ldq, ldk, ldv, valid, store, NP < 16 ? NP : 0);
       }
       fence_proxy_async();
       wg_sync(wg);
