@@ -23,7 +23,8 @@ SYMBOLS = [
     'dqmc_workspace_bytes_min', 'dqmc_debug_plan', 'dqmc_stats_pack', 'dqmc_debug_mlp_block', 'dqmc_debug_trunk',
     'dqmc_profile_end_classes', 'dqmc_debug_trunk_phases', 'dqmc_debug_attention', 'dqmc_debug_mlp',
     'dqmc_debug_slater', 'dqmc_debug_det_sum', 'dqmc_spin', 'dqmc_ecp_forward_count', 'dqmc_wf_grad_positions',
-    'dqmc_force_terms', 'dqmc_ecp_force',
+    'dqmc_force_terms', 'dqmc_ecp_force', 'dqmc_debug_wgrad',
+    'dqmc_debug_attention_bwd',
 ]
 
 
@@ -89,6 +90,8 @@ def load(path: str | None = None) -> C.CDLL:
     lib.dqmc_debug_mlp.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32, C.POINTER(i32), vp]
     lib.dqmc_debug_slater.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, C.POINTER(i32), vp]
     lib.dqmc_debug_det_sum.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp]
+    lib.dqmc_debug_wgrad.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp]
+    lib.dqmc_debug_attention_bwd.argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, vp]
     lib.dqmc_wf_forward.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, i64, vp]
     lib.dqmc_wf_orbitals.argtypes = [vp, vp, vp, i32, i32, vp, vp, i64, vp]
     lib.dqmc_local_energy.argtypes = [vp, vp, vp, i32, i32, u64, vp, vp, vp, vp, vp, vp, vp, i64, vp]

@@ -187,6 +187,10 @@ struct EngineBase {
   virtual int debug_det_sum(const void* r, const void* R, const void* dsign, const void* dlog, const void* dgrad,
                             const void* dlap, int B, int S, void* sign, void* logp, void* grad, void* stats,
                             cudaStream_t st) = 0;
+  virtual int debug_wgrad(const void* A, const void* dY, int rows, int Kc, int Nc, int lo, int hi, void* dW, void* db,
+                          cudaStream_t st) = 0;
+  virtual int debug_attention_bwd(int layer, const void* QKV, const void* dO, void* dQKV, void* dKn, void* dVn, int rows,
+                                  cudaStream_t st) = 0;
   virtual int forward(const void* r, const void* R, int Rb, int B, void* sign, void* logp, void* ws, int64_t wsb,
                       cudaStream_t st) = 0;
   virtual int local_energy(const void* r, const void* R, int Rb, int B, uint64_t seed, const void* twist, void* E,
@@ -1404,6 +1408,29 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  int debug_attention_bwd(int layer, const void* QKV, const void* dO, void* dQKV, void* dKn, void* dVn, int rows,
+                          cudaStream_t st) override {
+    if (!(cfg.kind == DQMC_PSIFORMER || trans)) { err = "debug_attention_bwd: the configuration has no softmax attention layers"; return 2; }
+    if (layer < 0 || layer >= cfg.n_layers) { err = "debug_attention_bwd: layer out of range"; return 2; }
+    if (rows < 1 || rows % N != 0) { err = "debug_attention_bwd: rows must be a positive multiple of N"; return 2; }
+    if (Mn > 0 && (!dKn || !dVn)) { err = "debug_attention_bwd: nuclear tokens need the dKn / dVn outputs"; return 2; }
+    int rc = attention_bwd(layer, (const T*)QKV, (const T*)dO, (T*)dQKV, rows / N, Mn > 0 ? (T*)dKn : nullptr,
+                           Mn > 0 ? (T*)dVn : nullptr, st);
+    if (rc) return rc;
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
+  int debug_wgrad(const void* A, const void* dY, int rows, int Kc, int Nc, int lo, int hi, void* dW, void* db,
+                  cudaStream_t st) override {
+    if (rows < 1 || Kc < 1 || Nc < 1) { err = "debug_wgrad: rows, K and Nc must be positive"; return 2; }
+    if (hi != ALL_ROWS && (lo < 0 || hi < lo || hi > N)) { err = "debug_wgrad: the electron range must lie in [0, N]"; return 2; }
+    wgrad((const T*)A, Kc, (const T*)dY, Nc, rows, Kc, Nc, (T*)dW, lo, hi, st);
+    bgrad((const T*)dY, Nc, rows, Nc, (T*)db, st, lo, hi);
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
   int debug_gemm(const char* wname, const char* bname, const void* A, const void* Res, void* C, int Mr, int S,
                  int sliced, int backend, cudaStream_t st) override {
     int64_t o = off(wname);
@@ -1974,25 +2001,27 @@ struct Engine : EngineBase {
     DQ_LAUNCH((gemm_kernel<T, BM, BN, BK, TM, TN>), grid, dim3(256), 0, st, g);
     return 0;
   }
-  // dW += A^T dY over `rows` rows (optionally only electrons lo <= i < hi of every walker), db += column sums; a null dW / db
-  // (PG in the position mode) accumulates nothing
+  // dW += A^T dY over `rows` rows, db += column sums.  The rows are (walker, electron i) pairs; [lo, hi) selects electrons
+  // lo <= i < hi of every walker (the per-spin heads), hi = ALL_ROWS takes every row.  An empty selection (a spin block with
+  // no electrons) accumulates nothing, and so does a null dW / db (PG in the position mode).
+  static constexpr int ALL_ROWS = -1;
   void wgrad(const T* A, int lda, const T* dY, int ldy, int rows, int Kc, int Nc, T* dW, int lo, int hi, cudaStream_t st) {
-    if (!dW) return;
+    if (!dW || (hi != ALL_ROWS && hi <= lo)) return;
     int nz = (rows + 4095) / 4096;
     if (nz > 256) nz = 256;
     if (nz < 1) nz = 1;
     const int rpb = ((rows + nz - 1) / nz + 31) / 32 * 32;
     DQ_LAUNCH(gemm_tn_kernel<T>, dim3((Nc + 31) / 32, (Kc + 31) / 32, (rows + rpb - 1) / rpb), dim3(256), 0, st, A, lda, dY, ldy,
-              rows, Kc, Nc, rpb, hi > lo ? N : 0, lo, hi, dW, Nc);
+              rows, Kc, Nc, rpb, hi == ALL_ROWS ? 0 : N, lo, hi, dW, Nc);
   }
-  void bgrad(const T* dZ, int ld, int rows, int Nc, T* db, cudaStream_t st, int lo = 0, int hi = 0) {
-    if (!db) return;
+  void bgrad(const T* dZ, int ld, int rows, int Nc, T* db, cudaStream_t st, int lo = 0, int hi = ALL_ROWS) {
+    if (!db || (hi != ALL_ROWS && hi <= lo)) return;
     int ny = (rows + 2047) / 2048;
     if (ny > 128) ny = 128;
     if (ny < 1) ny = 1;
     const int rpb = (rows + ny - 1) / ny;
     DQ_LAUNCH(colsum_kernel<T>, dim3((Nc + 127) / 128, (rows + rpb - 1) / rpb), dim3(128), 0, st, dZ, ld, rows, Nc, rpb, db,
-              hi > lo ? N : 0, lo, hi);
+              hi == ALL_ROWS ? 0 : N, lo, hi);
   }
 
   // Position mode of the reverse passes (dqmc_wf_grad_positions): cotangent 1 per walker, no parameter gradients, the chain
@@ -2066,6 +2095,19 @@ struct Engine : EngineBase {
     wgrad(XL, d, dBF, KN, Bc * N, d, KN, PG(G, "bf.dn"), cfg.n_up, N, st);
   }
 
+  // Softmax attention backward of layer `layer` (plain forward, one slot), one block per (walker, head): QKV / dQKV rows
+  // [Bc N][3d], dO [Bc N][d].  With nuclear tokens (TransPsiformer) the cotangents of their keys / values are accumulated
+  // over walkers into dKn / dVn [Mn][d] (null: not wanted).  vjp_chunk and dqmc_debug_attention_bwd both run this.
+  int attention_bwd(int layer, const T* QKV, const T* dO, T* dQKV, int Bc, T* dKn, T* dVn, cudaStream_t st) {
+    const std::string q = "L" + std::to_string(layer) + ".";
+    const size_t smem = attn_bwd_smem_bytes<T>(N, dh, Mn);
+    if (smem > 227 * 1024) { err = "system too large for the shared-memory tiling of the attention reverse pass (N)"; return 2; }
+    DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)smem));
+    DQ_LAUNCH(attn_bwd_kernel<T>, dim3(Bc, H), dim3(128), smem, st, QKV, 3 * d, dO, d, N, dh, d, (T)(1.0 / std::sqrt((double)dh)),
+              dQKV, Mn > 0 ? P(q + "kn") : (const T*)nullptr, Mn > 0 ? P(q + "vn") : (const T*)nullptr, Mn, dKn, dVn);
+    return 0;
+  }
+
   int vjp_chunk(const T* r, const T* R, int Rb, int Bc, const T* wts, T* sign, T* logp, T* G, Arena a, cudaStream_t st,
                 const PosOut* po) {
     const int L = cfg.n_layers, rows = Bc * N, F = 4 * M + 1;
@@ -2106,22 +2148,20 @@ struct Engine : EngineBase {
       DQ_LAUNCH(tanh_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dXn, (const T*)X[l + 1],
                 (const T*)A[l], dZ, nel);
       bgrad(dZ, d, rows, d, PG(G, q + "b2"), st);
-      wgrad(M1[l], d, dZ, d, rows, d, d, PG(G, q + "w2"), 0, 0, st);
+      wgrad(M1[l], d, dZ, d, rows, d, d, PG(G, q + "w2"), 0, ALL_ROWS, st);
       gemm_raw(dZ, d, PT(q + "w2"), nullptr, 0, d, nullptr, 0, dM1, d, rows, d, d, 0, st);
       // M1 = tanh(A W1 + b1)
       DQ_LAUNCH(tanh_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dM1, (const T*)M1[l],
                 (const T*)nullptr, dZ, nel);
       bgrad(dZ, d, rows, d, PG(G, q + "b1"), st);
-      wgrad(A[l], d, dZ, d, rows, d, d, PG(G, q + "w1"), 0, 0, st);
+      wgrad(A[l], d, dZ, d, rows, d, d, PG(G, q + "w1"), 0, ALL_ROWS, st);
       gemm_raw(dZ, d, PT(q + "w1"), nullptr, 0, d, dXn, d, dA, d, rows, d, d, 0, st);  // dA = dX_{l+1} + dZ1 W1^T
       // A = X + O Wo
-      wgrad(O[l], d, dA, d, rows, d, d, PG(G, q + "wo"), 0, 0, st);
+      wgrad(O[l], d, dA, d, rows, d, d, PG(G, q + "wo"), 0, ALL_ROWS, st);
       gemm_raw(dA, d, PT(q + "wo"), nullptr, 0, d, nullptr, 0, dO, d, rows, d, d, 0, st);
-      DQ_LAUNCH(attn_bwd_kernel<T>, dim3(Bc, H), dim3(128), attn_bwd_smem_bytes<T>(N, dh, Mn), st, (const T*)QKV[l], 3 * d,
-                (const T*)dO, d, N, dh, d, scale, dQKV, Mn > 0 ? P(q + "kn") : (const T*)nullptr,
-                Mn > 0 ? P(q + "vn") : (const T*)nullptr, Mn, Mn > 0 ? PG(G, q + "kn") : (T*)nullptr,
-                Mn > 0 ? PG(G, q + "vn") : (T*)nullptr);
-      wgrad(X[l], d, dQKV, 3 * d, rows, d, 3 * d, PG(G, q + "wqkv"), 0, 0, st);
+      rc = attention_bwd(l, QKV[l], dO, dQKV, Bc, Mn > 0 ? PG(G, q + "kn") : (T*)nullptr, Mn > 0 ? PG(G, q + "vn") : (T*)nullptr, st);
+      if (rc) return rc;
+      wgrad(X[l], d, dQKV, 3 * d, rows, d, 3 * d, PG(G, q + "wqkv"), 0, ALL_ROWS, st);
       gemm_raw(dQKV, 3 * d, PT(q + "wqkv"), nullptr, 0, d, dA, d, dX, d, rows, d, 3 * d, 0, st);  // dX_l = dA + dQKV Wqkv^T
       T* t = dXn; dXn = dX; dX = t;
     }
@@ -2131,7 +2171,7 @@ struct Engine : EngineBase {
       return 0;
     }
     DQ_LAUNCH(embed_feat_kernel<T>, dim3((rows * M + 127) / 128), dim3(128), 0, st, r, R, Rb, N, M, cfg.n_up, Feat, rows);
-    wgrad(Feat, F, dXn, d, rows, F, d, G + off("emb.w"), 0, 0, st);
+    wgrad(Feat, F, dXn, d, rows, F, d, G + off("emb.w"), 0, ALL_ROWS, st);
     return 0;
   }
 
@@ -2193,7 +2233,7 @@ struct Engine : EngineBase {
       DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nel + 255) / 256)), dim3(256), 0, st, (const T*)dHn, (const T*)Hs[l + 1],
                 (const T*)(res_h ? Hs[l] : nullptr), res_h ? isq2 : T(1), dZ, nel);
       bgrad(dZ, d, rows, d, PG(G, q + "bg"), st);
-      wgrad(Fs[l], fin, dZ, d, rows, fin, d, PG(G, q + "wg"), 0, 0, st);
+      wgrad(Fs[l], fin, dZ, d, rows, fin, d, PG(G, q + "wg"), 0, ALL_ROWS, st);
       if (l > 0 || po) {
         gemm_raw(dZ, d, PT(q + "wg"), nullptr, 0, fin, nullptr, 0, dF, fin, rows, fin, d, 0, st);
         DQ_LAUNCH(fermi_agg_bwd_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)dF, dc, ec, N, cfg.n_up,
@@ -2205,7 +2245,7 @@ struct Engine : EngineBase {
         DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nee + 255) / 256)), dim3(256), 0, st, (const T*)dEn, (const T*)Es[l + 1],
                   (const T*)(res_e ? Es[l] : nullptr), res_e ? isq2 : T(1), dZe, nee);
         bgrad(dZe, de, rowsE, de, PG(G, q + "bu"), st);
-        wgrad(Es[l], ec, dZe, de, rowsE, ec, de, PG(G, q + "wu"), 0, 0, st);
+        wgrad(Es[l], ec, dZe, de, rowsE, ec, de, PG(G, q + "wu"), 0, ALL_ROWS, st);
         if (l > 0 || po) {
           gemm_raw(dZe, de, PT(q + "wu"), nullptr, 0, ec, dEc, ec, dEc, ec, rowsE, ec, de, 0, st);  // dE_l += dZe Wu^T
           if (res_e) {
@@ -2260,7 +2300,7 @@ struct Engine : EngineBase {
         DQ_LAUNCH(act_bwd_kernel<T>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, cur, (const T*)t.a[i + 1], act, n);
       const bool b_i = bias && (!last_linear || base[0] != 'J' || i < nl - 1);
       if (b_i) bgrad(cur, dout, rows_, dout, G + off(q + ".b"), st);
-      wgrad(t.a[i], din, cur, dout, rows_, din, dout, G + off(q + ".w"), 0, 0, st);
+      wgrad(t.a[i], din, cur, dout, rows_, din, dout, G + off(q + ".w"), 0, ALL_ROWS, st);
       if (i > 0) {
         T* nxt = (cur == s0) ? s1 : s0;
         gemm_raw(cur, dout, PT(q + ".w"), nullptr, 0, din, nullptr, 0, nxt, din, rows_, din, dout, 0, st);
@@ -2442,7 +2482,7 @@ struct Engine : EngineBase {
         DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nd + 255) / 256)), dim3(256), 0, st, (const T*)dXn, (const T*)X[l + 1],
                   (const T*)(res ? X[l] : nullptr), sc, sr0, nd);
         if (cfg.gnn_g_bias) bgrad(sr0, d, rows, d, G + off(q + "g.b"), st);
-        wgrad(Fc[l], fin, sr0, d, rows, fin, d, G + off(q + "g.w"), 0, 0, st);
+        wgrad(Fc[l], fin, sr0, d, rows, fin, d, G + off(q + "g.w"), 0, ALL_ROWS, st);
         gemm_raw(sr0, d, PT(q + "g.w"), nullptr, 0, fin, nullptr, 0, dFb, fin, rows, fin, d, 0, st);
         // dF -> dX_l (own row + spin means + residual) and dC (the convolution columns); F = [x, mean_up, mean_down, conv_*]
         if (nt != 2) { err = "dqmc_wf_vjp_params: concatenate update with nucleus-electron convolutions not supported"; return 2; }
@@ -2460,7 +2500,7 @@ struct Engine : EngineBase {
           bgrad(sr0, d, rows, d, G + off(q + "g_" + tn[t] + ".b"), st);
           const size_t ne_ = (size_t)rows * e;  // conv_t is a column slice of C: copy it out for the weight gradient
           DQ_LAUNCH(slice_cols_kernel<T>, dim3((unsigned)((ne_ + 255) / 256)), dim3(256), 0, st, (const T*)C[l], nt * e, t * e, e, dCt, ne_);
-          wgrad(dCt, e, sr0, d, rows, e, d, G + off(q + "g_" + tn[t] + ".w"), 0, 0, st);
+          wgrad(dCt, e, sr0, d, rows, e, d, G + off(q + "g_" + tn[t] + ".w"), 0, ALL_ROWS, st);
           gemm_raw(sr0, d, PT(q + "g_" + tn[t] + ".w"), nullptr, 0, e, nullptr, 0, dCb + t * e, nt * e, rows, e, d, 0, st);
         }
       }
@@ -2512,7 +2552,6 @@ struct Engine : EngineBase {
     int64_t Bc = largest_fit(B, wsb, [&](int64_t n) { return vjp_chunk_bytes((int)n, po != nullptr); });
     if (Bc < 1) { err = std::string("workspace too small for a single walker (") + what + ")"; return 3; }
     if (!gnn && cfg.kind != DQMC_FERMINET) {
-      DQ_CHECK(raise_dyn_smem(attn_bwd_kernel<T>, (int)attn_bwd_smem_bytes<T>(N, dh, Mn)));
       // the chunk's forward runs the generic attention with one slot, which fp32 engines on the specialised kernels never
       // opted in at creation (benzene, N = 30, dh = 64: 69 KB)
       DQ_CHECK(raise_dyn_smem(attn_fl_kernel<T>, (int)attn_smem_bytes<T>(N, dh, 1, Mn)));
@@ -3098,6 +3137,20 @@ int dqmc_debug_det_sum(dqmc_handle h, const void* r, const void* R, const void* 
   DQ_NEED_DEVICE(h);
   if (!r || !R || !det_sign || !det_log || !sign || !logp) { h->e->err = "dqmc_debug_det_sum: null array"; return 2; }
   return h->e->debug_det_sum(r, R, det_sign, det_log, det_grad, det_lap, B, S, sign, logp, grad, stats, (cudaStream_t)stream);
+}
+int dqmc_debug_attention_bwd(dqmc_handle h, int32_t layer, const void* QKV, const void* dO, void* dQKV, void* dKn, void* dVn,
+                             int32_t rows, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!QKV || !dO || !dQKV) { h->e->err = "dqmc_debug_attention_bwd: null array"; return 2; }
+  return h->e->debug_attention_bwd(layer, QKV, dO, dQKV, dKn, dVn, rows, (cudaStream_t)stream);
+}
+int dqmc_debug_wgrad(dqmc_handle h, const void* A, const void* dY, int32_t rows, int32_t K, int32_t Nc, int32_t lo, int32_t hi,
+                     void* dW, void* db, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!A || !dY || !dW || !db) { h->e->err = "dqmc_debug_wgrad: null array"; return 2; }
+  return h->e->debug_wgrad(A, dY, rows, K, Nc, lo, hi, dW, db, (cudaStream_t)stream);
 }
 int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n) {
   if (!h) return 2;

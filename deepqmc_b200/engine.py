@@ -854,6 +854,35 @@ class Engine:
         self._check(rc, 'dqmc_debug_det_sum')
         return sign, log, grad, stats
 
+    def debug_attention_bwd(self, layer, QKV, dO):
+        """The softmax attention backward of `layer` (Engine::attention_bwd, the kernel the reverse passes run) on Q | K | V rows
+        [rows, 3d] and output cotangents dO [rows, d] (row b N + i) -> (dQKV [rows, 3d], dKn [Mn, d], dVn [Mn, d]): the last two
+        are the TransPsiformer nuclear tokens' cotangents summed over the walkers, None without nuclear tokens (self-test hook)."""
+        QKV, dO = self._prep(QKV), self._prep(dO)
+        d = self.spec.embedding_dim
+        assert QKV.dim() == 2 and QKV.shape[1] == 3 * d and dO.shape == (QKV.shape[0], d), (tuple(QKV.shape), tuple(dO.shape))
+        dQKV = torch.empty_like(QKV)
+        Mn = self.spec.n_nuc if self.spec.kind == 'transpsiformer' else 0
+        dKn = torch.zeros(Mn, d, dtype=self.dtype, device=self.device) if Mn else None
+        dVn = torch.zeros(Mn, d, dtype=self.dtype, device=self.device) if Mn else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        rc = self.lib.dqmc_debug_attention_bwd(self.h, layer, QKV.data_ptr(), dO.data_ptr(), dQKV.data_ptr(), ptr(dKn), ptr(dVn),
+                                               QKV.shape[0], self._stream())
+        self._check(rc, 'dqmc_debug_attention_bwd')
+        return dQKV, dKn, dVn
+
+    def debug_wgrad(self, A, dY, lo=0, hi=-1):
+        """The reverse passes' weight- and bias-gradient reductions on A [rows, K] and dY [rows, Nc] -> (dW [K, Nc] = A^T dY,
+        db [Nc] = column sums of dY), both over the rows b N + i with lo <= i < hi (hi = -1: every row) (self-test hook)."""
+        A, dY = self._prep(A), self._prep(dY)
+        assert A.dim() == 2 and dY.dim() == 2 and A.shape[0] == dY.shape[0], (tuple(A.shape), tuple(dY.shape))
+        dW = torch.zeros(A.shape[1], dY.shape[1], dtype=self.dtype, device=self.device)
+        db = torch.zeros(dY.shape[1], dtype=self.dtype, device=self.device)
+        rc = self.lib.dqmc_debug_wgrad(self.h, A.data_ptr(), dY.data_ptr(), A.shape[0], A.shape[1], dY.shape[1], lo, hi,
+                                       dW.data_ptr(), db.data_ptr(), self._stream())
+        self._check(rc, 'dqmc_debug_wgrad')
+        return dW, db
+
     TRUNK_PHASES = ('tile_load', 'qkv_mainloop', 'qkv_epilogue', 'attention', 'wo_mainloop', 'wo_epilogue', 'w1_mainloop',
                     'w1_epilogue', 'w2_mainloop', 'w2_epilogue', 'weight_wait', 'mma_turn', 'tile_layer_pairs')
 

@@ -380,6 +380,25 @@ int dqmc_debug_det_sum(dqmc_handle h, const void* r, const void* R, const void* 
                        const void* det_grad, const void* det_lap, int32_t B, int32_t S, void* sign, void* logp, void* grad,
                        void* stats, void* stream);
 
+/* Self-test hook: the softmax attention backward of layer `layer` (plain forward), run by the same Engine::attention_bwd the
+ * parameter and position reverse passes call, on caller-supplied Q | K | V rows QKV [rows][3d] (layout of dqmc_debug_attention
+ * with S = 1) and output cotangents dO [rows][d] -> dQKV [rows][3d] (dQ | dK | dV).  TransPsiformer: the keys and values also
+ * hold the layer's nuclear tokens from the parameter table, and the cotangents of those tokens are ADDED over every walker into
+ * dKn / dVn [Mn][d] (caller-zeroed; not read without nuclear tokens).  Status 2 for kinds without softmax attention, a layer out
+ * of range, rows not a positive multiple of N, or missing dKn / dVn.  reference: the cotangents jax.grad takes through
+ * hk.MultiHeadAttention (gnn/update_features.py:273-280). */
+int dqmc_debug_attention_bwd(dqmc_handle h, int32_t layer, const void* QKV, const void* dO, void* dQKV, void* dKn, void* dVn,
+                             int32_t rows, void* stream);
+
+/* Self-test hook: the weight- and bias-gradient reductions of the reverse passes (Engine::wgrad / Engine::bgrad, the row split
+ * the reverse passes use) on caller-supplied A [rows][K] and dY [rows][Nc]:  dW [K][Nc] += A^T dY and db [Nc] += column sums of
+ * dY, over the rows (b N + i) whose electron i lies in [lo, hi) (N of the handle; the per-spin backflow heads), or over every row
+ * with hi = -1.  An empty range (lo = hi) adds nothing.  dW / db must be zeroed by the caller to read the sums.
+ * Status 2 for rows, K or Nc < 1, or a range outside [0, N].  reference: the parameter cotangents jax.grad takes through
+ * hk.Linear. */
+int dqmc_debug_wgrad(dqmc_handle h, const void* A, const void* dY, int32_t rows, int32_t K, int32_t Nc, int32_t lo, int32_t hi,
+                     void* dW, void* db, void* stream);
+
 /* Measurement aid: the phase timers of the whole-trunk kernel, summed over every launch since the last call, then reset.  On
  * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 13.  out[0..11]: clock64()
  * cycles of the consumer warpgroups in tile load, QKV mainloop, QKV epilogue, attention, Wo mainloop, Wo epilogue, W1

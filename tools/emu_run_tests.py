@@ -16,8 +16,8 @@ The emulator replaces ex2.approx / rcp.approx / redux.sync by exact code: it che
 
 Usage:  python tools/emu_run_tests.py [--lib PATH] [--nobuild] [--asan] test_name[substring] [test_name ...]
         python tools/emu_run_tests.py --all-small          (every test small enough for the emulator, parity files)
-Tests come from test_gpu_parity.py, test_gpu_z_next_rows.py, test_gpu_ecp_cutoff.py, test_gpu_force.py, test_gpu_reverse_chunks.py
-and test_gpu_slater_conformance.py; stacked parametrize marks run
+Tests come from test_gpu_parity.py, test_gpu_z_next_rows.py, test_gpu_ecp_cutoff.py, test_gpu_force.py, test_gpu_reverse_chunks.py,
+test_gpu_reverse_conformance.py and test_gpu_slater_conformance.py; stacked parametrize marks run
 as their cartesian product, and `name[substring]` keeps the cases whose arguments' repr contains the substring.
 """
 import argparse
@@ -109,10 +109,11 @@ def main():
     import test_gpu_force as FC
     import test_gpu_parity as P
     import test_gpu_reverse_chunks as RC
+    import test_gpu_reverse_conformance as RV
     import test_gpu_slater_conformance as SC
     import test_gpu_z_next_rows as Z
 
-    P.DEV = Z.DEV = SC.DEV = EC.DEV = FC.DEV = RC.DEV = 'cpu'
+    P.DEV = Z.DEV = SC.DEV = EC.DEV = FC.DEV = RC.DEV = RV.DEV = 'cpu'
     torch.cuda.synchronize = lambda *args, **kw: None
     names = list(a.names)
     if a.all_small:
@@ -122,7 +123,7 @@ def main():
         name, _, sel = name.partition('[')
         sel = sel.rstrip(']')
         f = (getattr(Z, name, None) or getattr(P, name, None) or getattr(EC, name, None) or getattr(FC, name, None)
-             or getattr(RC, name, None) or getattr(SC, name))
+             or getattr(RC, name, None) or getattr(RV, name, None) or getattr(SC, name))
         wants_tmp = 'tmp_path' in f.__code__.co_varnames[:f.__code__.co_argcount]
         # stacked parametrize marks: the cartesian product of their cases, passed by argument name
         axes = []
