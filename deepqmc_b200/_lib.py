@@ -23,7 +23,7 @@ SYMBOLS = [
     'dqmc_workspace_bytes_min', 'dqmc_debug_plan', 'dqmc_stats_pack', 'dqmc_debug_mlp_block', 'dqmc_debug_trunk',
     'dqmc_profile_end_classes', 'dqmc_debug_trunk_phases', 'dqmc_debug_attention', 'dqmc_debug_mlp',
     'dqmc_debug_slater', 'dqmc_debug_det_sum', 'dqmc_spin', 'dqmc_ecp_forward_count', 'dqmc_wf_grad_positions',
-    'dqmc_force_terms', 'dqmc_ecp_force', 'dqmc_debug_wgrad',
+    'dqmc_force_terms', 'dqmc_ecp_force', 'dqmc_debug_wgrad', 'dqmc_zv_force',
     'dqmc_debug_attention_bwd',
 ]
 
@@ -106,6 +106,7 @@ def load(path: str | None = None) -> C.CDLL:
     lib.dqmc_wf_grad_positions.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, i64, vp]
     lib.dqmc_force_terms.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp]
     lib.dqmc_ecp_force.argtypes = [vp, vp, vp, i32, i32, u64, vp, vp, vp, vp, i64, vp]
+    lib.dqmc_zv_force.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, i64, vp]
     lib.dqmc_set_pseudo_hamiltonian.argtypes = [vp, i32, i32, C.c_double, C.POINTER(C.c_double), C.POINTER(i32)]
     lib.dqmc_launch_count.argtypes = [vp]
     lib.dqmc_launch_count.restype = i64

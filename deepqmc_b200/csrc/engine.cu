@@ -20,6 +20,7 @@
 #include "kernels_trunk.cuh"
 #include "kernels_gnn.cuh"
 #include "kernels_bwd.cuh"
+#include "kernels_zv.cuh"
 #include "attn_mma.cuh"
 #if !defined(DQMC_NO_TCGEN05)
 #include "gemm_wgmma.cuh"
@@ -209,6 +210,8 @@ struct EngineBase {
                           cudaStream_t st) = 0;
   virtual int ecp_force(const void* r, const void* R, int Rb, int B, uint64_t seed, const void* twist, void* bare, void* nl,
                         void* ws, int64_t wsb, cudaStream_t st) = 0;
+  virtual int zv_force(const void* r, const void* R, int Rb, int B, void* zv, void* grad_R, void* ws, int64_t wsb,
+                       cudaStream_t st) = 0;
   virtual int orbitals(const void* r, const void* R, int Rb, int B, void* out, void* ws, int64_t wsb, cudaStream_t st) = 0;
   virtual int set_ph(int n_tab, int n_grid, double r_max, const double* tables, const int32_t* tab_of_nuc) = 0;
   virtual int debug_gemm(const char* wname, const char* bname, const void* A, const void* Res, void* C, int Mr, int S,
@@ -1039,6 +1042,7 @@ struct Engine : EngineBase {
       const int64_t vper = (int64_t)J * N * 12, nb = std::min<int64_t>(B, group_cap(vper));
       return ecp_force_bytes(nb, nb * vper);
     }
+    if (mode == DQMC_MODE_ZV_FORCE) return zv_refusal() ? 0 : zv_chunk_bytes(B);
     if (mode == DQMC_MODE_SPIN) {  // sized for the exact estimator, the larger of the two; no down electrons: no forwards
       const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
       if (!P) return 0;
@@ -1064,6 +1068,7 @@ struct Engine : EngineBase {
       case DQMC_MODE_LANGEVIN: return sweep_bytes(B, true, 1);
       case DQMC_MODE_LOCAL_ENERGY: return std::max<int64_t>(chunk_bytes(1, S), J > 0 ? ecp_bytes(1, 1) : 0);
       case DQMC_MODE_ECP_FORCE: return J > 0 && has_nl_force() ? ecp_force_bytes(1, 1) : 0;
+      case DQMC_MODE_ZV_FORCE: return zv_refusal() ? 0 : zv_chunk_bytes(1);
       case DQMC_MODE_SPIN: {
         const int64_t P = (int64_t)cfg.n_up * cfg.n_down;
         return P ? spin_bytes(1, P, 1) : 0;
@@ -1101,6 +1106,7 @@ struct Engine : EngineBase {
       case DQMC_MODE_ECP_FORCE:
         rc = ecp_force(nullptr, nullptr, 0, B, 0, nullptr, nullptr, has_nl_force() ? ws : nullptr, ws, wsb, nullptr);
         break;
+      case DQMC_MODE_ZV_FORCE: rc = zv_force(nullptr, nullptr, 0, B, nullptr, nullptr, ws, wsb, nullptr); break;
       default: err = "unknown mode"; rc = 2;
     }
     if (carved) *carved = dp.bytes();
@@ -2615,6 +2621,187 @@ struct Engine : EngineBase {
     return 0;
   }
 
+  // ---- AC-ZV force term: nuclear-coordinate companion of the forward-Laplacian pass (kernels_zv.cuh) ----------------
+  // Companion buffers of one chunk of Bc walkers, carved in front of the primal forward chunk (carve()): the companion rows
+  // of the trunk (X, O, QKV and for the Psiformer A, M1) and of the backflow heads, the determinants' companions zl [Bc K],
+  // zg [Bc K T3], zlap [Bc K], and the primal outputs the companion pass reads or finalize_kernel writes (sign, log, E,
+  // stats [6][Bc], grad [Bc T3]).
+  struct ZvWs { T *X, *O, *QKV, *A, *M1, *BF, *zl, *zg, *zlap, *sign, *logp, *E, *stats, *grad; };
+  ZvWs carve_zv(Arena& a, int Bc) const {
+    ZvWs z;
+    const size_t rows = (size_t)Bc * N * (T3 + 2);
+    if (cfg.kind == DQMC_FERMINET) {
+      const size_t dm = fermi_dmax(), fin = 3 * dm + 2 * fermi_emax();
+      z.X = a.take<T>(rows * dm); z.O = a.take<T>(rows * dm); z.QKV = a.take<T>(rows * fin);
+      z.A = z.M1 = nullptr;
+    } else {
+      z.X = a.take<T>(rows * d); z.O = a.take<T>(rows * d); z.QKV = a.take<T>(rows * 3 * d);
+      z.A = a.take<T>(rows * d); z.M1 = a.take<T>(rows * d);
+    }
+    z.BF = a.take<T>(rows * BFW);
+    z.zl = a.take<T>((size_t)Bc * K); z.zg = a.take<T>((size_t)Bc * K * T3); z.zlap = a.take<T>((size_t)Bc * K);
+    z.sign = a.take<T>(Bc); z.logp = a.take<T>(Bc); z.E = a.take<T>(Bc); z.stats = a.take<T>((size_t)6 * Bc);
+    z.grad = a.take<T>((size_t)Bc * T3);
+    return z;
+  }
+  int64_t zv_chunk_bytes(int Bc) const {
+    return prefixed_bytes([&](Arena& a) { carve_zv(a, Bc); }, Bc, T3 + 2);
+  }
+  // why dqmc_zv_force refuses this engine (null: it does not)
+  const char* zv_refusal() const {
+    if (trans) return "the TransPsiformer's nuclear tokens and envelope exponents depend on R through the host-side nuclear stream";
+    if (gnn) return "the conv-GNN kinds have no nuclear companion pass";
+    if (cfg.kind != DQMC_PSIFORMER && cfg.kind != DQMC_FERMINET) return "Psiformer and FermiNet only";
+    if (cfg.backflow_add) return "the additive backflow branch has no nuclear companion pass";
+    if (J > 0 || cfg.ecp_loc_terms > 0) return "effective core potentials are not supported (all-electron only)";
+    if (d_ph_tabs || ph_on) return "pseudo-Hamiltonians are not supported (all-electron only)";
+    return nullptr;
+  }
+
+  // one chunk, one nuclear coordinate kappa = (m, c): the primal forward-Laplacian pass (its dense layers without fused
+  // epilogues, so that every pre-activation is there for its companion rule) and the companion pass beside it.  Writes
+  // zv[b][kappa] (and gR[b][kappa]) with row stride 3 M.
+  int zv_chunk(const T* r, const T* R, int Rb, int Bc, int kappa, const ZvWs& z, Ws& w, T* zv, T* gR, cudaStream_t st) {
+    const int S = T3 + 2, rows = Bc * N * S, m = kappa / 3, c = kappa % 3;
+    const T isq2 = (T)0.70710678118654752440;
+    const dim3 blk(128);
+    T* X;
+    T* Xd;
+    int rc;
+    if (cfg.kind == DQMC_FERMINET) {
+      const int de = cfg.edge_dim, d0 = 4 * M;
+      DQ_LAUNCH(embed_kernel<T>, dim3(Bc * N), blk, sizeof(T) * 5 * d0, st, r, R, Rb, N, M, cfg.n_up, S, 0, 0, (const T*)nullptr,
+                d0, w.X, Bc * N, 1, (const T*)nullptr);
+      DQ_LAUNCH(zv_embed_kernel<T>, dim3(Bc * N), blk, 0, st, r, R, Rb, N, M, S, 0, (const T*)nullptr, d0, z.X, Bc * N, m, c);
+      DQ_LAUNCH(edge_feat_kernel<T>, dim3((Bc * N * N + 127) / 128), blk, 0, st, r, N, S, w.A, Bc * N * N, (const T*)nullptr);
+      T *Hc = w.X, *Hn = w.O, *Ec = w.A, *En = w.M1, *Hcd = z.X, *Hnd = z.O;
+      int dcur = d0, ecur = 4;
+      for (int l = 0; l < cfg.n_layers; ++l) {
+        const std::string p = "F" + std::to_string(l) + ".";
+        const int fin = 3 * dcur + 2 * ecur;
+        const T sc = dcur == d ? isq2 : T(1);
+        DQ_LAUNCH(fermi_agg_kernel<T>, dim3(Bc * S, N), blk, 0, st, (const T*)Hc, dcur, (const T*)Ec, ecur, N, cfg.n_up, S, w.QKV);
+        DQ_LAUNCH(zv_agg_kernel<T>, dim3(Bc * S, N), blk, 0, st, (const T*)Hcd, dcur, ecur, N, cfg.n_up, S, z.QKV);
+        if ((rc = gemm(w.QKV, fin, (p + "wg").c_str(), nullptr, 0, d, P(p + "bg"), nullptr, 0, Hn, d, rows, d, fin, S, 0, N, st)))
+          return rc;
+        if ((rc = gemm(z.QKV, fin, (p + "wg").c_str(), nullptr, 0, d, nullptr, nullptr, 0, Hnd, d, rows, d, fin, S, 0, N, st)))
+          return rc;
+        DQ_LAUNCH(zv_act_kernel<T>, dim3(Bc * N, (d + 127) / 128), blk, 0, st, (const T*)Hn, d, Hnd, d,
+                  (const T*)(dcur == d ? Hcd : nullptr), dcur, S, d, sc, 0);
+        DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, (d + 127) / 128), blk, 0, st, Hn, d, (const T*)(dcur == d ? Hc : nullptr), dcur,
+                  S, d, sc);
+        if (l < cfg.n_layers - 1) {  // the two-particle stream: primal only (its companion is zero)
+          if ((rc = gemm(Ec, ecur, (p + "wu").c_str(), nullptr, 0, de, P(p + "bu"), nullptr, 0, En, de, Bc * N * N * S, de, ecur, S,
+                         0, N, st)))
+            return rc;
+          DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N * N, 1), dim3(32), 0, st, En, de, (const T*)(ecur == de ? Ec : nullptr), ecur,
+                    S, de, ecur == de ? isq2 : T(1));
+          std::swap(Ec, En);
+          ecur = de;
+        }
+        std::swap(Hc, Hn);
+        std::swap(Hcd, Hnd);
+        dcur = d;
+      }
+      X = Hc;
+      Xd = Hcd;
+    } else {
+      DQ_LAUNCH(embed_kernel<T>, dim3(Bc * N), blk, sizeof(T) * 5 * (4 * M + 1), st, r, R, Rb, N, M, cfg.n_up, S, 1, 1,
+                P("emb.w"), d, w.X, Bc * N, 1, (const T*)nullptr);
+      DQ_LAUNCH(zv_embed_kernel<T>, dim3(Bc * N), blk, 0, st, r, R, Rb, N, M, S, 1, P("emb.w"), d, z.X, Bc * N, m, c);
+      T *O = w.O, *Od = z.O;
+      X = w.X;
+      Xd = z.X;
+      const T scale = (T)(1.0 / std::sqrt((double)dh));
+      const int dblk = (d + 127) / 128;
+      for (int l = 0; l < cfg.n_layers; ++l) {
+        const std::string p = "L" + std::to_string(l) + ".";
+        if ((rc = gemm(X, d, (p + "wqkv").c_str(), nullptr, 0, 3 * d, nullptr, nullptr, 0, w.QKV, 3 * d, rows, 3 * d, d, S, 0, N, st)))
+          return rc;
+        if ((rc = gemm(Xd, d, (p + "wqkv").c_str(), nullptr, 0, 3 * d, nullptr, nullptr, 0, z.QKV, 3 * d, rows, 3 * d, d, S, 0, N, st)))
+          return rc;
+        DQ_LAUNCH(zv_attn_kernel<T>, dim3(Bc, H), blk, zv_attn_smem_bytes<T>(N, dh), st, (const T*)w.QKV, (const T*)z.QKV, 3 * d,
+                  Od, d, N, S, dh, d, scale);
+        if ((rc = attention(w.QKV, O, Bc, S, l, st))) return rc;
+        if ((rc = gemm(O, d, (p + "wo").c_str(), nullptr, 0, d, nullptr, X, d, w.A, d, rows, d, d, S, 0, N, st))) return rc;
+        if ((rc = gemm(Od, d, (p + "wo").c_str(), nullptr, 0, d, nullptr, Xd, d, z.A, d, rows, d, d, S, 0, N, st))) return rc;
+        if ((rc = gemm(w.A, d, (p + "w1").c_str(), nullptr, 0, d, P(p + "b1"), nullptr, 0, w.M1, d, rows, d, d, S, 0, N, st)))
+          return rc;
+        if ((rc = gemm(z.A, d, (p + "w1").c_str(), nullptr, 0, d, nullptr, nullptr, 0, z.M1, d, rows, d, d, S, 0, N, st))) return rc;
+        DQ_LAUNCH(zv_act_kernel<T>, dim3(Bc * N, dblk), blk, 0, st, (const T*)w.M1, d, z.M1, d, (const T*)nullptr, 0, S, d, T(1), 0);
+        DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, dblk), blk, 0, st, w.M1, d, (const T*)nullptr, 0, S, d, T(1));
+        if ((rc = gemm(w.M1, d, (p + "w2").c_str(), nullptr, 0, d, P(p + "b2"), nullptr, 0, O, d, rows, d, d, S, 0, N, st))) return rc;
+        if ((rc = gemm(z.M1, d, (p + "w2").c_str(), nullptr, 0, d, nullptr, nullptr, 0, Od, d, rows, d, d, S, 0, N, st))) return rc;
+        DQ_LAUNCH(zv_act_kernel<T>, dim3(Bc * N, dblk), blk, 0, st, (const T*)O, d, Od, d, (const T*)z.A, d, S, d, T(1), 0);
+        DQ_LAUNCH(tanh_fl_kernel<T>, dim3(Bc * N, dblk), blk, 0, st, O, d, (const T*)w.A, d, S, d, T(1));
+        std::swap(X, O);
+        std::swap(Xd, Od);
+      }
+    }
+    // backflow heads (no bias for these kinds), mult_act, determinants, determinant sum
+    if ((rc = gemm(X, bf_in, "bf.up", "bf.dn", cfg.n_up, BFW, nullptr, nullptr, 0, w.BF, BFW, Bc * S, BFW, bf_in, S, 1, N, st)))
+      return rc;
+    if ((rc = gemm(Xd, bf_in, "bf.up", "bf.dn", cfg.n_up, BFW, nullptr, nullptr, 0, z.BF, BFW, Bc * S, BFW, bf_in, S, 1, N, st)))
+      return rc;
+    if (cfg.mult_act == 1)
+      DQ_LAUNCH(zv_act_kernel<T>, dim3(Bc * N, (KN + 127) / 128), blk, 0, st, (const T*)w.BF, KN, z.BF, KN, (const T*)nullptr, 0,
+                S, KN, T(1), 2);
+    if ((rc = slater(r, R, Rb, Bc, S, w.BF, w.Gadd, w.dsign, w.dlog, w.dgrad, w.dlap, st, nullptr, FwdIn{}, 0))) return rc;
+    const int full_det = cfg.factorized_det ? 0 : 1;
+    const int wpb = zv_slater_warps_per_block<T>(N);
+    DQ_LAUNCH(zv_slater_kernel<T>, dim3((Bc * K + wpb - 1) / wpb), dim3(32 * wpb), zv_slater_smem_per_warp<T>(N) * wpb, st, r, R,
+              Rb, N, M, cfg.n_up, K, S, Bc * K, P("env.pi_up"), P("env.pi_dn"), P("env.zeta_up"), P("env.zeta_dn"),
+              (const T*)w.BF, (const T*)z.BF, BFW, z.zl, z.zg, z.zlap, env_rep, full_det, m, c);
+    const FinalizeCfg fc = finalize_cfg(S);
+    const T* nuc = cfg.nuc_cusp_kind ? P("cusp.nuc") : (const T*)nullptr;
+    const T* conf = cfg.conf_linear ? P("conf.w") : (const T*)nullptr;
+    DQ_LAUNCH(finalize_kernel<T>, dim3(Bc), blk, finalize_smem_bytes<T>(N, K), st, fc, r, R, Rb, (const T*)w.dsign,
+              (const T*)w.dlog, (const T*)w.dgrad, (const T*)w.dlap, P("cusp.alpha"), (const T*)d_zval, (const T*)d_ecp_loc,
+              (const int*)d_ecp_mask, Bc, z.sign, z.logp, z.E, z.stats, z.grad, conf, (const T*)nullptr, nuc, PhArgs<T>());
+    DQ_LAUNCH(zv_finalize_kernel<T>, dim3(Bc), blk, zv_finalize_smem_bytes<T>(K), st, N, M, K, S, cfg.nuc_cusp_kind, r, R, Rb,
+              (const T*)w.dsign, (const T*)w.dlog, (const T*)w.dgrad, (const T*)w.dlap, (const T*)z.zl, (const T*)z.zg,
+              (const T*)z.zlap, conf, (const T*)z.grad, nuc, m, c, 3 * M, kappa, zv, gR);
+    return 0;
+  }
+
+  // -dT/dR and (optionally) grad_R log|psi| per walker [B][M][3]: for every chunk and nuclear coordinate one zv_chunk
+  int zv_force(const void* r_, const void* R_, int Rb, int B, void* zv_, void* gR_, void* ws, int64_t wsb,
+               cudaStream_t st) override {
+    if (const char* why = zv_refusal()) { err = std::string("dqmc_zv_force: ") + why; return 2; }
+    if (B == 0) return 0;
+    const size_t s_attn = cfg.kind == DQMC_PSIFORMER ? zv_attn_smem_bytes<T>(N, dh) : 0;
+    const size_t s_sl = zv_slater_smem_per_warp<T>(N) * zv_slater_warps_per_block<T>(N);
+    if (s_attn > 227 * 1024 || s_sl > 227 * 1024) {
+      err = "dqmc_zv_force: system too large for the companion kernels' shared memory (N, head width)";
+      return 2;
+    }
+    int64_t row_cap = kRowCap / ((int64_t)N * (T3 + 2) * 3 * d);
+    if (cfg.kind == DQMC_FERMINET) row_cap = kRowCap / ((int64_t)N * N * (T3 + 2) * (3 * (int64_t)fermi_dmax() + 64));
+    const int Bc = (int)largest_fit(std::min<int64_t>(B, row_cap), wsb, [&](int64_t n) { return zv_chunk_bytes((int)n); });
+    if (Bc < 1) { err = "workspace too small for a single walker"; return 3; }
+    Arena a(this, ws, wsb);
+    const ZvWs z = carve_zv(a, Bc);
+    Ws w = carve(a.top, Bc, T3 + 2);
+    if (dry) return 0;
+    if (s_attn) DQ_CHECK(raise_dyn_smem(zv_attn_kernel<T>, (int)s_attn));
+    DQ_CHECK(raise_dyn_smem(zv_slater_kernel<T>, (int)s_sl));
+    const T* r = (const T*)r_;
+    const T* R = (const T*)R_;
+    T* zv = (T*)zv_;
+    T* gR = (T*)gR_;
+    for (int b0 = 0; b0 < B; b0 += Bc) {
+      const int nb = std::min(Bc, B - b0);
+      for (int kappa = 0; kappa < 3 * M; ++kappa) {
+        int rc = zv_chunk(r + (size_t)b0 * 3 * N, R + (Rb ? (size_t)b0 * 3 * M : 0), Rb, nb, kappa, z, w,
+                          zv + (size_t)b0 * 3 * M, gR ? gR + (size_t)b0 * 3 * M : nullptr, st);
+        if (rc) return rc;
+        if ((rc = check_guards())) return rc;
+      }
+    }
+    DQ_CHECK(cudaGetLastError());
+    return 0;
+  }
+
   int stats_pack(const void* E, const void* stats, int B, double* out, cudaStream_t st) override {
     DQ_LAUNCH(stats_pack_kernel<T>, dim3(1), dim3(1024), 0, st, (const T*)E, (const T*)stats, B, out);
     DQ_CHECK(cudaGetLastError());
@@ -3070,6 +3257,14 @@ int dqmc_ecp_force(dqmc_handle h, const void* r, const void* R, int32_t R_batche
   if (n_walkers > 0 && (!r || !R)) { h->e->err = "dqmc_ecp_force: null array"; return 2; }
   return h->e->ecp_force(r, R, R_batched, n_walkers, seed, ecp_twist, out_bare, out_nl, workspace, workspace_bytes,
                          (cudaStream_t)stream);
+}
+int dqmc_zv_force(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, void* out_zv,
+                  void* out_grad_R, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (n_walkers < 0) { h->e->err = "negative walker count"; return 2; }
+  if (n_walkers > 0 && (!r || !R || !out_zv)) { h->e->err = "dqmc_zv_force: null array"; return 2; }
+  return h->e->zv_force(r, R, R_batched, n_walkers, out_zv, out_grad_R, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 int dqmc_set_pseudo_hamiltonian(dqmc_handle h, int32_t n_tab, int32_t n_grid, double r_max, const double* tables,
                                 const int32_t* tab_of_nuc) {

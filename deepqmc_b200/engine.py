@@ -15,6 +15,7 @@ from . import params as PN
 from .spec import AnsatzSpec
 
 MODE_FORWARD, MODE_LOCAL_ENERGY, MODE_VJP, MODE_MCMC, MODE_LANGEVIN, MODE_SPIN, MODE_GRAD_POS, MODE_ECP_FORCE = 0, 1, 2, 3, 4, 5, 6, 7
+MODE_ZV_FORCE = 8
 _TORCH_DTYPE = {0: torch.float64, 1: torch.float32}
 
 
@@ -653,6 +654,24 @@ class Engine:
                                      ws.numel() if ws is not None else 0, self._stream())
         self._check(rc, 'dqmc_ecp_force')
         return bare, nl
+
+    def zv_force(self, r, R, want_grad_R=False, max_ws_bytes=None):
+        """-> (zv[B, M, 3], grad_R[B, M, 3] or None): the zero-variance term of the AC-ZV / AC-ZVZB force estimators,
+        zv = -dT/dR_kappa at fixed r (T the local kinetic energy), by a nuclear-coordinate companion of the forward-Laplacian
+        pass (dqmc_zv_force; reference force.py:135-169 for an all-electron Hamiltonian); grad_R = grad_R log|psi| from the
+        same pass.  Psiformer and FermiNet with multiplicative backflow, all-electron."""
+        r = self._prep(r)
+        B = r.shape[0]
+        R, Rb = self._R(R, B)
+        mk = lambda *s: torch.empty(*s, dtype=self.dtype, device=self.device)
+        M = self.spec.n_nuc
+        zv = mk(B, M, 3)
+        gR = mk(B, M, 3) if want_grad_R else None
+        ws = self.workspace(B, MODE_ZV_FORCE, max_ws_bytes)
+        rc = self.lib.dqmc_zv_force(self.h, r.data_ptr(), R.data_ptr(), Rb, B, zv.data_ptr(),
+                                    gR.data_ptr() if gR is not None else None, ws.data_ptr(), ws.numel(), self._stream())
+        self._check(rc, 'dqmc_zv_force')
+        return zv, gR
 
     def mcmc_sweep(self, state, R, n_sub, target_acceptance=0.57, max_age=None, seed=0, step0=0, walker_offset=0,
                    noise_normal=None, noise_uniform=None, max_ws_bytes=None, exchange_probability=0.0, exchange_flags=None,

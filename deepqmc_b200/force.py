@@ -14,8 +14,15 @@ and the non-local part -grad_nonloc_potential (``dqmc_ecp_force``; Psiformer and
 (nucleus, electron) pair of a walker shares one quadrature twist, drawn per walker from ``rng`` (the energy pass draws one per
 pair); unlike the reference, nucleus I's non-local force lands in row I, not in row j (its index among the non-local nuclei):
 the two agree when the ECP nuclei come first, as in every molecule the reference ships.  The ZVQ family refuses ECP engines,
-which the reference documents as incompatible.  Not built: AC-ZV / AC-ZVZB (the local energy of the nuclear-JVP wave
-function); see DESIGN.md.
+which the reference documents as incompatible.
+
+AC-ZV and AC-ZVZB take their zero-variance term from the wave function itself: the reference evaluates the local energy
+E'_kappa of psi'_kappa = d psi / dR_kappa and forms -(E'_kappa - E_loc) d_kappa log|psi|.  With an all-electron Hamiltonian
+the potential cancels there, and the term equals -dT/dR_kappa at fixed electron positions (T the local kinetic energy)
+whenever E_loc is the walker's exact local energy, as the reference's monitors pass it.  ``dqmc_zv_force`` computes that
+closed form by a nuclear-coordinate companion of the forward-Laplacian pass (Psiformer and FermiNet with multiplicative
+backflow); it neither divides by d_kappa log|psi| nor reads ``e_loc``.  ECP engines are refused (the reference's E'_kappa
+then contains the non-local operator acting on psi').
 """
 from __future__ import annotations
 
@@ -223,6 +230,46 @@ def evaluate_hf_force_ac_zvqzb(hamil, wf):
         return _unbatch(f, single)
 
     return evaluate_hf_force_ac_zvqzb_
+
+
+def _zv(hamil, eng, r, R, want_grad_R):
+    """(-dT/dR [B, M, 3], grad_R log|psi| or None) of dqmc_zv_force, with the refusals of the AC-ZV family."""
+    spec = eng.spec
+    if spec.kind not in ('psiformer', 'ferminet') or spec.backflow_transform != 'mult':
+        raise ValueError(f'the AC-ZV / AC-ZVZB force estimators are not available for the {spec.kind!r} ansatz kind '
+                         f'(backflow {spec.backflow_transform!r}): Psiformer and FermiNet with multiplicative backflow only')
+    if _has_ecp(hamil) or getattr(hamil, 'ph', None) is not None:
+        raise ValueError(f'the AC-ZV / AC-ZVZB force estimators need an all-electron Hamiltonian (ecp_type '
+                         f'{hamil.ecp_type!r})')
+    return eng.zv_force(r, R, want_grad_R=want_grad_R)
+
+
+def evaluate_hf_force_ac_zv(hamil, wf):
+    """-> f(rng, params, phys_conf, e_loc=None, energy=None) -> bare + f_zv [B, M, 3] (reference force.py:304-355), with
+    f_zv = -dT/dR at fixed r (see the module docstring).  ``e_loc`` and ``energy`` are accepted for the reference's
+    signature; the closed form uses neither."""
+
+    def evaluate_hf_force_ac_zv_(rng, params, phys_conf: PhysicalConfiguration, e_loc=None, energy=None):
+        r, R, single = _batched(phys_conf)
+        eng = _engine(hamil, wf, params)
+        zv, _ = _zv(hamil, eng, r, R, False)
+        return _unbatch(_bare(hamil, eng, rng, r, R) + zv, single)
+
+    return evaluate_hf_force_ac_zv_
+
+
+def evaluate_hf_force_ac_zvzb(hamil, wf):
+    """-> f(rng, params, phys_conf, e_loc, energy) -> bare + f_zv - 2 (E_loc - energy) grad_R log|psi| [B, M, 3]
+    (reference force.py:358-411); grad_R log|psi| comes from the same companion pass as f_zv."""
+
+    def evaluate_hf_force_ac_zvzb_(rng, params, phys_conf: PhysicalConfiguration, e_loc, energy):
+        r, R, single = _batched(phys_conf)
+        eng = _engine(hamil, wf, params)
+        zv, gR = _zv(hamil, eng, r, R, True)
+        f = _bare(hamil, eng, rng, r, R) + zv + _zb_factor(e_loc, energy, gR).reshape(-1, 1, 1) * gR
+        return _unbatch(f, single)
+
+    return evaluate_hf_force_ac_zvzb_
 
 
 def finite_difference_displacements(r, R, step_size):

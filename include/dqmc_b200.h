@@ -31,7 +31,8 @@ enum { DQMC_PSIFORMER = 0, DQMC_FERMINET = 1, DQMC_TRANSPSIFORMER = 2, DQMC_PAUL
 enum { DQMC_F64 = 0, DQMC_F32 = 1 };
 enum { DQMC_GEMM_SIMT = 0, DQMC_GEMM_TCGEN05 = 1 };
 enum { DQMC_MODE_FORWARD = 0, DQMC_MODE_LOCAL_ENERGY = 1, DQMC_MODE_VJP = 2, DQMC_MODE_MCMC = 3, DQMC_MODE_LANGEVIN = 4,
-       DQMC_MODE_SPIN = 5, DQMC_MODE_GRAD_POS = 6, DQMC_MODE_ECP_FORCE = 7 };
+       DQMC_MODE_SPIN = 5, DQMC_MODE_GRAD_POS = 6, DQMC_MODE_ECP_FORCE = 7,
+       DQMC_MODE_ZV_FORCE = 8 };
 
 /* Ansatz + Hamiltonian constants that fix the kernel shapes.
  * reference: src/deepqmc/conf/ansatz/psiformer.yaml, ferminet.yaml (SURVEY.md 8(a0));
@@ -255,6 +256,22 @@ int dqmc_force_terms(dqmc_handle h, const void* r, const void* R, int32_t R_batc
  *           ecp/gaussian_type_ecp.py:257-328 grad_nonloc_potential, ecp/ecp_force_utils.py). */
 int dqmc_ecp_force(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, uint64_t seed,
                    const void* ecp_twist, void* out_bare, void* out_nl, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* Zero-variance term of the AC-ZV / AC-ZVZB force estimators per walker [B][M][3] (device):
+ *   out_zv     = -dT/dR = 1/2 d/dR (Lap_r log|psi| + |grad_r log|psi||^2) at fixed electron positions, T the local kinetic
+ *                energy (stats E_kin of dqmc_local_energy).  With an all-electron Hamiltonian the potential cancels in the
+ *                reference's -(E'_kappa - E_loc) g_kappa (E'_kappa: local energy of d psi / dR_kappa, g_kappa = d log|psi| / dR_kappa)
+ *                when E_loc is the walker's exact local energy; this closed form needs no division by g_kappa and no E_loc.
+ *   out_grad_R = grad_R log|psi| (nullable), the companion of the value slot (equal to dqmc_wf_grad_positions' grad_R).
+ * Each nuclear coordinate runs a forward-Laplacian pass with a companion state dX/dR of every activation beside it
+ * (kernels_zv.cuh).  Psiformer and FermiNet with multiplicative backflow (nuclear cusp included), shared or per-walker R;
+ * the TransPsiformer, the conv-GNN kinds, the additive backflow branch, engines with an effective core potential and
+ * pseudo-Hamiltonians return status 2.  Every sum runs in a fixed order without atomics: a repeated call is bitwise
+ * identical.  n_walkers = 0 is a no-op.  Workspace: dqmc_workspace_bytes(h, B, DQMC_MODE_ZV_FORCE) (walkers are chunked to fit).
+ * replaces: force.py:135-169 make_zv_term_via_jvp (the local energy of the nuclear-JVP wave function, scanned over the 3M
+ *           tangents), used by :304-411 evaluate_hf_force_ac_zv / evaluate_hf_force_ac_zvzb. */
+int dqmc_zv_force(dqmc_handle h, const void* r, const void* R, int32_t R_batched, int32_t n_walkers, void* out_zv,
+                  void* out_grad_R, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* Switch the handle's Hamiltonian to a pseudo-Hamiltonian (fully local replacement of the semi-local ECP):
  * tables[n_tab][2][n_grid] (host, fp64) = r V_loc(r) and r V_L2(r) per tabulated element on the uniform grid
