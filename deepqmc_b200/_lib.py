@@ -24,7 +24,7 @@ SYMBOLS = [
     'dqmc_profile_end_classes', 'dqmc_debug_trunk_phases', 'dqmc_debug_attention', 'dqmc_debug_mlp',
     'dqmc_debug_slater', 'dqmc_debug_det_sum', 'dqmc_spin', 'dqmc_ecp_forward_count', 'dqmc_wf_grad_positions',
     'dqmc_force_terms', 'dqmc_ecp_force', 'dqmc_debug_wgrad', 'dqmc_zv_force',
-    'dqmc_debug_attention_bwd',
+    'dqmc_debug_attention_bwd', 'dqmc_debug_tc_error',
 ]
 
 
@@ -86,6 +86,7 @@ def load(path: str | None = None) -> C.CDLL:
     lib.dqmc_debug_mlp_block.argtypes = [vp, i32, vp, vp, vp, i32, vp]
     lib.dqmc_debug_trunk.argtypes = [vp, vp, vp, i32, vp]
     lib.dqmc_debug_trunk_phases.argtypes = [vp, C.POINTER(u64), i32]
+    lib.dqmc_debug_tc_error.argtypes = [vp, C.POINTER(i32)]
     lib.dqmc_debug_attention.argtypes = [vp, i32, vp, vp, i32, i32, C.POINTER(i32), vp]
     lib.dqmc_debug_mlp.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32, C.POINTER(i32), vp]
     lib.dqmc_debug_slater.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, C.POINTER(i32), vp]

@@ -183,6 +183,7 @@ struct EngineBase {
   virtual int debug_mlp(int layer, int S, const void* O, const void* X, void* Out, void* scratch, int rows, int32_t* path,
                         cudaStream_t st) = 0;
   virtual int debug_trunk_phases(uint64_t* out, int n) = 0;
+  virtual int debug_tc_error(int32_t* flag) = 0;
   virtual int debug_slater(const void* r, const void* R, const void* BF, int rows, int S, void* dsign, void* dlog, void* dgrad,
                            void* dlap, int32_t* kernel, cudaStream_t st) = 0;
   virtual int debug_det_sum(const void* r, const void* R, const void* dsign, const void* dlog, const void* dgrad,
@@ -536,6 +537,7 @@ struct Engine : EngineBase {
   };
   CUtensorMap* d_trunk_maps = nullptr;       // [L][4][2]
   unsigned char* d_trunk_scratch = nullptr;  // n_sms x 384 KB: split K / V and residual rows of a tile
+  int* d_tc_err = nullptr;                     // error word of the whole-trunk and MLP-block kernels (tc::lock_take past its bound)
   unsigned long long* d_trunk_phase = nullptr;  // DQMC_TRUNK_PHASES=1: the whole-trunk kernel's phase timers (tc::kPhases)
   static constexpr float kActScale = 16.f;  // 2^4: |activation| < 4094 representable, absolute floor 2^-29
   std::map<std::string, TcWeight> tcw;
@@ -737,6 +739,8 @@ struct Engine : EngineBase {
       DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<8>, tc::TrSmem::total()));
       DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<16>, tc::TrSmem::total()));
       DQ_CHECK(raise_dyn_smem(tc::trunk_f16_kernel<32>, tc::TrSmem::total()));
+      DQ_CHECK(cudaMalloc((void**)&d_tc_err, sizeof(int)));
+      DQ_CHECK(cudaMemset(d_tc_err, 0, sizeof(int)));
       if (psif && !trans && d == 256 && H == 4 && N <= 32 && cfg.n_layers <= tc::kTrMaxLayers) {
         DQ_CHECK(cudaMalloc((void**)&d_trunk_maps, sizeof(CUtensorMap) * 8 * cfg.n_layers));
         DQ_CHECK(cudaMalloc((void**)&d_trunk_scratch, (size_t)n_sms * tc::kTrScratchPerCta));
@@ -770,6 +774,7 @@ struct Engine : EngineBase {
     if (d_trunk_maps) cudaFree(d_trunk_maps);
     if (d_trunk_scratch) cudaFree(d_trunk_scratch);
     if (d_trunk_phase) cudaFree(d_trunk_phase);
+    if (d_tc_err) cudaFree(d_tc_err);
 #endif
   }
   const T* P(const std::string& n) const { return d_params + off(n); }
@@ -1216,7 +1221,7 @@ struct Engine : EngineBase {
       p.O = O; p.ldo = d; p.X = X; p.ldx = d; p.Out = Out; p.ldout = d; p.b1 = P(pfx + "b1"); p.b2 = P(pfx + "b2");
       p.M = rows; p.d = d; p.a_scale = kActScale;
       p.us0 = 1.f / (kActScale * wo.wscale); p.us1 = 1.f / (kActScale * w1.wscale); p.us2 = 1.f / (kActScale * w2.wscale);
-      p.err_flag = nullptr;
+      p.err_flag = d_tc_err;
       const int MT = (rows + 127) / 128;
       const int grid = MT < n_sms ? MT : n_sms;
 #ifndef DQMC_EMU
@@ -1283,7 +1288,7 @@ struct Engine : EngineBase {
       int np2 = 1;
       while (np2 < N) np2 *= 2;  // walker slot of the tile: electrons rounded up to a power of two (<= 32)
       p.walkers = rows / N; p.N = N; p.L = cfg.n_layers; p.a_scale = kActScale;
-      p.attn_scale = (float)(1.0 / std::sqrt((double)dh)); p.err_flag = nullptr; p.phase = d_trunk_phase;
+      p.attn_scale = (float)(1.0 / std::sqrt((double)dh)); p.err_flag = d_tc_err; p.phase = d_trunk_phase;
       for (int l = 0; l < cfg.n_layers; ++l) {
         const std::string pfx = "L" + std::to_string(l) + ".";
         p.b1[l] = P(pfx + "b1"); p.b2[l] = P(pfx + "b2");
@@ -1324,6 +1329,18 @@ struct Engine : EngineBase {
     if (n < tc::kPhases) { err = "dqmc_debug_trunk_phases: the output holds fewer than the kernel's counters"; return 2; }
     DQ_CHECK(cudaMemcpy(out, d_trunk_phase, sizeof(unsigned long long) * tc::kPhases, cudaMemcpyDeviceToHost));
     DQ_CHECK(cudaMemset(d_trunk_phase, 0, sizeof(unsigned long long) * tc::kPhases));
+    return 0;
+#else
+    err = "this build has no tensor-core backend"; return 2;
+#endif
+  }
+  int debug_tc_error(int32_t* flag) override {
+#if !defined(DQMC_NO_TCGEN05)
+    if (!d_tc_err) { err = "no tensor-core backend in this engine"; return 2; }
+    int v = 0;
+    DQ_CHECK(cudaMemcpy(&v, d_tc_err, sizeof(int), cudaMemcpyDeviceToHost));
+    DQ_CHECK(cudaMemset(d_tc_err, 0, sizeof(int)));
+    *flag = v;
     return 0;
 #else
     err = "this build has no tensor-core backend"; return 2;
@@ -3352,6 +3369,12 @@ int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n) {
   DQ_NEED_DEVICE(h);
   if (!out) { h->e->err = "dqmc_debug_trunk_phases: null output"; return 2; }
   return h->e->debug_trunk_phases(out, n);
+}
+int dqmc_debug_tc_error(dqmc_handle h, int32_t* flag) {
+  if (!h) return 2;
+  DQ_NEED_DEVICE(h);
+  if (!flag) { h->e->err = "dqmc_debug_tc_error: null output"; return 2; }
+  return h->e->debug_tc_error(flag);
 }
 
 int dqmc_profile_begin(dqmc_handle h) {

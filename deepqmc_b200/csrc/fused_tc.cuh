@@ -14,13 +14,15 @@
 //
 // 256 threads = two warpgroups; warpgroup w computes tile rows 64 w .. +63 over all d columns (wgmma m64 n = d, fp32
 // accumulators in registers) and owns those rows from the tile load to the output: its half of the operand buffer, its
-// residual rows, its weight ring.  The two warpgroups never wait for each other except for the MMA token (ping-pong): each
-// runs its own copy of the layer, and one warpgroup's epilogues (and the trunk's attention) run while the other's MMAs
-// keep the tensor cores busy.  Thread 0 of a warpgroup streams the pre-split weight half-planes [d rows x 32 halves] (hi,
-// lo per k-block, two halves each) of the GEMM through the warpgroup's 3-slot ring (TMA, 64-byte swizzle): the slots of the
-// next two k-steps land while the current one is multiplied.  A warpgroup takes the token before the first MMA of a GEMM
-// (of the trunk's whole QKV projection: its three column blocks have epilogues much shorter than a GEMM) and hands it to
-// the other after issuing the last one, so the two warpgroups' GEMMs alternate on the tensor cores.
+// residual rows, its weight ring.  The two warpgroups never wait for each other except for the tensor-core lock
+// (ping-pong): each runs its own copy of the layer, and one warpgroup's epilogues (and the trunk's attention) run while the
+// other's MMAs keep the tensor cores busy.  Thread 0 of a warpgroup streams the pre-split weight half-planes [d rows x 32
+// halves] (hi, lo per k-block, two halves each) through the warpgroup's 3-slot ring (TMA, 64-byte swizzle): the slots of
+// the next two k-steps land while the current one is multiplied.  The ring runs along one stream of slots per warpgroup
+// across GEMM boundaries (WeightStream): the last k-steps of a GEMM load the first slots of the warpgroup's next GEMM, so
+// they land during the epilogue in between.  A warpgroup takes the lock before the first MMA of a GEMM (each of the
+// trunk's three QKV column blocks is a GEMM of its own) and releases it after issuing the last one; whichever warpgroup
+// asks first gets the tensor cores next, so neither waits on a fixed turn order.
 // shared memory: operand buffer 4 k-blocks x {hi, lo} x 16 KB = 128 KB, weight rings 2 x 3 x 16 KB, barriers (224 KB).
 #pragma once
 #include <cstdint>
@@ -47,30 +49,54 @@ struct MlpParams {
 struct MlpSmem {
   static __host__ __device__ int abuf(int kb, int plane) { return (kb * 2 + plane) * 16384; }   // [128 rows][128 B]
   static __host__ __device__ int wring(int wg, int s) { return 131072 + (wg * kMlpSlots + s) * 16384; }  // [<= 256 rows][64 B]
-  static __host__ __device__ int bars() { return 131072 + 2 * kMlpSlots * 16384; }  // full [2][kMlpSlots], token [2]
+  static __host__ __device__ int bars() { return 131072 + 2 * kMlpSlots * 16384; }  // full [2][kMlpSlots], lock word
   static __host__ __device__ int phases() { return bars() + 64; }                                 // [2][16] u64
   static __host__ __device__ int total() { return phases() + 2 * 8 * 16; }
 };
-// mbarriers: slot s of warpgroup wg's ring landed (TMA tx); the MMA token of warpgroup wg (arrived by the other one)
+// mbarriers: slot s of warpgroup wg's ring landed (TMA tx)
 __device__ __forceinline__ uint64_t* ring_full(unsigned char* smem, int wg) {
   return (uint64_t*)(smem + MlpSmem::bars()) + wg * kMlpSlots;
 }
-__device__ __forceinline__ uint64_t* mma_token(unsigned char* smem, int wg) {
-  return (uint64_t*)(smem + MlpSmem::bars()) + 2 * kMlpSlots + wg;
+// the CTA's tensor-core lock: 0 free, 1 + w held by warpgroup w
+__device__ __forceinline__ uint32_t* mma_lock(unsigned char* smem) {
+  return (uint32_t*)((uint64_t*)(smem + MlpSmem::bars()) + 2 * kMlpSlots);
 }
-// Kernel prologue (thread 0 with the CTA barrier after it): the barriers of both rings and both tokens.
+static_assert(2 * kMlpSlots * 8 + 4 <= 64, "the ring barriers and the lock word fit below MlpSmem::phases()");
+// Kernel prologue (thread 0 with the CTA barrier after it): the barriers of both rings, the lock free.
 __device__ __forceinline__ void init_rings(unsigned char* smem) {
-  for (int i = 0; i < 2 * kMlpSlots + 2; ++i) mbar_init((uint64_t*)(smem + MlpSmem::bars()) + i, 1);
+  for (int i = 0; i < 2 * kMlpSlots; ++i) mbar_init((uint64_t*)(smem + MlpSmem::bars()) + i, 1);
+  *mma_lock(smem) = 0u;
   fence_barrier_init();
 }
-// After that CTA barrier: warpgroup 0 holds the token for the first GEMM.
-__device__ __forceinline__ void start_pingpong(unsigned char* smem) {
-  if (threadIdx.x == 128) mbar_arrive(mma_token(smem, 0));
+
+// Taken by the leader of warpgroup wg before the first MMA of a GEMM (then wg_sync releases the other 127 threads): a
+// shared-memory CAS, retried after a short sleep, since the spinning warp shares its SM sub-partition with an epilogue warp
+// of the other warpgroup and must leave it the issue slots.  Bounded like mbar_wait, but nothing the warpgroups compute
+// depends on the lock (their rows, accumulators and rings are disjoint; it only orders their MMAs on the tensor cores), so
+// on timeout the error flag is set and the warpgroup goes on without it.
+constexpr unsigned kLockSleepNs = 64;
+__device__ __forceinline__ void lock_take(unsigned char* smem, int wg, int* err) {
+  const uint32_t a = smem_u32(mma_lock(smem)), me = 1u + (uint32_t)wg;
+  if (smem_cas_acquire(a, 0u, me) == 0u) return;
+  const long long t0 = clock64();
+  while (true) {
+    __nanosleep(kLockSleepNs);
+    if (smem_cas_acquire(a, 0u, me) == 0u) return;
+    if (clock64() - t0 > 4000000000LL) {
+      if (err) atomicExch(err, 1);
+      return;
+    }
+  }
+}
+// By the same leader right after issuing the last MMA of the GEMM (release: no MMA issue moves below it).  Only a lock
+// this warpgroup holds is released.
+__device__ __forceinline__ void lock_release(unsigned char* smem, int wg) {
+  smem_cas_release(smem_u32(mma_lock(smem)), 1u + (uint32_t)wg, 0u);
 }
 
 // Phase timers of the whole-trunk kernel (TrunkParams::phase): clock64() cycles summed over the consumer warpgroups of all
-// CTAs, in this order; kPhWait (waiting for weight slots to land) and kPhTurn (waiting for the other warpgroup to hand over
-// the MMA token) are not part of the mainloop phases.
+// CTAs, in this order; kPhWait (waiting for weight slots to land) and kPhTurn (waiting for the tensor-core lock while the
+// other warpgroup's MMAs are issued) are not part of the mainloop phases.
 enum Phase {
   kPhLoad, kPhQkv, kPhQkvEpi, kPhAttn, kPhWo, kPhWoEpi, kPhW1, kPhW1Epi, kPhW2, kPhW2Epi, kPhWait, kPhTurn, kPhPairs, kPhases
 };
@@ -140,47 +166,94 @@ __device__ __forceinline__ void store_operand_quad(unsigned char* smem, int row,
   *(uint2*)(smem + MlpSmem::abuf(kb, 1) + off) = make_uint2(l01, l23);
 }
 
-// Per-warpgroup pipeline state: ring slots used so far (slot g lives in ring stage g % 3 and completes phase (g / 3) & 1 of
-// its barrier) and MMA tokens taken so far (token u completes phase u & 1 of the warpgroup's token barrier).
+// Per-warpgroup pipeline state: ring slots used so far (slot g of the warpgroup's weight stream lives in ring stage g % 3 and
+// completes phase (g / 3) & 1 of its barrier).
 struct Ring {
-  uint32_t nslot = 0, nturn = 0;
+  uint32_t nslot = 0;
 };
-// What a GEMM does with the MMA token: take it before its first MMA, pass it to the other warpgroup after its last.  A run of
-// GEMMs with short epilogues in between (the three column blocks of the QKV projection) holds the token throughout.
-enum Turn { kTurnTake = 1, kTurnPass = 2, kTurnOwn = kTurnTake | kTurnPass, kTurnKeep = 0 };
+// What a GEMM does with the tensor-core lock: take it before its first MMA, release it after its last.  A run of GEMMs may
+// hold it throughout (take, keep, ..., release); the kernels take and release it per GEMM (kTurnOwn).
+enum Turn { kTurnTake = 1, kTurnRelease = 2, kTurnOwn = kTurnTake | kTurnRelease, kTurnKeep = 0 };
 
-// acc = (this warpgroup's 64 operand rows, K = D) x (rows y0 .. y0 + D - 1 of W^T), hi / lo half-planes through the
-// warpgroup's 3-slot weight ring.  Called by the 128 threads of a warpgroup with its operand rows complete (fenced +
-// wg_sync); returns with every MMA retired and the ring free.
+// One GEMM's weights: the hi / lo half-plane maps of W^T and the first W^T row of its column block (hi == nullptr: none).
+struct WTile {
+  const CUtensorMap* hi;
+  const CUtensorMap* lo;
+  int y0;
+};
+// The weight stream of a warpgroup: every GEMM it runs, in order.  For each of the CTA's tiles (blockIdx.x, + gridDim.x,
+// ... < MT) and each of its L layers, the G = Maps::G GEMMs Maps::at(l, g), g = 0 .. G - 1.  A GEMM loads the first slots of
+// the next one (after()), and the stream ends with the last GEMM the CTA runs: no slot is loaded that no GEMM consumes, so
+// no TMA is in flight when the CTA exits.
+template <class Maps>
+struct WeightStream {
+  Maps maps;
+  int L, MT;
+  __device__ __forceinline__ WTile after(int tile, int l, int g) const {
+    if (++g == Maps::G) {
+      g = 0;
+      if (++l == L) {
+        l = 0;
+        tile += gridDim.x;
+      }
+    }
+    return tile < MT ? maps.at(l, g) : WTile{nullptr, nullptr, 0};
+  }
+};
+
+// TMA of slot i of a GEMM's weights (k-steps 2 (i % 2) .. +1 of plane (i / 2) % 2 (hi, lo) of k-block i / 4) into stage st of
+// warpgroup wg's ring
+template <int D>
+__device__ __forceinline__ void load_slot(unsigned char* smem, int wg, int st, const WTile& w, int i) {
+  uint64_t* full = ring_full(smem, wg) + st;
+  mbar_expect_tx(full, D * 64u);
+  tma_load_2d(((i >> 1) & 1) ? w.lo : w.hi, full, smem + MlpSmem::wring(wg, st), (i >> 2) * 64 + (i & 1) * 32, w.y0);
+}
+// Kernel prologue, after the CTA barrier that follows init_rings: the first kMlpSlots slots of the warpgroup's stream (GEMM
+// 0 of layer 0 of tile blockIdx.x).  Ring::nslot starts at 0.
+template <int D, class Maps>
+__device__ __forceinline__ void stream_start(unsigned char* smem, const WeightStream<Maps>& ws) {
+  if ((threadIdx.x & 127) == 0 && (int)blockIdx.x < ws.MT) {
+    const WTile w = ws.maps.at(0, 0);
+    for (int i = 0; i < kMlpSlots; ++i) load_slot<D>(smem, threadIdx.x >> 7, i, w, i);
+  }
+}
+
+// acc = (this warpgroup's 64 operand rows, K = D) x (rows y0 .. y0 + D - 1 of W^T) for GEMM g of layer l of tile `tile` of
+// the warpgroup's weight stream, hi / lo half-planes through its 3-slot ring.  Called by the 128 threads of a warpgroup with
+// its operand rows complete (fenced + wg_sync) and the first kMlpSlots slots of the GEMM loaded (stream_start or the GEMM
+// before); returns with every MMA retired and the first kMlpSlots slots of the next GEMM loaded.
 //
 // The MMAs run in the same order as with whole 64-half planes (per k-block: lo A x hi W and hi A x hi W for k-steps 0 .. 3,
 // then hi A x lo W for k-steps 0 .. 3), so every output element sums the same products in the same order.
-template <int D>
-__device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const CUtensorMap* mh,
-                                          const CUtensorMap* ml, int y0, int turn, int* err, PhaseClock& pc) {
+template <int D, class Maps>
+__device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const WeightStream<Maps>& ws,
+                                          int tile, int l, int g, int turn, int* err, PhaseClock& pc) {
   uint32_t& nslot = ring.nslot;
   constexpr int KB = D / 64;
-  constexpr int NS = 4 * KB;  // slots of this GEMM: slot i = k-steps 2 (i % 2) .. +1 of plane (i / 2) % 2 (hi, lo) of k-block i / 4
-  static_assert(NS >= kMlpSlots, "the ring is filled at the start of a GEMM");
-  constexpr uint32_t kSlot = D * 64u;
+  constexpr int NS = 4 * KB;  // slots of this GEMM
+  static_assert(NS >= kMlpSlots, "a GEMM has at least as many slots as the ring has stages");
   const int wg = threadIdx.x >> 7;
   const bool leader = (threadIdx.x & 127) == 0;
   uint64_t* full = ring_full(smem, wg);
+  const WTile cur = ws.maps.at(l, g), nxt = ws.after(tile, l, g);
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) acc[i] = 0.f;  // the previous contents are dead: registers free between GEMMs
+  // stage of slot i of this GEMM; i >= NS: slot i - NS of the next one
   auto stage = [&](int i) { return (int)((nslot + (uint32_t)i) % (uint32_t)kMlpSlots); };
-  auto load = [&](int i) {
-    const int st = stage(i);
-    mbar_expect_tx(&full[st], kSlot);
-    tma_load_2d(((i >> 1) & 1) ? ml : mh, &full[st], smem + MlpSmem::wring(wg, st), (i >> 2) * 64 + (i & 1) * 32, y0);
-  };
-  if (leader)
-    for (int i = 0; i < kMlpSlots; ++i) load(i);
-  // the first slots land while this warpgroup waits for the token
+  // the lock is asked for once the first slot has landed: a warpgroup never holds the tensor cores while it waits for L2.
+  // (This wait, bounded by a trap like every ring wait, also keeps ptxas from serialising the GEMM's wgmmas behind the
+  // lock's divergent spin loop.)
   if (turn & kTurnTake) {
-    const long long t0 = pc.acc ? clock64() : 0;
-    mbar_wait(mma_token(smem, wg), ring.nturn & 1u, err);
-    ++ring.nturn;
+    long long t0 = pc.acc ? clock64() : 0;
+    if (leader) mbar_wait(&full[stage(0)], (nslot / (uint32_t)kMlpSlots) & 1u, err);
+    if (pc.acc) {
+      const long long t1 = clock64();
+      pc.waited(t1 - t0, kPhWait);
+      t0 = t1;
+    }
+    if (leader) lock_take(smem, wg, err);
+    wg_sync(wg);
     if (pc.acc) pc.waited(clock64() - t0, kPhTurn);
   }
   // waits for slot i and returns its shared-memory address
@@ -192,12 +265,16 @@ __device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* sm
     return smem_u32(smem + MlpSmem::wring(wg, st));
   };
   // slot i's MMAs were just committed: once the previous slot's have retired in every warp of the warpgroup, its stage takes
-  // slot i + 2
-  auto retire = [&](int i) {
+  // slot i + 2, of this GEMM or (only after a lo-plane slot, `cross`) of the next one
+  auto retire = [&](int i, bool cross) {
     wgmma_wait1();
     if (i == 0) return;
     wg_sync(wg);
-    if (leader && i + kMlpSlots - 1 < NS) load(i + kMlpSlots - 1);
+    const int s = i + kMlpSlots - 1;
+    const bool own = !cross || s < NS;
+    if (leader && (own || nxt.hi))
+      load_slot<D>(smem, wg, stage(s), WTile{own ? cur.hi : nxt.hi, own ? cur.lo : nxt.lo, own ? cur.y0 : nxt.y0},
+                   own ? s : s - NS);
   };
   auto mma = [&](float (&d)[D / 2], uint32_t a, uint32_t w, int accumulate) {
     if constexpr (D == 256) wgmma_f16_n256(d, make_desc(a), make_desc64(w), accumulate);
@@ -219,7 +296,7 @@ __device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* sm
         mma(acc, ah + 32 * k, w + 32 * kk, 1);
       }
       wgmma_commit();
-      retire(4 * kb + q);
+      retire(4 * kb + q, false);
     }
 #pragma unroll
     for (int q = 0; q < 2; ++q) {  // lo plane
@@ -228,14 +305,15 @@ __device__ __forceinline__ void gemm_abuf(float (&acc)[D / 2], unsigned char* sm
 #pragma unroll
       for (int kk = 0; kk < 2; ++kk) mma(acc, ah + 32 * (2 * q + kk), w + 32 * kk, 1);
       wgmma_commit();
-      retire(4 * kb + 2 + q);
+      retire(4 * kb + 2 + q, true);
     }
   }
-  // every MMA of the GEMM is issued: the other warpgroup's GEMM queues behind them
-  if ((turn & kTurnPass) && leader) mbar_arrive(mma_token(smem, wg ^ 1));
+  // every MMA of the GEMM is issued: the other warpgroup's GEMM may queue behind them
+  if ((turn & kTurnRelease) && leader) lock_release(smem, wg);
   wgmma_wait0();
   fence_acc(acc);
-  wg_sync(wg);  // the last slots are retired in every warp: the next GEMM may refill their stages
+  wg_sync(wg);  // the last slot is retired in every warp: its stage takes the next GEMM's third slot
+  if (leader && nxt.hi) load_slot<D>(smem, wg, stage(NS + kMlpSlots - 1), nxt, kMlpSlots - 1);
   nslot += NS;
 }
 
@@ -315,19 +393,18 @@ __device__ __forceinline__ void mlp_epilogue(float (&acc)[D / 2], unsigned char*
 // The three GEMMs of the MLP block with their epilogues, run by one warpgroup on its 64 rows, its operand rows holding O
 // (scaled, split) on entry.  Per fragment row h (tile rows fr, fr + 8): xin[h] residual X (nullptr: zero), aout[h] where A is
 // parked (nullptr: row not stored), xout[h] where X' goes (nullptr: not stored); operand_out: X' also becomes the operand
-// rows (next layer of the trunk).  wmaps: (Wo, W1, W2) x (hi, lo) tensor maps; b1, b2: the biases in global memory (read
-// through the read-only cache).  One call site of the GEMM for all three (a rolled loop): the kernel's code stays small.
-template <int D>
-__device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const CUtensorMap* const (&wmaps)[6],
-                                     float us0, float us1, float us2, float a_scale, const float* b1, const float* b2,
-                                     const float* const (&xin)[2], float* const (&aout)[2], float* const (&xout)[2],
-                                     bool operand_out, int* err, PhaseClock& pc) {
+// rows (next layer of the trunk).  Wo, W1, W2 are the last three GEMMs of layer l of tile `tile` in the weight stream ws;
+// b1, b2: the biases in global memory (read through the read-only cache).  One call site of the GEMM for all three (a rolled
+// loop): the kernel's code stays small.
+template <int D, class Maps>
+__device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, Ring& ring, const WeightStream<Maps>& ws,
+                                     int tile, int l, float us0, float us1, float us2, float a_scale, const float* b1,
+                                     const float* b2, const float* const (&xin)[2], float* const (&aout)[2],
+                                     float* const (&xout)[2], bool operand_out, int* err, PhaseClock& pc) {
   const int wg = threadIdx.x >> 7;
 #pragma unroll 1
   for (int g = 0; g < 3; ++g) {
-    const CUtensorMap* mh = g == 0 ? wmaps[0] : (g == 1 ? wmaps[2] : wmaps[4]);
-    const CUtensorMap* ml = g == 0 ? wmaps[1] : (g == 1 ? wmaps[3] : wmaps[5]);
-    gemm_abuf<D>(acc, smem, ring, mh, ml, 0, kTurnOwn, err, pc);
+    gemm_abuf<D>(acc, smem, ring, ws, tile, l, Maps::G - 3 + g, kTurnOwn, err, pc);
     pc.mark(kPhWo + 2 * g);
     if (g == 0) {  // ---- A = X + O Wo -> parked rows and the operand buffer
       mlp_epilogue<D, kEpiWo>(acc, smem, us0, nullptr, a_scale, xin, aout, true);
@@ -347,6 +424,15 @@ __device__ __forceinline__ void mlp3(float (&acc)[D / 2], unsigned char* smem, R
   }
 }
 
+// The MLP block's weight stream: per tile Wo, W1, W2
+struct MlpMaps {
+  static constexpr int G = 3;
+  const CUtensorMap *wo_hi, *wo_lo, *w1_hi, *w1_lo, *w2_hi, *w2_lo;
+  __device__ __forceinline__ WTile at(int, int g) const {
+    return g == 0 ? WTile{wo_hi, wo_lo, 0} : (g == 1 ? WTile{w1_hi, w1_lo, 0} : WTile{w2_hi, w2_lo, 0});
+  }
+};
+
 template <int D>
 __global__ void __launch_bounds__(kMlpThreads, 1)
 mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_constant__ CUtensorMap wo_lo,
@@ -356,6 +442,7 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
   if ((smem_u32(smem) & 1023u) != 0u) tc_trap();
   const int tid = threadIdx.x, wg = tid >> 7;
   const int MT = (p.M + 127) / 128;
+  const WeightStream<MlpMaps> ws{MlpMaps{&wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo}, 1, MT};
 
   if (tid == 0) {
     init_rings(smem);
@@ -363,13 +450,13 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
     tma_prefetch_desc(&w1_lo); tma_prefetch_desc(&w2_hi); tma_prefetch_desc(&w2_lo);
   }
   __syncthreads();
-  start_pingpong(smem);
+  stream_start<D>(smem, ws);
   const Frag f;
   Ring ring;
   float acc[D / 2];
   PhaseClock pc(nullptr);
-  // Both warpgroups run every tile of the CTA (a warpgroup without valid rows computes on zeros and stores nothing), so
-  // they take the MMA token equally often.
+  // Both warpgroups run every tile of the CTA (a warpgroup without valid rows computes on zeros and stores nothing): each
+  // runs the GEMMs its weight stream counts.
   for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
     // ---- stage this warpgroup's 64 rows of the O tile: coalesced float4 loads, hi / lo split
     for (int idx = tid & 127; idx < 64 * (D / 4); idx += 128) {
@@ -391,8 +478,7 @@ mlp_block_f16_kernel(const __grid_constant__ CUtensorMap wo_hi, const __grid_con
       xin[h] = valid ? p.X + (size_t)grow * p.ldx : nullptr;
       aout[h] = valid ? p.Out + (size_t)grow * p.ldout : nullptr;
     }
-    const CUtensorMap* const wmaps[6] = {&wo_hi, &wo_lo, &w1_hi, &w1_lo, &w2_hi, &w2_lo};
-    mlp3<D>(acc, smem, ring, wmaps, p.us0, p.us1, p.us2, p.a_scale, p.b1, p.b2, xin, aout, aout, false, p.err_flag, pc);
+    mlp3<D>(acc, smem, ring, ws, tile, 0, p.us0, p.us1, p.us2, p.a_scale, p.b1, p.b2, xin, aout, aout, false, p.err_flag, pc);
   }
 }
 

@@ -43,6 +43,17 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* e
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// compare-and-swap of a 32-bit shared-memory word, CTA scope, acquire / release; returns the old value
+__device__ __forceinline__ uint32_t smem_cas_acquire(uint32_t saddr, uint32_t cmp, uint32_t val) {
+  uint32_t old;
+  asm volatile("atom.acquire.cta.shared::cta.cas.b32 %0, [%1], %2, %3;" : "=r"(old) : "r"(saddr), "r"(cmp), "r"(val) : "memory");
+  return old;
+}
+__device__ __forceinline__ uint32_t smem_cas_release(uint32_t saddr, uint32_t cmp, uint32_t val) {
+  uint32_t old;
+  asm volatile("atom.release.cta.shared::cta.cas.b32 %0, [%1], %2, %3;" : "=r"(old) : "r"(saddr), "r"(cmp), "r"(val) : "memory");
+  return old;
+}
 // barrier of the 128 threads of one warpgroup (named barrier id = 1 + warpgroup; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }

@@ -65,6 +65,17 @@ struct TrunkParams {
   unsigned long long* phase;     // kPhases cycle / pair counters (fused_tc.cuh Phase), accumulated; nullptr: timers off
 };
 
+// The trunk's weight stream: per layer the K, V, Q column blocks of Wqkv (W^T rows 256, 512, 0), then Wo, W1, W2; maps
+// [L][4][2] as TrunkParams::maps
+struct TrunkMaps {
+  static constexpr int G = 6;
+  const CUtensorMap* maps;
+  __device__ __forceinline__ WTile at(int l, int g) const {
+    const CUtensorMap* m = maps + 8 * l + 2 * (g < 3 ? 0 : g - 2);
+    return WTile{m, m + 1, g < 2 ? 256 * (g + 1) : 0};
+  }
+};
+
 // NP: the walker slot (electrons rounded up to a power of two, <= 32), one instance each: an instance carries only the
 // attention variant of its slot size.
 template <int NP>
@@ -89,8 +100,9 @@ trunk_f16_kernel(TrunkParams p) {
   }
   unsigned long long* ph = (unsigned long long*)(smem + TrSmem::phases());
   if (tid < 32) ph[tid] = 0ull;
+  const WeightStream<TrunkMaps> ws{TrunkMaps{p.maps}, L, MT};
   __syncthreads();
-  start_pingpong(smem);
+  stream_start<256>(smem, ws);
   PhaseClock pc(p.phase && (tid & 127) == 0 ? ph + 16 * wg : nullptr);
   const Frag f;
   Ring ring;
@@ -99,9 +111,10 @@ trunk_f16_kernel(TrunkParams p) {
   // the warpgroup's 64 rows: a walker slot is at most 32 rows and aligned)
   const int lane = tid & 31, r0 = 16 * (tid >> 5), ag = lane >> 2;
   const int k0 = r0 & ~((NP > 16 ? NP : 16) - 1);
-  // From here on the warpgroups only meet at the MMA token: warpgroup w owns tile rows 64 w .. +63 (operand rows, residual
-  // and Q / K / V scratch rows, attention keys) and synchronises its own 128 threads.  Both run every tile and layer of the
-  // CTA (a warpgroup without walkers computes on zero rows and stores nothing), so they take the token equally often.
+  // From here on the warpgroups only meet at the tensor-core lock: warpgroup w owns tile rows 64 w .. +63 (operand rows,
+  // residual and Q / K / V scratch rows, attention keys, weight ring) and synchronises its own 128 threads.  Both run every
+  // tile and layer of the CTA (a warpgroup without walkers computes on zero rows and stores nothing): each runs the GEMMs its
+  // weight stream counts.
   for (int tile = blockIdx.x; tile < MT; tile += gridDim.x) {
     // global row of tile row r (-1: padding row or walker past the end)
     auto grow_of = [&](int r) -> long long {
@@ -153,14 +166,12 @@ trunk_f16_kernel(TrunkParams p) {
     pc.mark(kPhLoad);
     for (int l = 0; l < L; ++l) {
       const bool last = l == L - 1;
-      const CUtensorMap* lm = p.maps + 8 * l;
       // ---- K | V | Q = X Wqkv, 256 columns at a time, split for the attention
 #pragma unroll 1
       for (int j = 0; j < 3; ++j) {
         const int blk = j == 2 ? 0 : j + 1;  // column block: K, V, then Q (its epilogue overwrites the operand X)
-        // one MMA token for the three column blocks: their epilogues are much shorter than a GEMM
-        const int turn = j == 0 ? kTurnTake : (j == 2 ? kTurnPass : kTurnKeep);
-        gemm_abuf<256>(acc, smem, ring, lm, lm + 1, 256 * blk, turn, p.err_flag, pc);
+        // one hold of the tensor-core lock per column block: the other warpgroup's MMAs may run under the K and V epilogues
+        gemm_abuf<256>(acc, smem, ring, ws, tile, l, j, kTurnOwn, p.err_flag, pc);
         pc.mark(kPhQkv);
         const float us = p.us[l][0];
         const int odd = ag & 1;  // fragment rows fr, fr + 8 have the parity of ag
@@ -252,9 +263,8 @@ trunk_f16_kernel(TrunkParams p) {
         const long long row = grow_of(r);
         xout[h] = !last ? resid + r * 256 : (row >= 0 ? p.Out + (size_t)row * p.ldout : nullptr);
       }
-      const CUtensorMap* const wmaps[6] = {lm + 2, lm + 3, lm + 4, lm + 5, lm + 6, lm + 7};
-      mlp3<256>(acc, smem, ring, wmaps, p.us[l][1], p.us[l][2], p.us[l][3], p.a_scale, p.b1[l], p.b2[l], xin, aout, xout,
-                !last, p.err_flag, pc);
+      mlp3<256>(acc, smem, ring, ws, tile, l, p.us[l][1], p.us[l][2], p.us[l][3], p.a_scale, p.b1[l], p.b2[l], xin, aout,
+                xout, !last, p.err_flag, pc);
       fence_proxy_async();
       wg_sync(wg);  // next layer's operand rows complete / next tile's load may overwrite the residual rows
       pc.mark(kPhW2Epi);

@@ -913,6 +913,13 @@ class Engine:
         self._check(rc, 'dqmc_debug_trunk_phases')
         return dict(zip(self.TRUNK_PHASES, out))
 
+    def debug_tc_error(self):
+        """The error word of the whole-trunk and fused MLP-block kernels since creation or the last call (0: none), then reset;
+        synchronous."""
+        flag = C.c_int32()
+        self._check(self.lib.dqmc_debug_tc_error(self.h, C.byref(flag)), 'dqmc_debug_tc_error')
+        return flag.value
+
     def profile_begin(self):
         self.lib.dqmc_profile_begin(self.h)
 

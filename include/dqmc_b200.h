@@ -419,9 +419,14 @@ int dqmc_debug_wgrad(dqmc_handle h, const void* A, const void* dY, int32_t rows,
 /* Measurement aid: the phase timers of the whole-trunk kernel, summed over every launch since the last call, then reset.  On
  * only for an engine created with DQMC_TRUNK_PHASES=1 in the environment (status 2 otherwise); n >= 13.  out[0..11]: clock64()
  * cycles of the consumer warpgroups in tile load, QKV mainloop, QKV epilogue, attention, Wo mainloop, Wo epilogue, W1
- * mainloop, W1 epilogue, W2 mainloop, W2 epilogue, waiting for weight slots (not part of the mainloops), waiting for the MMA
- * token; out[12]: the number of (tile, layer) pairs processed. */
+ * mainloop, W1 epilogue, W2 mainloop, W2 epilogue, waiting for weight slots (not part of the mainloops), waiting for the
+ * tensor-core lock; out[12]: the number of (tile, layer) pairs processed. */
 int dqmc_debug_trunk_phases(dqmc_handle h, uint64_t* out, int32_t n);
+
+/* Self-test hook: the error word of the whole-trunk and fused MLP-block kernels since the engine was created or the last
+ * call (synchronous), then reset; *flag = 0: no error.  A kernel sets it when a wait passes its bound (the tensor-core lock:
+ * the warpgroup goes on without it, the results are unchanged).  Status 2 for an engine without the tensor-core backend. */
+int dqmc_debug_tc_error(dqmc_handle h, int32_t* flag);
 
 /* Measurement aid (bench.py roofline): between begin/end every dense-layer GEMM launch is
  * bracketed by CUDA events on the caller's stream; end() returns their summed duration [ms],

@@ -8,9 +8,10 @@ Builds the benzene / ccECP Psiformer engine (fp32, tensor-core backend; N = 30 e
 kernel time (CUDA events over --launches launches after a warm-up), one created with DQMC_TRUNK_PHASES=1 for the phase shares.
 Prints and writes OUT_DIR/trunk_phases_<mol>.json: us per (tile, layer) per SM, algorithmic TFLOP/s (counted as the engine's
 profiler counts the trunk class: 2 rows (6 d^2 + 2 N d) per layer), each phase's share of the consumer warpgroups' cycles,
-and the card's name, power limit and SM clocks (read-only nvidia-smi query).  The two warpgroups of a CTA hand an MMA token
-back and forth: 'mma_turn' is the time a warpgroup waited for the other one's MMAs (the part of its own non-MMA work that
-did not cover them), 'weight_wait' the time it waited for weight slots to land.
+and the card's name, power limit and SM clocks (read-only nvidia-smi query).  The two warpgroups of a CTA share the tensor
+cores through a lock that whichever asks first takes: 'mma_turn' is the time a warpgroup waited for that lock while the
+other one issued its MMAs (the part of those MMAs its own non-MMA work did not cover), 'weight_wait' the time it waited
+for weight slots to land.
 
 'sass_bytes' is the machine code of the trunk instance the run launched (cuobjdump -sass of the built library), split at the
 phase timers in address order: the code between two timer marks belongs to the phase the later mark books, a mark whose
