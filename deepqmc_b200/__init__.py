@@ -2,7 +2,7 @@
 neural wave functions, behind the reference's Ansatz / Hamiltonian / ElectronSampler plugin
 interfaces.  See DESIGN.md and INTEGRATION.md."""
 from .molecule import Molecule
-from .spec import AnsatzSpec, ferminet_spec, psiformer_spec
+from .spec import AnsatzSpec, deeperwin_spec, ferminet_spec, psiformer_spec
 from .types import PhysicalConfiguration, Psi
 
-__all__ = ['Molecule', 'AnsatzSpec', 'psiformer_spec', 'ferminet_spec', 'PhysicalConfiguration', 'Psi']
+__all__ = ['Molecule', 'AnsatzSpec', 'psiformer_spec', 'ferminet_spec', 'deeperwin_spec', 'PhysicalConfiguration', 'Psi']

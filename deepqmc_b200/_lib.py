@@ -47,6 +47,8 @@ class DqmcConfig(C.Structure):
         ('gnn_deep_edges', C.c_int32), ('gnn_res_norm', C.c_int32), ('gnn_g_bias', C.c_int32), ('gnn_w_bias', C.c_int32),
         ('gnn_w_dims', C.c_int32 * 32), ('gnn_h_dims', C.c_int32 * 32), ('gnn_u_dims', C.c_int32 * 32),
         ('nuc_cusp_kind', C.c_int32), ('z_nuclear', C.c_double * MAX_NUC), ('backflow_add', C.c_int32),
+        ('gnn_sep_edges', C.c_int32), ('gnn_self_edges', C.c_int32), ('gnn_ne_identity', C.c_int32),
+        ('gnn_no_res', C.c_int32), ('gnn_edge_in', C.c_int32 * 3),
     ]
 
 

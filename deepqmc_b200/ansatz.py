@@ -13,7 +13,8 @@ import torch
 
 from . import params as PN
 from .engine import Engine
-from .spec import AnsatzSpec, ferminet_spec, paulinet_default_spec, paulinet_spec, psiformer_spec, transpsiformer_spec
+from .spec import (AnsatzSpec, deeperwin_spec, ferminet_spec, paulinet_default_spec, paulinet_spec, psiformer_spec,
+                   transpsiformer_spec)
 from .types import PhysicalConfiguration, Psi
 
 
@@ -22,7 +23,7 @@ class B200Ansatz:
         self.hamil = hamil
         self.spec: AnsatzSpec = {'psiformer': psiformer_spec, 'ferminet': ferminet_spec,
                                  'transpsiformer': transpsiformer_spec, 'paulinet': paulinet_spec,
-                                 'paulinet_default': paulinet_default_spec}[kind](hamil, **hyper)
+                                 'paulinet_default': paulinet_default_spec, 'deeperwin': deeperwin_spec}[kind](hamil, **hyper)
         self.dtype, self.device, self.gemm_backend = dtype, device, gemm_backend
         self._engine = None
         self._uploaded = None

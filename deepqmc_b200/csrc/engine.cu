@@ -222,6 +222,17 @@ struct EngineBase {
                    const void* nu, void* stats, void* ws, int64_t wsb, cudaStream_t st, double p_exchange = 0.0,
                    const int32_t* ex_flags = nullptr, const int32_t* ex_idx = nullptr) = 0;
 
+  // width of the type-t edge stream (same / anti / ne) entering layer l: the raw features, or edge_dim after a deep layer
+  int gnn_ein(int t, int l) const {
+    if (cfg.gnn_deep_edges && l > 0) return cfg.edge_dim;
+    return cfg.gnn_edge_in[t] > 0 ? cfg.gnn_edge_in[t] : 4;
+  }
+  // width of the h_ne rows of layer l: the filter's width, i.e. the ne edge stream itself when it is the filter
+  int gnn_hne_w(int l) const { return cfg.gnn_ne_identity ? gnn_ein(2, l) : cfg.edge_dim; }
+  // convolution columns of layer l: [conv_same | conv_anti (| conv_ne)] or [conv_same + conv_anti | conv_ne]
+  int gnn_conv_w(int l) const {
+    return (cfg.gnn_ne_identity ? 1 : 2) * cfg.edge_dim + (cfg.gnn_conv_ne ? gnn_hne_w(l) : 0);
+  }
   void add(const std::string& n, int rows, int cols) {
     entries.push_back({n, total, rows, cols});
     total += (int64_t)rows * cols;
@@ -250,14 +261,14 @@ struct EngineBase {
       // reference tests/conf/ansatz.yaml and conf/ansatz/default.yaml; entry names mirror the Haiku modules
       const int e = cfg.edge_dim, nl = cfg.gnn_sub_n > 0 ? cfg.gnn_sub_n : 1;
       if (!cfg.gnn_features) add("emb.table", cfg.n_elec_types > 0 ? cfg.n_elec_types : 1, d);
-      int dcur = cfg.gnn_features ? 4 * M : d, ecur = 4;
+      int dcur = cfg.gnn_features ? 4 * M : d;
       const int nt = cfg.gnn_conv_ne ? 3 : 2;
       const char* tn[3] = {"same", "anti", "ne"};
       for (int l = 0; l < cfg.n_layers; ++l) {
         std::string p = "G" + std::to_string(l) + ".";
         for (int t = 0; t < nt; ++t) {
-          int din = ecur;
-          for (int i = 0; i < nl; ++i) {
+          int din = gnn_ein(t, l);
+          for (int i = 0; i < nl && !(t == 2 && cfg.gnn_ne_identity); ++i) {
             const std::string q = p + "w_" + tn[t] + "." + std::to_string(i);
             add(q + ".w", din, cfg.gnn_w_dims[l][i]);
             if (cfg.gnn_w_bias) add(q + ".b", 1, cfg.gnn_w_dims[l][i]);
@@ -271,22 +282,23 @@ struct EngineBase {
               din = cfg.gnn_h_dims[l][i];
             }
           } else {
-            add(p + "hne", M, e);  // h_ne(nuclear embedding table): walker-independent, evaluated on the host
+            add(p + "hne", M, gnn_hne_w(l));  // h_ne(nuclear embedding table): walker-independent, evaluated on the host
           }
           if (!cfg.gnn_concat) { add(p + "g_" + tn[t] + ".w", e, d); add(p + "g_" + tn[t] + ".b", 1, d); }
         }
         if (cfg.gnn_concat) {
-          add(p + "g.w", 3 * dcur + nt * e, d);
+          add(p + "g.w", 3 * dcur + gnn_conv_w(l), d);
           if (cfg.gnn_g_bias) add(p + "g.b", 1, d);
         }
         if (cfg.gnn_deep_edges && l < cfg.n_layers - 1) {
-          int din = ecur;
-          for (int i = 0; i < nl; ++i) {
-            const std::string q = p + "u." + std::to_string(i);
-            add(q + ".w", din, cfg.gnn_u_dims[l][i]); add(q + ".b", 1, cfg.gnn_u_dims[l][i]);
-            din = cfg.gnn_u_dims[l][i];
+          for (int t = 0; t < (cfg.gnn_sep_edges ? nt : 1); ++t) {
+            int din = gnn_ein(t, l);
+            for (int i = 0; i < nl; ++i) {
+              const std::string q = p + (cfg.gnn_sep_edges ? std::string("u_") + tn[t] : std::string("u")) + "." + std::to_string(i);
+              add(q + ".w", din, cfg.gnn_u_dims[l][i]); add(q + ".b", 1, cfg.gnn_u_dims[l][i]);
+              din = cfg.gnn_u_dims[l][i];
+            }
           }
-          ecur = e;
         }
         dcur = d;
       }
@@ -607,6 +619,15 @@ struct Engine : EngineBase {
     if (cfg.kind == DQMC_FERMINET || cfg.kind == DQMC_PAULINET) { H = 1; dh = d; }
     gnn = cfg.kind == DQMC_PAULINET;
     if (gnn && (cfg.jastrow_n > 8 || cfg.backflow_n > 8 || cfg.jastrow_n < 0 || cfg.backflow_n < 0)) { err = "bad MLP depth"; return 2; }
+    for (int t = 0; t < 3; ++t)
+      if (cfg.gnn_edge_in[t] != 0 && cfg.gnn_edge_in[t] != 1 && cfg.gnn_edge_in[t] != 4) { err = "bad edge feature width"; return 2; }
+    if (gnn && ((cfg.gnn_ne_identity && (!cfg.gnn_concat || !cfg.gnn_conv_ne || cfg.edge_dim < 4)) ||
+                (cfg.gnn_no_res && !cfg.gnn_concat) || (cfg.gnn_sep_edges && !cfg.gnn_deep_edges) ||
+                (cfg.gnn_sub_n > 1 && (cfg.gnn_edge_in[0] || cfg.gnn_edge_in[1] || cfg.gnn_edge_in[2])))) {
+      err = "bad conv-GNN config (identity ne filter / no residual need the concatenate update with ne edges, separate u "
+            "needs deep edges, per-type edge widths need one-layer w / u MLPs)";
+      return 2;
+    }
     bf_in = d;
     if (gnn && cfg.backflow_n > 0) bf_in = cfg.backflow_dims[cfg.backflow_n - 1];
     if (M > DQMC_MAX_NUC || d % H != 0 || N < 2) { err = "bad config"; return 2; }
@@ -1552,19 +1573,20 @@ struct Engine : EngineBase {
   // transforms h_t, convolution over same / anti / ne edges, featurewise update sum_t g_t(conv_t) + residual;
   // then the Jastrow MLP on sum_i x_i and the hidden layers of the per-spin backflow MLPs (ssp).
   // MLP of `nl` Linear(+bias)+tanh layers on augmented rows (groups of Sg slots): in -> out, ping-pong through tmp
+  // (lda: row stride of `in` when its first din columns are the input, 0 = din)
   int gnn_mlp(const T* in, int din, const std::string& base, const int* dims, int nl, bool bias, T* tmp, T* out, int rows_,
-              int Sg, cudaStream_t st) {
+              int Sg, cudaStream_t st, int lda = 0) {
     const T* cur = in;
-    int dc = din;
+    int dc = din, ld = lda > 0 ? lda : din;
     for (int i = 0; i < nl; ++i) {
       T* dst = (i == nl - 1) ? out : tmp;
       const std::string q = base + "." + std::to_string(i);
-      int rc = gemm(cur, dc, (q + ".w").c_str(), nullptr, 0, dims[i], bias ? P(q + ".b") : nullptr, nullptr, 0, dst, dims[i], rows_,
+      int rc = gemm(cur, ld, (q + ".w").c_str(), nullptr, 0, dims[i], bias ? P(q + ".b") : nullptr, nullptr, 0, dst, dims[i], rows_,
                     dims[i], dc, Sg, 0, 1, st);
       if (rc) return rc;
       DQ_LAUNCH(act_fl_kernel<T>, dim3(rows_ / Sg, (dims[i] + 63) / 64), dim3(64), 0, st, dst, dims[i], (const T*)nullptr, 0, Sg,
                 dims[i], T(1), 0);
-      cur = dst; dc = dims[i];
+      cur = dst; dc = ld = dims[i];
     }
     return 0;
   }
@@ -1584,7 +1606,8 @@ struct Engine : EngineBase {
       DQ_LAUNCH(gnn_embed_kernel<T>, dim3((Bc * N * d + 127) / 128), dim3(128), 0, st, P("emb.table"),
                 cfg.n_elec_types > 0 ? cfg.n_elec_types : 1, N, cfg.n_up, S, d, w.X, Bc * N);
     }
-    DQ_LAUNCH(gnn_edge_feat_kernel<T>, dim3((pairs + 63) / 64), dim3(64), 0, st, r, R, Rb, N, M, Mne, w.E0, pairs, S > 1 ? qa : (const T*)nullptr);
+    DQ_LAUNCH(gnn_edge_feat_kernel<T>, dim3((pairs + 63) / 64), dim3(64), 0, st, r, R, Rb, N, M, Mne, w.E0, pairs, S > 1 ? qa : (const T*)nullptr,
+              cfg.gnn_self_edges);
     T* X = w.X;
     T* Xn = w.O;
     T* E = w.E0;
@@ -1593,28 +1616,32 @@ struct Engine : EngineBase {
     for (int l = 0; l < cfg.n_layers; ++l) {
       const std::string p = "G" + std::to_string(l) + ".";
       // edge filters of every type on all pairs (compact rows), node transforms h_same / h_anti
+      // (E holds ecur columns; the type-t stream is its first gnn_ein(t, l), e.g. [|d|] of the raw [|d|, d])
       for (int t = 0; t < nt; ++t) {
-        int rc = gnn_mlp(E, ecur, p + "w_" + tn[t], cfg.gnn_w_dims[l], nl, cfg.gnn_w_bias != 0, w.ET0, w.W3 + (size_t)t * prow * e,
-                         prow, 8, st);
+        if (t == 2 && cfg.gnn_ne_identity) continue;  // w_for_ne = false: the ne edge stream is the filter
+        int rc = gnn_mlp(E, gnn_ein(t, l), p + "w_" + tn[t], cfg.gnn_w_dims[l], nl, cfg.gnn_w_bias != 0, w.ET0,
+                         w.W3 + (size_t)t * prow * e, prow, 8, st, ecur);
         if (rc) return rc;
       }
       int rc = gnn_mlp(X, dcur, p + "h_same", cfg.gnn_h_dims[l], nl, true, w.HT, w.Hs, rows, S, st);
       if (rc) return rc;
       rc = gnn_mlp(X, dcur, p + "h_anti", cfg.gnn_h_dims[l], nl, true, w.HT, w.Ha, rows, S, st);
       if (rc) return rc;
+      const int dconv = gnn_conv_w(l);
       DQ_LAUNCH(gnn_conv_kernel<T>, dim3(groups), dim3(128), 0, st, (const T*)w.W3, (const T*)(w.W3 + (size_t)prow * e),
-                (const T*)(w.W3 + (size_t)2 * prow * e), (const T*)w.Hs, (const T*)w.Ha,
-                cfg.gnn_conv_ne ? P(p + "hne") : (const T*)nullptr, N, Mne, cfg.n_up, S, e, w.C);
+                cfg.gnn_ne_identity ? (const T*)E : (const T*)(w.W3 + (size_t)2 * prow * e), cfg.gnn_ne_identity ? ecur : e,
+                gnn_hne_w(l), (const T*)w.Hs, (const T*)w.Ha, cfg.gnn_conv_ne ? P(p + "hne") : (const T*)nullptr, N, Mne,
+                cfg.n_up, S, e, cfg.gnn_ne_identity, cfg.gnn_self_edges, w.C);
       T* Xout;
       if (cfg.gnn_concat) {
         // x <- [(x +) tanh(g([x, mean_up x, mean_down x, conv_*]))] (/ sqrt 2)   (electron_gnn.py:243-259)
-        const int fin = 3 * dcur + nt * e;
-        DQ_LAUNCH(gnn_concat_kernel<T>, dim3(Bc * S, N), dim3(128), 0, st, (const T*)X, dcur, (const T*)w.C, nt * e, N, cfg.n_up,
+        const int fin = 3 * dcur + dconv;
+        DQ_LAUNCH(gnn_concat_kernel<T>, dim3(Bc * S, N), dim3(128), 0, st, (const T*)X, dcur, (const T*)w.C, dconv, N, cfg.n_up,
                   S, w.Fc);
         rc = gemm(w.Fc, fin, (p + "g.w").c_str(), nullptr, 0, d, cfg.gnn_g_bias ? P(p + "g.b") : nullptr, nullptr, 0, Xn, d, rows,
                   d, fin, S, 0, N, st);
         if (rc) return rc;
-        const bool res = dcur == d;
+        const bool res = dcur == d && !cfg.gnn_no_res;
         DQ_LAUNCH(act_fl_kernel<T>, dim3(groups, (d + 63) / 64), dim3(64), 0, st, Xn, d, res ? (const T*)X : (const T*)nullptr,
                   d, S, d, (res && cfg.gnn_res_norm) ? isq2 : T(1), 0);
         Xout = Xn; Xn = X;
@@ -1638,7 +1665,22 @@ struct Engine : EngineBase {
       }
       X = Xout;
       dcur = d;
-      if (cfg.gnn_deep_edges && l < cfg.n_layers - 1) {
+      if (cfg.gnn_deep_edges && l < cfg.n_layers - 1 && cfg.gnn_sep_edges) {
+        // one edge MLP u_t per edge type on the compact rows (into the free filter buffer), then per pair its own type's
+        // output + normalised residual (electron_gnn.py:176-188)
+        int res_mask = 0;
+        for (int t = 0; t < nt; ++t) {
+          rc = gnn_mlp(E, gnn_ein(t, l), p + "u_" + tn[t], cfg.gnn_u_dims[l], nl, true, w.ET0, w.W3 + (size_t)t * prow * e, prow,
+                       8, st, ecur);
+          if (rc) return rc;
+          if (gnn_ein(t, l) == e && ecur == e) res_mask |= 1 << t;
+        }
+        DQ_LAUNCH((gnn_edge_select_kernel<T>), dim3((unsigned)(((size_t)prow * e + 255) / 256)), dim3(256), 0, st, (const T*)E,
+                  (const T*)w.W3, (const T*)(w.W3 + (size_t)prow * e), (const T*)(w.W3 + (size_t)2 * prow * e), 8, N, Mne,
+                  cfg.n_up, e, res_mask, isq2, En, (size_t)prow * e);
+        T* tmp = E; E = En; En = tmp;
+        ecur = e;
+      } else if (cfg.gnn_deep_edges && l < cfg.n_layers - 1) {
         // shared edge MLP u on the compact rows + normalised residual (electron_gnn.py:160-192)
         rc = gnn_mlp(E, ecur, p + "u", cfg.gnn_u_dims[l], nl, true, w.ET0, w.ET1, prow, 8, st);
         if (rc) return rc;
@@ -2260,7 +2302,7 @@ struct Engine : EngineBase {
       if (l > 0 || po) {
         gemm_raw(dZ, d, PT(q + "wg"), nullptr, 0, fin, nullptr, 0, dF, fin, rows, fin, d, 0, st);
         DQ_LAUNCH(fermi_agg_bwd_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)dF, dc, ec, N, cfg.n_up,
-                  (const T*)(res_h ? dHn : nullptr), isq2, dHc, dEc);
+                  (const T*)(res_h ? dHn : nullptr), isq2, dHc, dEc, 0);
       }
       if (l < L - 1) {
         // E_{l+1} = s (E_l + tanh(E_l Wu + bu))  |  tanh(E_l Wu + bu)
@@ -2289,16 +2331,18 @@ struct Engine : EngineBase {
   struct Tape {
     std::vector<T*> a;     // a[0] input, a[k] output of layer k (after its activation)
     std::vector<int> dim;  // widths
+    int lda0 = 0;          // row stride of the input a[0] (its first dim[0] columns are the input)
   };
   int tape_fwd(const T* in, int din, const int* dims, int nl, const std::string& base, bool bias, int act, bool last_linear,
-               int rows_, Arena& a, Tape& t, cudaStream_t st) {
+               int rows_, Arena& a, Tape& t, cudaStream_t st, int lda = 0) {
     t.a.assign(1, const_cast<T*>(in));
     t.dim.assign(1, din);
+    t.lda0 = lda > 0 ? lda : din;
     for (int i = 0; i < nl; ++i) {
       T* out = a.take<T>((size_t)rows_ * dims[i]);
       const std::string q = base + std::to_string(i);
       const bool b_i = bias && (!last_linear || base[0] != 'J' || i < nl - 1);  // Jastrow: bias 'not_last'
-      int rc = gemm(t.a.back(), t.dim.back(), (q + ".w").c_str(), nullptr, 0, dims[i], b_i ? P(q + ".b") : nullptr, nullptr, 0, out,
+      int rc = gemm(t.a.back(), i == 0 ? t.lda0 : t.dim.back(), (q + ".w").c_str(), nullptr, 0, dims[i], b_i ? P(q + ".b") : nullptr, nullptr, 0, out,
                     dims[i], rows_, dims[i], t.dim.back(), 1, 0, 1, st);
       if (rc) return rc;
       if (i < nl - 1 || !last_linear)
@@ -2323,13 +2367,14 @@ struct Engine : EngineBase {
         DQ_LAUNCH(act_bwd_kernel<T>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, cur, (const T*)t.a[i + 1], act, n);
       const bool b_i = bias && (!last_linear || base[0] != 'J' || i < nl - 1);
       if (b_i) bgrad(cur, dout, rows_, dout, G + off(q + ".b"), st);
-      wgrad(t.a[i], din, cur, dout, rows_, din, dout, G + off(q + ".w"), 0, ALL_ROWS, st);
+      const int lda = i == 0 ? t.lda0 : din;
+      wgrad(t.a[i], lda, cur, dout, rows_, din, dout, G + off(q + ".w"), 0, ALL_ROWS, st);
       if (i > 0) {
         T* nxt = (cur == s0) ? s1 : s0;
         gemm_raw(cur, dout, PT(q + ".w"), nullptr, 0, din, nullptr, 0, nxt, din, rows_, din, dout, 0, st);
         cur = nxt;
-      } else if (dIn) {
-        gemm_raw(cur, dout, PT(q + ".w"), nullptr, 0, din, accumulate ? dIn : nullptr, din, dIn, din, rows_, din, dout, 0, st);
+      } else if (dIn) {  // dIn has the input's row stride; its columns past din are left alone
+        gemm_raw(cur, dout, PT(q + ".w"), nullptr, 0, din, accumulate ? dIn : nullptr, lda, dIn, lda, rows_, din, dout, 0, st);
       }
     }
     return 0;
@@ -2349,6 +2394,8 @@ struct Engine : EngineBase {
     std::vector<std::array<Tape, 3>> Wt(L);
     std::vector<std::array<Tape, 2>> Ht(L);
     std::vector<Tape> Ut(L);
+    std::vector<std::array<Tape, 3>> Us(L);  // deep_features 'separate': one u tape per edge type
+    const bool dw = cfg.gnn_ne_identity != 0, sep = cfg.gnn_sep_edges != 0;
     xd[0] = cfg.gnn_features ? 4 * M : d;
     X[0] = a.take<T>((size_t)rows * xd[0]);
     if (cfg.gnn_features)  // raw nucleus-electron features [|d|, d]: no parameters
@@ -2358,31 +2405,40 @@ struct Engine : EngineBase {
       DQ_LAUNCH(gnn_embed_kernel<T>, dim3((rows * d + 127) / 128), dim3(128), 0, st, P("emb.table"), n_types, N, cfg.n_up, 1, d, X[0], rows);
     E[0] = a.take<T>((size_t)pairs * 4);
     ed[0] = 4;
-    DQ_LAUNCH(gnn_edge_val_kernel<T>, dim3((pairs + 127) / 128), dim3(128), 0, st, r, R, Rb, N, M, Mne, E[0], pairs);
+    DQ_LAUNCH(gnn_edge_val_kernel<T>, dim3((pairs + 127) / 128), dim3(128), 0, st, r, R, Rb, N, M, Mne, E[0], pairs,
+              cfg.gnn_self_edges);
     for (int l = 0; l < L; ++l) {
       const std::string q = "G" + std::to_string(l) + ".";
       for (int t = 0; t < nt; ++t) {
-        int rc = tape_fwd(E[l], ed[l], cfg.gnn_w_dims[l], nl, q + "w_" + tn[t] + ".", cfg.gnn_w_bias != 0, 0, false, pairs, a, Wt[l][t], st);
+        if (t == 2 && dw) continue;  // identity ne filter
+        int rc = tape_fwd(E[l], gnn_ein(t, l), cfg.gnn_w_dims[l], nl, q + "w_" + tn[t] + ".", cfg.gnn_w_bias != 0, 0, false, pairs,
+                          a, Wt[l][t], st, ed[l]);
         if (rc) return rc;
       }
       for (int t = 0; t < 2; ++t) {
         int rc = tape_fwd(X[l], xd[l], cfg.gnn_h_dims[l], nl, q + "h_" + tn[t] + ".", true, 0, false, rows, a, Ht[l][t], st);
         if (rc) return rc;
       }
-      C[l] = a.take<T>((size_t)rows * nt * e);
-      DQ_LAUNCH(gnn_conv_val_kernel<T>, dim3(rows), dim3(64), 0, st, (const T*)Wt[l][0].a.back(), (const T*)Wt[l][1].a.back(),
-                (const T*)(nt == 3 ? Wt[l][2].a.back() : nullptr), (const T*)Ht[l][0].a.back(), (const T*)Ht[l][1].a.back(),
-                nt == 3 ? P(q + "hne") : (const T*)nullptr, N, Mne, cfg.n_up, e, C[l]);
+      const int dconv = gnn_conv_w(l);
+      C[l] = a.take<T>((size_t)rows * dconv);
+      if (dw)
+        DQ_LAUNCH(gnn_conv_val_dw_kernel<T>, dim3(rows), dim3(64), 0, st, (const T*)Wt[l][0].a.back(), (const T*)Wt[l][1].a.back(),
+                  (const T*)E[l], ed[l], gnn_hne_w(l), (const T*)Ht[l][0].a.back(), (const T*)Ht[l][1].a.back(), P(q + "hne"), N,
+                  Mne, cfg.n_up, e, cfg.gnn_self_edges, C[l]);
+      else
+        DQ_LAUNCH(gnn_conv_val_kernel<T>, dim3(rows), dim3(64), 0, st, (const T*)Wt[l][0].a.back(), (const T*)Wt[l][1].a.back(),
+                  (const T*)(nt == 3 ? Wt[l][2].a.back() : nullptr), (const T*)Ht[l][0].a.back(), (const T*)Ht[l][1].a.back(),
+                  nt == 3 ? P(q + "hne") : (const T*)nullptr, N, Mne, cfg.n_up, e, C[l]);
       xd[l + 1] = d;
       if (cfg.gnn_concat) {  // x <- [(x +) tanh(g([x, mean_up x, mean_down x, conv_*]))] (/ sqrt 2)
-        const int fin = 3 * xd[l] + nt * e;
+        const int fin = 3 * xd[l] + dconv;
         Fc[l] = a.take<T>((size_t)rows * fin);
-        DQ_LAUNCH(gnn_concat_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)X[l], xd[l], (const T*)C[l], nt * e, N, cfg.n_up, 1, Fc[l]);
+        DQ_LAUNCH(gnn_concat_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)X[l], xd[l], (const T*)C[l], dconv, N, cfg.n_up, 1, Fc[l]);
         X[l + 1] = a.take<T>((size_t)rows * d);
         int rc = gemm(Fc[l], fin, (q + "g.w").c_str(), nullptr, 0, d, cfg.gnn_g_bias ? P(q + "g.b") : nullptr, nullptr, 0, X[l + 1], d,
                       rows, d, fin, 1, 0, N, st);
         if (rc) return rc;
-        const bool res = xd[l] == d;
+        const bool res = xd[l] == d && !cfg.gnn_no_res;
         DQ_LAUNCH(act_fl_kernel<T>, dim3(rows, (d + 63) / 64), dim3(64), 0, st, X[l + 1], d, res ? (const T*)X[l] : (const T*)nullptr, d, 1,
                   d, (res && cfg.gnn_res_norm) ? isq2 : T(1), 0);
       } else {  // featurewise: x <- x + sum_t tanh(g_t(conv_t)); each G_t holds the running sum
@@ -2398,7 +2454,20 @@ struct Engine : EngineBase {
         if (cfg.gnn_res_norm) { err = "dqmc_wf_vjp_params: normalised featurewise residual not supported"; return 2; }
         X[l + 1] = Gt[l][nt - 1];
       }
-      if (deep && l < L - 1) {  // shared edge MLP u + normalised residual (electron_gnn.py:160-192)
+      if (deep && l < L - 1 && sep) {  // one u per edge type, each pair keeps its own type's (electron_gnn.py:176-188)
+        int res_mask = 0;
+        for (int t = 0; t < nt; ++t) {
+          int rc = tape_fwd(E[l], gnn_ein(t, l), cfg.gnn_u_dims[l], nl, q + "u_" + tn[t] + ".", true, 0, false, pairs, a, Us[l][t], st,
+                            ed[l]);
+          if (rc) return rc;
+          if (gnn_ein(t, l) == e && ed[l] == e) res_mask |= 1 << t;
+        }
+        ed[l + 1] = e;
+        E[l + 1] = a.take<T>((size_t)pairs * e);
+        DQ_LAUNCH((gnn_edge_select_kernel<T>), dim3((unsigned)(((size_t)pairs * e + 255) / 256)), dim3(256), 0, st, (const T*)E[l],
+                  (const T*)Us[l][0].a.back(), (const T*)Us[l][1].a.back(), (const T*)(nt == 3 ? Us[l][2].a.back() : nullptr), 1, N,
+                  Mne, cfg.n_up, e, res_mask, isq2, E[l + 1], (size_t)pairs * e);
+      } else if (deep && l < L - 1) {  // shared edge MLP u + normalised residual (electron_gnn.py:160-192)
         int rc = tape_fwd(E[l], ed[l], cfg.gnn_u_dims[l], nl, q + "u.", true, 0, false, pairs, a, Ut[l], st);
         if (rc) return rc;
         ed[l + 1] = e;
@@ -2447,10 +2516,11 @@ struct Engine : EngineBase {
     // scratch for the reverse sweep
     const int xm = std::max(d, xd[0]);
     const int hm = std::max(gnn_hmax(), xm), hn = std::max(gnn_hnode_max(), e), em = gnn_emax();
-    const int fmax = 3 * xm + nt * e;
+    int fmax = 0, cmax = 0;
+    for (int l = 0; l < L; ++l) { fmax = std::max(fmax, 3 * xd[l] + gnn_conv_w(l)); cmax = std::max(cmax, gnn_conv_w(l)); }
     T* dXa = a.take<T>((size_t)rows * xm); T* dXb = a.take<T>((size_t)rows * xm);
     T* sr0 = a.take<T>((size_t)rows * std::max(hm, hn)); T* sr1 = a.take<T>((size_t)rows * std::max(hm, hn));
-    T* dCb = a.take<T>((size_t)rows * nt * e); T* dCt = a.take<T>((size_t)rows * e);
+    T* dCb = a.take<T>((size_t)rows * cmax); T* dCt = a.take<T>((size_t)rows * e);
     T* dFb = cfg.gnn_concat ? a.take<T>((size_t)rows * fmax) : nullptr;
     T* dWb[3] = {a.take<T>((size_t)pairs * e), a.take<T>((size_t)pairs * e), a.take<T>((size_t)pairs * e)};
     T* sp0 = a.take<T>((size_t)pairs * em); T* sp1 = a.take<T>((size_t)pairs * em);
@@ -2458,6 +2528,7 @@ struct Engine : EngineBase {
     T* dEa = deep ? a.take<T>((size_t)pairs * e) : nullptr;
     T* dEb = deep ? a.take<T>((size_t)pairs * e) : nullptr;
     T* dUb = deep ? a.take<T>((size_t)pairs * e) : nullptr;
+    T* dUs[3] = {dUb, sep ? a.take<T>((size_t)pairs * e) : nullptr, sep && nt == 3 ? a.take<T>((size_t)pairs * e) : nullptr};
     // orbital head
     if (cfg.mult_act == 1) {
       const size_t n = (size_t)rows * KN;
@@ -2499,8 +2570,8 @@ struct Engine : EngineBase {
       const size_t nd = (size_t)rows * d;
       const bool need_dx = l > 0 || !cfg.gnn_features;  // layer 0 of the raw-feature variant has nothing trainable upstream
       if (cfg.gnn_concat) {
-        const int fin = 3 * xd[l] + nt * e;
-        const bool res = xd[l] == d;
+        const int dconv = gnn_conv_w(l), fin = 3 * xd[l] + dconv;
+        const bool res = xd[l] == d && !cfg.gnn_no_res;
         const T sc = (res && cfg.gnn_res_norm) ? isq2 : T(1);
         DQ_LAUNCH(tanh_res_bwd_kernel<T>, dim3((unsigned)((nd + 255) / 256)), dim3(256), 0, st, (const T*)dXn, (const T*)X[l + 1],
                   (const T*)(res ? X[l] : nullptr), sc, sr0, nd);
@@ -2508,11 +2579,11 @@ struct Engine : EngineBase {
         wgrad(Fc[l], fin, sr0, d, rows, fin, d, G + off(q + "g.w"), 0, ALL_ROWS, st);
         gemm_raw(sr0, d, PT(q + "g.w"), nullptr, 0, fin, nullptr, 0, dFb, fin, rows, fin, d, 0, st);
         // dF -> dX_l (own row + spin means + residual) and dC (the convolution columns); F = [x, mean_up, mean_down, conv_*]
-        if (nt != 2) { err = "dqmc_wf_vjp_params: concatenate update with nucleus-electron convolutions not supported"; return 2; }
+        if (nt != 2 && !dw) { err = "dqmc_wf_vjp_params: concatenate update with nucleus-electron convolutions not supported"; return 2; }
         DQ_LAUNCH(fermi_agg_bwd_kernel<T>, dim3(Bc, N), dim3(128), 0, st, (const T*)dFb, xd[l], e, N, cfg.n_up,
-                  (const T*)(res ? dXn : nullptr), sc, dXc, (T*)nullptr);
-        const size_t nc = (size_t)rows * nt * e;
-        DQ_LAUNCH(slice_cols_kernel<T>, dim3((unsigned)((nc + 255) / 256)), dim3(256), 0, st, (const T*)dFb, fin, 3 * xd[l], nt * e, dCb, nc);
+                  (const T*)(res ? dXn : nullptr), sc, dXc, (T*)nullptr, fin);
+        const size_t nc = (size_t)rows * dconv;
+        DQ_LAUNCH(slice_cols_kernel<T>, dim3((unsigned)((nc + 255) / 256)), dim3(256), 0, st, (const T*)dFb, fin, 3 * xd[l], dconv, dCb, nc);
       } else {
         // X_{l+1} = X_l + sum_t tanh(z_t): tanh outputs are the differences of the running sums
         if (xd[l] == d) DQ_CHECK(cudaMemcpyAsync(dXc, dXn, sizeof(T) * nd, cudaMemcpyDeviceToDevice, st));  // residual
@@ -2529,18 +2600,33 @@ struct Engine : EngineBase {
       }
       DQ_CHECK(cudaMemsetAsync(dHb[0], 0, sizeof(T) * (size_t)rows * e, st));
       DQ_CHECK(cudaMemsetAsync(dHb[1], 0, sizeof(T) * (size_t)rows * e, st));
-      DQ_LAUNCH(gnn_conv_bwd_kernel<T>, dim3(rows), dim3(64), 0, st, (const T*)dCb, (const T*)Wt[l][0].a.back(),
-                (const T*)Wt[l][1].a.back(), (const T*)(nt == 3 ? Wt[l][2].a.back() : nullptr), (const T*)Ht[l][0].a.back(),
-                (const T*)Ht[l][1].a.back(), nt == 3 ? P(q + "hne") : (const T*)nullptr, N, Mne, cfg.n_up, e, dWb[0], dWb[1], dWb[2],
-                dHb[0], dHb[1], nt == 3 ? G + off(q + "hne") : (T*)nullptr);
       // gradient w.r.t. this layer's edge features E_l (only the deep-edge variant carries it; E_0 has nothing upstream)
       const bool need_de = deep && l > 0;
       if (need_de) DQ_CHECK(cudaMemsetAsync(dEc, 0, sizeof(T) * (size_t)pairs * ed[l], st));
+      if (dw)
+        DQ_LAUNCH(gnn_conv_bwd_dw_kernel<T>, dim3(rows), dim3(64), 0, st, (const T*)dCb, (const T*)Wt[l][0].a.back(),
+                  (const T*)Wt[l][1].a.back(), (const T*)E[l], ed[l], gnn_hne_w(l), (const T*)Ht[l][0].a.back(),
+                  (const T*)Ht[l][1].a.back(), P(q + "hne"), N, Mne, cfg.n_up, e, cfg.gnn_self_edges, dWb[0], dWb[1],
+                  need_de ? dEc : (T*)nullptr, dHb[0], dHb[1], G + off(q + "hne"));
+      else
+        DQ_LAUNCH(gnn_conv_bwd_kernel<T>, dim3(rows), dim3(64), 0, st, (const T*)dCb, (const T*)Wt[l][0].a.back(),
+                  (const T*)Wt[l][1].a.back(), (const T*)(nt == 3 ? Wt[l][2].a.back() : nullptr), (const T*)Ht[l][0].a.back(),
+                  (const T*)Ht[l][1].a.back(), nt == 3 ? P(q + "hne") : (const T*)nullptr, N, Mne, cfg.n_up, e, dWb[0], dWb[1], dWb[2],
+                  dHb[0], dHb[1], nt == 3 ? G + off(q + "hne") : (T*)nullptr);
       for (int t = 0; t < nt; ++t)
-        tape_bwd(Wt[l][t], dWb[t], q + "w_" + tn[t] + ".", cfg.gnn_w_bias != 0, 0, false, pairs, sp0, sp1, need_de ? dEc : nullptr, true, G, st);
+        if (!(t == 2 && dw)) tape_bwd(Wt[l][t], dWb[t], q + "w_" + tn[t] + ".", cfg.gnn_w_bias != 0, 0, false, pairs, sp0, sp1, need_de ? dEc : nullptr, true, G, st);
       for (int t = 0; t < 2; ++t)
         tape_bwd(Ht[l][t], dHb[t], q + "h_" + tn[t] + ".", true, 0, false, rows, sr0, sr1, need_dx ? dXc : nullptr, true, G, st);
-      if (deep && l < L - 1) {  // E_{l+1} = s (E_l + u(E_l))  |  u(E_l); dEn holds the gradient w.r.t. E_{l+1}
+      if (deep && l < L - 1 && sep) {  // E_{l+1} = per pair s (E_l + u_t(E_l)) | u_t(E_l) of its type t
+        int res_mask = 0;
+        for (int t = 0; t < nt; ++t)
+          if (gnn_ein(t, l) == e && ed[l] == e) res_mask |= 1 << t;
+        const size_t ne2 = (size_t)pairs * e;
+        DQ_LAUNCH(gnn_edge_select_bwd_kernel<T>, dim3((unsigned)((ne2 + 255) / 256)), dim3(256), 0, st, (const T*)dEn, N, Mne, cfg.n_up,
+                  e, res_mask, isq2, dUs[0], dUs[1], dUs[2], need_de ? dEc : (T*)nullptr, ne2);
+        for (int t = 0; t < nt; ++t)
+          tape_bwd(Us[l][t], dUs[t], q + "u_" + tn[t] + ".", true, 0, false, pairs, sp0, sp1, need_de ? dEc : nullptr, true, G, st);
+      } else if (deep && l < L - 1) {  // E_{l+1} = s (E_l + u(E_l))  |  u(E_l); dEn holds the gradient w.r.t. E_{l+1}
         const bool res_e = ed[l] == e;
         const size_t ne2 = (size_t)pairs * e;
         DQ_LAUNCH((axpby_kernel<T>), dim3((unsigned)((ne2 + 255) / 256)), dim3(256), 0, st, (const T*)dEn, (const T*)dEn, res_e ? isq2 / T(2) : T(0.5),

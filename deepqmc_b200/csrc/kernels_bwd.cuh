@@ -95,9 +95,9 @@ __global__ void tanh_res_bwd_kernel(const T* __restrict__ dY, const T* __restric
 // One block per (walker, electron j).  dH / dE may be null (first layer: nothing upstream has parameters).
 template <class T>
 __global__ void fermi_agg_bwd_kernel(const T* __restrict__ dF, int dh, int de, int N, int n_up, const T* __restrict__ dRes,
-                                     T res_scale, T* __restrict__ dH, T* __restrict__ dE) {
+                                     T res_scale, T* __restrict__ dH, T* __restrict__ dE, int ldf_ /*row stride, 0: 3 dh + 2 de*/) {
   const int b = blockIdx.x, j = blockIdx.y;
-  const int ldf = 3 * dh + 2 * de;
+  const int ldf = ldf_ > 0 ? ldf_ : 3 * dh + 2 * de;
   const bool down = j >= n_up;
   const T inv = T(1) / (T)(down ? N - n_up : n_up);
   const T* dFb = dF + (size_t)b * N * ldf;
@@ -589,14 +589,17 @@ __global__ void force_terms_kernel(const T* __restrict__ r, const T* __restrict_
 // ==========================================================================================
 template <class T>
 __global__ void gnn_edge_val_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M, int Mne,
-                                    T* __restrict__ E, int total) {
+                                    T* __restrict__ E, int total, int self_edges) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int NS = N + Mne;
   const int jj = idx % NS, i = (idx / NS) % N, b = idx / (NS * N);
   T* out = E + (size_t)idx * 4;
   out[0] = out[1] = out[2] = out[3] = T(0);
-  if (jj == i) return;
+  if (jj == i) {
+    if (self_edges) out[0] = m_sqrt(Num<T>::eps());  // self-interaction edge: |0| eps-safe (gnn_edge_feat_kernel)
+    return;
+  }
   const T* ri = r + ((size_t)b * N + i) * 3;
   const T* pj = jj >= N ? R + (R_batched ? (size_t)b * M * 3 : 0) + (size_t)(jj - N) * 3 : r + ((size_t)b * N + jj) * 3;
   const T d0 = ri[0] - pj[0], d1 = ri[1] - pj[1], d2 = ri[2] - pj[2];
@@ -655,6 +658,87 @@ __global__ void gnn_conv_bwd_kernel(const T* __restrict__ dC, const T* __restric
       if (nt == 3) dWne[p] = wn;
     }
   }
+}
+
+// DeepErwin convolutions on the value layouts (kernels_gnn.cuh gnn_conv_kernel with S = 1): C[b][i][:] =
+// [conv_same + conv_anti (e) | conv_ne (ene)], the same-spin sum over j = i too with self_edges; the ne filter is the ne
+// edge stream Ene (row stride ldne), Hne[M][ene].
+template <class T>
+__global__ void gnn_conv_val_dw_kernel(const T* __restrict__ Wsame, const T* __restrict__ Wanti, const T* __restrict__ Ene,
+                                       int ldne, int ene, const T* __restrict__ Hs, const T* __restrict__ Ha,
+                                       const T* __restrict__ Hne, int N, int M, int n_up, int e, int self_edges,
+                                       T* __restrict__ C) {
+  const int bi = blockIdx.x, b = bi / N, i = bi - b * N;
+  const int NS = N + M, dc = e + ene;
+  for (int k = threadIdx.x; k < dc; k += blockDim.x) {
+    T acc = T(0);
+    if (k < e) {
+      for (int j = 0; j < N; ++j) {
+        if (j == i && !self_edges) continue;
+        const bool same = (i < n_up) == (j < n_up);
+        acc += (same ? Wsame : Wanti)[((size_t)bi * NS + j) * e + k] * (same ? Hs : Ha)[((size_t)b * N + j) * e + k];
+      }
+    } else {
+      const int f = k - e;
+      for (int m = 0; m < M; ++m) acc += Ene[((size_t)bi * NS + N + m) * ldne + f] * Hne[m * ene + f];
+    }
+    C[(size_t)bi * dc + k] = acc;
+  }
+}
+
+// Backward of gnn_conv_val_dw_kernel.  dW_same / dW_anti are written for every pair (zero where the pair is not of that
+// type); dEne (nullable: nothing upstream) is INCREASED on the ne rows by dconv_ne * Hne -- the identity filter hands its
+// cotangent to the ne edge stream; dH_* / dHne are accumulated atomically (callers zero them).  Block per (walker, receiver).
+template <class T>
+__global__ void gnn_conv_bwd_dw_kernel(const T* __restrict__ dC, const T* __restrict__ Wsame, const T* __restrict__ Wanti,
+                                       const T* __restrict__ Ene, int ldne, int ene, const T* __restrict__ Hs,
+                                       const T* __restrict__ Ha, const T* __restrict__ Hne, int N, int M, int n_up, int e,
+                                       int self_edges, T* __restrict__ dWsame, T* __restrict__ dWanti, T* __restrict__ dEne,
+                                       T* __restrict__ dHs, T* __restrict__ dHa, T* __restrict__ dHne) {
+  const int bi = blockIdx.x, b = bi / N, i = bi - b * N;
+  const int NS = N + M, dc = e + ene;
+  const T* dc_ = dC + (size_t)bi * dc;
+  for (int f = threadIdx.x; f < e; f += blockDim.x) {
+    const T g = dc_[f];
+    for (int jj = 0; jj < NS; ++jj) {
+      const size_t p = ((size_t)bi * NS + jj) * e + f;
+      T ws = T(0), wa = T(0);
+      if (jj < N && (jj != i || self_edges)) {
+        const size_t hj = ((size_t)b * N + jj) * e + f;
+        if ((i < n_up) == (jj < n_up)) { ws = g * Hs[hj]; atomic_add(dHs + hj, g * Wsame[p]); }
+        else { wa = g * Ha[hj]; atomic_add(dHa + hj, g * Wanti[p]); }
+      }
+      dWsame[p] = ws; dWanti[p] = wa;
+    }
+  }
+  for (int f = threadIdx.x; f < ene; f += blockDim.x) {
+    const T g = dc_[e + f];
+    for (int m = 0; m < M; ++m) {
+      const size_t p = ((size_t)bi * NS + N + m) * ldne + f;
+      if (dEne) dEne[p] += g * Hne[m * ene + f];
+      atomic_add(dHne + m * ene + f, g * Ene[p]);
+    }
+  }
+}
+
+// Backward of gnn_edge_select_kernel (kernels_gnn.cuh) on the value layout [pairs][e]: dU_t = s_t dE' on the pairs of type
+// t (zero elsewhere), and dE += isq2 dE' on the pairs whose type kept the residual (dE nullable).
+template <class T>
+__global__ void gnn_edge_select_bwd_kernel(const T* __restrict__ dEn, int N, int M, int n_up, int e, int res_mask, T scale,
+                                           T* __restrict__ dU0, T* __restrict__ dU1, T* __restrict__ dU2, T* __restrict__ dE,
+                                           size_t n) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const int NS = N + M;
+  const size_t pair = idx / e;
+  const int jj = (int)(pair % NS), i = (int)((pair / NS) % N);
+  const int t = jj >= N ? 2 : (((i < n_up) == (jj < n_up)) ? 0 : 1);
+  const bool res = (res_mask >> t) & 1;
+  const T g = dEn[idx], gu = res ? scale * g : g;
+  dU0[idx] = t == 0 ? gu : T(0);
+  dU1[idx] = t == 1 ? gu : T(0);
+  if (dU2) dU2[idx] = t == 2 ? gu : T(0);
+  if (dE && res) dE[idx] += scale * g;
 }
 
 // In-place backward of an activation from its stored OUTPUT y: dZ = dY f'(z).  kind 0 tanh (1 - y^2); 1 ssp = softplus + log(1/2)

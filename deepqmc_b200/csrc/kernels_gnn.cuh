@@ -30,21 +30,26 @@ __global__ void gnn_embed_kernel(const T* __restrict__ emb, int n_types, int N, 
 // edge_features.py:42-78), sender = electron j != i (same / anti edges) or nucleus (ne edges).  An edge
 // depends on r_i and r_j only, so its forward-Laplacian state is COMPACT:
 //   slot 0 value | 1..3 d/dr_i | 4..6 d/dr_j (zero for nuclei) | 7 Laplacian over both particles.
-// Layout E[b][i][jj][8][4], jj < N: electron sender, jj >= N: nucleus jj - N; (i, i) is zero.  The edge MLPs
+// Layout E[b][i][jj][8][4], jj < N: electron sender, jj >= N: nucleus jj - N.  The (i, i) row is zero, or with
+// self_edges (self_interaction, graph.py:226-335) the edge r_i - r_i: |d| = sqrt(eps) (eps-safe norm of a zero vector,
+// utils.py:79-85), d = 0 and no derivative at all, since the difference vanishes identically.  The edge MLPs
 // (w_t, u) run on these rows with the ordinary row GEMM and act_fl_kernel with S = 8 (slots 1..6 are the
 // tangents, slot 7 the Laplacian).  One thread per (b, i, jj).
 // ------------------------------------------------------------------------------------------
 template <class T>
 __global__ void gnn_edge_feat_kernel(const T* __restrict__ r, const T* __restrict__ R, int R_batched, int N, int M,
                                      int Mne, T* __restrict__ E, int total,
-                                     const T* __restrict__ QA /*pseudo-Hamiltonian metric or null*/) {
+                                     const T* __restrict__ QA /*pseudo-Hamiltonian metric or null*/, int self_edges) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int NS = N + Mne;
   const int jj = idx % NS, i = (idx / NS) % N, b = idx / (NS * N);
   T* out = E + (size_t)idx * 32;
   for (int k = 0; k < 32; ++k) out[k] = T(0);
-  if (jj == i) return;
+  if (jj == i) {
+    if (self_edges) out[0] = m_sqrt(Num<T>::eps());
+    return;
+  }
   const T* ri = r + ((size_t)b * N + i) * 3;
   const bool nuc = jj >= N;
   const T* pj = nuc ? R + (R_batched ? (size_t)b * M * 3 : 0) + (size_t)(jj - N) * 3 : r + ((size_t)b * N + jj) * 3;
@@ -112,61 +117,88 @@ __global__ void gnn_concat_kernel(const T* __restrict__ X, int dx, const T* __re
 
 // ------------------------------------------------------------------------------------------
 // Convolution  conv_t(i) = sum_{senders j of type t} w_t(e_ji) * h_t(x_j)  (update_features.py:
-// 196-209; no normalisation) with the product rule on the augmented rows:
+// 196-211; no normalisation) with the product rule on the augmented rows:
 //   value   sum_j w h
 //   d_t     sum_j (d_t w) h + w d_t h           (d_t w != 0 only for t in electron i or j)
 //   Lap     sum_j (Lap w) h + w Lap h + 2 sum_{t in i, j} d_t w d_t h
-// Hs / Ha: h_same(x_j) / h_anti(x_j) augmented rows [b][j][s][e]; Hne[M][e]: h_ne of the (constant)
-// nuclear embeddings.  C[b][i][s][3 e] = [conv_same | conv_anti | conv_ne].  Block per (b, i).
+// Hs / Ha: h_same(x_j) / h_anti(x_j) augmented rows [b][j][s][e]; Hne[M][ene]: h_ne of the (constant)
+// nuclear embeddings.  Block per (b, i).
+// Wsame / Wanti: the filters of the electron edge types evaluated on ALL (i, jj) pairs (compact layout, M = number of
+// nuclear senders in it, 0 without 'ne' edges, row stride e); the kernel reads the one matching the pair.  Wne: the ne
+// filter rows of the same layout with row stride ldne and width ene -- the w_ne output (ene = e), or with w_for_ne =
+// false the ne edge stream itself (update_features.py:199-210).  self_edges: the same-spin sum includes j = i; that
+// filter row carries no derivative (gnn_edge_feat_kernel), so the product rule counts the receiver's tangent once.
+// C[b][i][s][:] = [conv_same | conv_anti | conv_ne], or with ee_sum [conv_same + conv_anti | conv_ne] (the 'ee' edge
+// type, update_features.py:218-224).
 // ------------------------------------------------------------------------------------------
-// Wsame / Wanti / Wne: the filters of the three edge types evaluated on ALL (i, jj) pairs (compact layout, M = number
-// of nuclear senders in it, 0 without 'ne' edges); the kernel reads the one matching the pair.  C has nt * e columns.
 template <class T>
 __global__ void gnn_conv_kernel(const T* __restrict__ Wsame, const T* __restrict__ Wanti, const T* __restrict__ Wne,
-                                const T* __restrict__ Hs, const T* __restrict__ Ha,
-                                const T* __restrict__ Hne, int N, int M, int n_up, int S, int e,
+                                int ldne, int ene, const T* __restrict__ Hs, const T* __restrict__ Ha,
+                                const T* __restrict__ Hne, int N, int M, int n_up, int S, int e, int ee_sum, int self_edges,
                                 T* __restrict__ C) {
   const int bi = blockIdx.x, b = bi / N, i = bi - b * N;
   const int NS = N + M, T3 = S > 1 ? S - 2 : 0;
-  const int nt = M > 0 ? 3 : 2;
+  const int ee_w = ee_sum ? e : 2 * e, dc = ee_w + (M > 0 ? ene : 0);
   const size_t wbase = (size_t)bi * NS * 8 * e;
-  for (int idx = threadIdx.x; idx < S * e; idx += blockDim.x) {
-    const int s = idx / e, f = idx - s * e;
-    T acc_same = T(0), acc_anti = T(0), acc_ne = T(0);
+  for (int idx = threadIdx.x; idx < S * dc; idx += blockDim.x) {
+    const int s = idx / dc, k = idx - s * dc;
     const int t = s - 1;             // tangent index for 1 <= s <= T3
     const int te = t / 3, tc = t - 3 * te;
-    for (int j = 0; j < N; ++j) {
-      if (j == i) continue;
-      const bool same = (i < n_up) == (j < n_up);
-      const T* w = (same ? Wsame : Wanti) + wbase + (size_t)j * 8 * e + f;
-      const T* h = (same ? Hs : Ha) + ((size_t)(b * N + j) * S) * e + f;
-      T v;
-      if (s == 0) {
-        v = w[0] * h[0];
-      } else if (s <= T3) {
-        v = w[0] * h[(size_t)s * e];
-        if (te == i) v += w[(1 + tc) * e] * h[0];
-        else if (te == j) v += w[(4 + tc) * e] * h[0];
-      } else {
-        v = w[7 * e] * h[0] + w[0] * h[(size_t)s * e];
-        T cr = T(0);
-        for (int c = 0; c < 3; ++c)
-          cr += w[(1 + c) * e] * h[(size_t)(1 + 3 * i + c) * e] + w[(4 + c) * e] * h[(size_t)(1 + 3 * j + c) * e];
-        v += T(2) * cr;
+    T acc = T(0);
+    if (k < ee_w) {
+      const int grp = ee_sum ? -1 : (k >= e ? 1 : 0), f = k >= e ? k - e : k;  // grp 0: same only, 1: anti only
+      for (int j = 0; j < N; ++j) {
+        if (j == i && !self_edges) continue;
+        const bool same = (i < n_up) == (j < n_up);
+        if ((grp == 0 && !same) || (grp == 1 && same)) continue;
+        const T* w = (same ? Wsame : Wanti) + wbase + (size_t)j * 8 * e + f;
+        const T* h = (same ? Hs : Ha) + ((size_t)(b * N + j) * S) * e + f;
+        T v;
+        if (s == 0) {
+          v = w[0] * h[0];
+        } else if (s <= T3) {
+          v = w[0] * h[(size_t)s * e];
+          if (te == i) v += w[(1 + tc) * e] * h[0];
+          else if (te == j) v += w[(4 + tc) * e] * h[0];
+        } else {
+          v = w[7 * e] * h[0] + w[0] * h[(size_t)s * e];
+          T cr = T(0);
+          for (int c = 0; c < 3; ++c)
+            cr += w[(1 + c) * e] * h[(size_t)(1 + 3 * i + c) * e] + w[(4 + c) * e] * h[(size_t)(1 + 3 * j + c) * e];
+          v += T(2) * cr;
+        }
+        acc += v;
       }
-      if (same) acc_same += v; else acc_anti += v;
+    } else {
+      const int f = k - ee_w;
+      for (int m = 0; m < M; ++m) {
+        const T* w = Wne + ((size_t)bi * NS + N + m) * 8 * ldne + f;
+        const T h0 = Hne[m * ene + f];
+        if (s == 0) acc += w[0] * h0;
+        else if (s <= T3) { if (te == i) acc += w[(1 + tc) * ldne] * h0; }
+        else acc += w[7 * ldne] * h0;
+      }
     }
-    for (int m = 0; m < M; ++m) {
-      const T* w = Wne + wbase + (size_t)(N + m) * 8 * e + f;
-      const T h0 = Hne[m * e + f];
-      if (s == 0) acc_ne += w[0] * h0;
-      else if (s <= T3) { if (te == i) acc_ne += w[(1 + tc) * e] * h0; }
-      else acc_ne += w[7 * e] * h0;
-    }
-    T* c = C + ((size_t)bi * S + s) * nt * e;
-    c[f] = acc_same; c[e + f] = acc_anti;
-    if (nt == 3) c[2 * e + f] = acc_ne;
+    C[((size_t)bi * S + s) * dc + k] = acc;
   }
+}
+
+// Deep edge update with one u MLP per edge type (deep_features 'separate', electron_gnn.py:176-188): the MLPs ran on
+// every pair into U0 / U1 / U2; each pair keeps its own type's output, with the normalised residual
+// (e + u(e)) / sqrt 2 for the types whose width did not change (bit t of res_mask; hkext.py:116-137).  E / Eo: rows
+// [pairs][slots][e] (slots = 8: compact forward-Laplacian rows, 1: values).  One thread per element.
+template <class T>
+__global__ void gnn_edge_select_kernel(const T* __restrict__ E, const T* __restrict__ U0, const T* __restrict__ U1,
+                                       const T* __restrict__ U2, int slots, int N, int M, int n_up, int e, int res_mask,
+                                       T scale, T* __restrict__ Eo, size_t n) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const int NS = N + M;
+  const size_t pair = idx / ((size_t)slots * e);
+  const int jj = (int)(pair % NS), i = (int)((pair / NS) % N);
+  const int t = jj >= N ? 2 : (((i < n_up) == (jj < n_up)) ? 0 : 1);
+  const T u = (t == 0 ? U0 : t == 1 ? U1 : U2)[idx];
+  Eo[idx] = ((res_mask >> t) & 1) ? scale * (E[idx] + u) : u;
 }
 
 // ------------------------------------------------------------------------------------------

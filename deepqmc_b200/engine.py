@@ -30,10 +30,49 @@ def paulinet_env_rep(spec: AnsatzSpec) -> int:
     return max(max((spec.env_centers.count(c) for c in set(spec.env_centers)), default=1), 1)
 
 
+def softplus(x):
+    return np.logaddexp(0.0, x)
+
+
+def nuclear_types(spec: AnsatzSpec) -> np.ndarray:
+    """Atom type of every nucleus: the index of its charge among the sorted distinct charges (the hk.Embed input of
+    NucleiEmbedding with atom_type_embedding, gnn/electron_gnn.py:516-524)."""
+    return np.unique(np.asarray(spec.charges), return_inverse=True)[1]
+
+
+def _pack_deeperwin(spec: AnsatzSpec, params: dict) -> dict[str, np.ndarray]:
+    """DeepErwin tree -> engine entries.  Walker-independent preparation only: h_ne of the nuclear embeddings per layer
+    (the sender data of the ne convolution, as the test ansatz's hne table) and the envelope exponents softplus(zeta)
+    (wf/env.py:55-70; the Slater kernels take |exponent|, and softplus > 0)."""
+    g = lambda k: np.asarray(params[k], dtype=np.float64)
+    K, N = spec.n_determinants, spec.n_elec
+    xn = g(PN.GNN + 'nuclei_embedding/~/embed:embeddings')[nuclear_types(spec)]  # [M, 32]
+    out = {}
+    for l in range(spec.n_layers):
+        c, lp = PN.conv_prefix(l), PN.layer_prefix(l)
+        for t in ('same', 'anti'):
+            for m in ('w', 'h'):
+                out[f'G{l}.{m}_{t}.0.w'] = g(c + f'{m}_{t}/linear_0:w')
+                out[f'G{l}.{m}_{t}.0.b'] = g(c + f'{m}_{t}/linear_0:b')[None]
+        out[f'G{l}.hne'] = np.tanh(xn @ g(c + 'h_ne/linear_0:w') + g(c + 'h_ne/linear_0:b'))
+        out[f'G{l}.g.w'], out[f'G{l}.g.b'] = g(lp + 'g/linear_0:w'), g(lp + 'g/linear_0:b')[None]
+        if l < spec.n_layers - 1:
+            for t in PN.EDGE_TYPES:
+                out[f'G{l}.u_{t}.0.w'], out[f'G{l}.u_{t}.0.b'] = g(lp + f'u{t}/linear_0:w'), g(lp + f'u{t}/linear_0:b')[None]
+    for s_, t in (('up', 'up'), ('down', 'dn')):
+        out[f'bf.{t}'], out[f'bfb.{t}'] = g((PN.BF_UP if t == 'up' else PN.BF_DN) + ':w'), np.zeros((1, K * N))
+        out[f'env.pi_{t}'] = g(f'{PN.ENV}:pi_{s_}')
+        out[f'env.zeta_{t}'] = softplus(g(f'{PN.ENV}:zetas_{s_}'))
+    out['cusp.alpha'] = np.zeros((1, 2))
+    return out
+
+
 def _pack_haiku_params(spec: AnsatzSpec, params: dict, R=None) -> dict[str, np.ndarray]:
     """Haiku-named tree (deepqmc_b200.params) -> the engine's packed entries."""
     g = lambda k: np.asarray(params[k], dtype=np.float64)
     out = {}
+    if spec.kind == 'deeperwin':
+        return _pack_deeperwin(spec, params)
     if spec.kind in ('psiformer', 'transpsiformer'):
         out['emb.w'] = g(PN.GNN + 'electron_embedding/linear:w')
         for l in range(spec.n_layers):
@@ -188,6 +227,48 @@ def _unpack_psiformer_grads(spec: AnsatzSpec, entries: dict, flat) -> dict:
     return out
 
 
+def _unpack_deeperwin_grads(spec: AnsatzSpec, entries: dict, flat, params: dict) -> dict:
+    """Engine-layout gradient vector -> Haiku-named DeepErwin tree (inverse of _pack_deeperwin).  The walker-independent
+    preparation is differentiated here: the cotangents of the h_ne tables G<l>.hne are pulled back through
+    tanh(embed[type] W + b) to h_ne and the atom-type embedding table, and the uploaded exponent softplus(zeta) maps its
+    gradient through sigmoid(zeta)."""
+    def e(name):
+        off, rows, cols = entries[name]
+        return flat[off:off + rows * cols].reshape(rows, cols)
+
+    dev, dt = flat.device, flat.dtype
+    leaf = lambda k: torch.as_tensor(np.asarray(params[k], dtype=np.float64)).requires_grad_(True)
+    emb_k = PN.GNN + 'nuclei_embedding/~/embed:embeddings'
+    emb = leaf(emb_k)
+    types = torch.as_tensor(nuclear_types(spec))
+    out, loss = {}, 0.0
+    for l in range(spec.n_layers):
+        c, lp = PN.conv_prefix(l), PN.layer_prefix(l)
+        for t in ('same', 'anti'):
+            for m in ('w', 'h'):
+                out[c + f'{m}_{t}/linear_0:w'] = e(f'G{l}.{m}_{t}.0.w')
+                out[c + f'{m}_{t}/linear_0:b'] = e(f'G{l}.{m}_{t}.0.b')[0]
+        out[lp + 'g/linear_0:w'], out[lp + 'g/linear_0:b'] = e(f'G{l}.g.w'), e(f'G{l}.g.b')[0]
+        if l < spec.n_layers - 1:
+            for t in PN.EDGE_TYPES:
+                out[lp + f'u{t}/linear_0:w'], out[lp + f'u{t}/linear_0:b'] = e(f'G{l}.u_{t}.0.w'), e(f'G{l}.u_{t}.0.b')[0]
+        w, b = leaf(c + 'h_ne/linear_0:w'), leaf(c + 'h_ne/linear_0:b')
+        hn = torch.tanh(emb[types] @ w + b)
+        loss = loss + (hn * e(f'G{l}.hne').detach().cpu().double()).sum()
+        out[c + 'h_ne/linear_0:w'], out[c + 'h_ne/linear_0:b'] = w, b
+    loss.backward()
+    for k, v in list(out.items()):
+        if isinstance(v, torch.Tensor) and v.requires_grad:
+            out[k] = v.grad.to(device=dev, dtype=dt)
+    out[emb_k] = emb.grad.to(device=dev, dtype=dt)
+    for s_, t in (('up', 'up'), ('down', 'dn')):
+        out[(PN.BF_UP if t == 'up' else PN.BF_DN) + ':w'] = e(f'bf.{t}')
+        out[f'{PN.ENV}:pi_{s_}'] = e(f'env.pi_{t}')
+        z = torch.as_tensor(np.asarray(params[f'{PN.ENV}:zetas_{s_}'], dtype=np.float64), device=dev, dtype=dt)
+        out[f'{PN.ENV}:zetas_{s_}'] = e(f'env.zeta_{t}') * torch.sigmoid(z)
+    return out
+
+
 def _unpack_paulinet_grads(spec: AnsatzSpec, entries: dict, flat, params: dict) -> dict:
     """Engine-layout gradient vector -> Haiku-named tree for the conv-GNN test ansatz (inverse of _pack_haiku_params for
     spec.kind == 'paulinet', featurewise / hk.Embed variant).  The walker-independent h_ne(nuclear embedding) rows were
@@ -322,14 +403,14 @@ class Engine:
             self.device_index = 0 if self._host else (torch.cuda.current_device() if device is None else device)
             self.device = torch.device('cpu') if self._host else torch.device('cuda', self.device_index)
         cfg = _lib.DqmcConfig()
-        cfg.kind = {'psiformer': 0, 'ferminet': 1, 'transpsiformer': 2, 'paulinet': 3}[spec.kind]
+        cfg.kind = {'psiformer': 0, 'ferminet': 1, 'transpsiformer': 2, 'paulinet': 3, 'deeperwin': 3}[spec.kind]
         cfg.dtype, cfg.gemm_backend = self.dtype_code, gemm_backend
         cfg.n_up, cfg.n_down, cfg.n_nuc = spec.n_up, spec.n_down, spec.n_nuc
         cfg.embedding_dim, cfg.n_layers, cfg.n_heads = spec.embedding_dim, spec.n_layers, spec.n_heads
         cfg.n_determinants, cfg.edge_dim = spec.n_determinants, spec.edge_dim
         cfg.n_env_per_nuc = spec.n_env_per_nuc
         cfg.n_nuc_tokens = spec.n_nuc if spec.kind == 'transpsiformer' else 0
-        if spec.kind == 'paulinet':
+        if spec.kind in ('paulinet', 'deeperwin'):
             cfg.n_env_per_nuc = paulinet_env_rep(spec) if spec.env_per_shell else 1
             cfg.gnn_features = 1 if spec.gnn_embedding == 'features' else 0
             cfg.gnn_concat = 1 if spec.gnn_update == 'concatenate' else 0
@@ -340,6 +421,9 @@ class Engine:
             cfg.gnn_g_bias = 1 if spec.gnn_g_bias else 0
             cfg.gnn_w_bias = 1 if spec.gnn_update == 'concatenate' else 0
             assert spec.n_layers <= 8 and spec.gnn_subnet_layers <= 4
+            if spec.kind == 'deeperwin':  # conf/ansatz/deeperwin.yaml (deepqmc_b200.spec.deeperwin_spec)
+                cfg.gnn_sep_edges = cfg.gnn_self_edges = cfg.gnn_ne_identity = cfg.gnn_no_res = 1
+                cfg.gnn_edge_in[:] = [PN.DEEPERWIN_EDGE_IN[t] for t in PN.EDGE_TYPES]
             d_in, e_in = (spec.embedding_dim if spec.gnn_embedding == 'embed' else 4 * spec.n_nuc), 4
             for l in range(spec.n_layers):
                 for i, v in enumerate(PN.log_dims(e_in, spec.edge_dim, spec.gnn_subnet_layers)):
@@ -552,7 +636,9 @@ class Engine:
         rc = self.lib.dqmc_wf_vjp_params(self.h, r.data_ptr(), R.data_ptr(), Rb, B, w.data_ptr(), sign.data_ptr(), log.data_ptr(),
                                          flat.data_ptr(), ws.data_ptr(), ws.numel(), self._stream())
         self._check(rc, 'dqmc_wf_vjp_params')
-        if self.spec.kind == 'paulinet':
+        if self.spec.kind == 'deeperwin':
+            grads = _unpack_deeperwin_grads(self.spec, self.entries, flat, self._params)
+        elif self.spec.kind == 'paulinet':
             grads = _unpack_paulinet_grads(self.spec, self.entries, flat, self._params)
         else:
             unpack = _unpack_ferminet_grads if self.spec.kind == 'ferminet' else _unpack_psiformer_grads

@@ -116,6 +116,8 @@ def param_shapes(spec: AnsatzSpec) -> dict[str, tuple[int, ...]]:
         if spec.conf_coeff == 'linear':
             s[CONF + ':w'] = (K, 1)
         return s
+    if spec.kind == 'deeperwin':
+        return deeperwin_shapes(spec)
     if spec.kind != 'transpsiformer':
         for nm in ('pi_up', 'pi_down', 'zetas_up', 'zetas_down'):
             s[f'{ENV}:{nm}'] = (K * N, M)
@@ -175,13 +177,62 @@ def param_shapes(spec: AnsatzSpec) -> dict[str, tuple[int, ...]]:
     return s
 
 
+DEEPERWIN_EDGE_IN = {'same': 1, 'anti': 1, 'ne': 4}  # DistancePowerEdgeFeature([1]) | + DifferenceEdgeFeature
+
+
+def deeperwin_edge_width(spec, t, l):
+    """Width of the type-t edge stream entering layer l: the raw features, then two_particle_stream_dim after the
+    first deep update (electron_gnn.py:160-192)."""
+    return DEEPERWIN_EDGE_IN[t] if l == 0 else spec.edge_dim
+
+
+def n_atom_types(spec):
+    return len(set(spec.charges))
+
+
+def deeperwin_shapes(spec: AnsatzSpec) -> dict[str, tuple[int, ...]]:
+    """reference: conf/ansatz/deeperwin.yaml; gnn/electron_gnn.py:72-158 (u<type> per edge type), :435-537
+    (NucleiEmbedding: hk.Embed over atom types), gnn/update_features.py:162-238 (w_same / w_anti, no w_ne, h_<type> with
+    the width of the filter), hkext.py:22-113 (MLP ['log', 1] = one Linear), wf/env.py:10-75 (one shell per nucleus)."""
+    N, M, d, K, e = spec.n_elec, spec.n_nuc, spec.embedding_dim, spec.n_determinants, spec.edge_dim
+    s: dict[str, tuple[int, ...]] = {}
+    for nm in ('pi_up', 'pi_down', 'zetas_up', 'zetas_down'):
+        s[f'{ENV}:{nm}'] = (K * N, M)
+    s[GNN + 'nuclei_embedding/~/embed:embeddings'] = (n_atom_types(spec), spec.nuc_embedding_dim)
+    d_in = 4 * M
+    for l in range(spec.n_layers):
+        c, lp = conv_prefix(l), layer_prefix(l)
+        for t in ('same', 'anti'):
+            s[c + f'w_{t}/linear_0:w'] = (deeperwin_edge_width(spec, t, l), e)
+            s[c + f'w_{t}/linear_0:b'] = (e,)
+            s[c + f'h_{t}/linear_0:w'] = (d_in, e)
+            s[c + f'h_{t}/linear_0:b'] = (e,)
+        ene = deeperwin_edge_width(spec, 'ne', l)
+        s[c + 'h_ne/linear_0:w'] = (spec.nuc_embedding_dim, ene)
+        s[c + 'h_ne/linear_0:b'] = (ene,)
+        s[lp + 'g/linear_0:w'] = (3 * d_in + e + ene, d)
+        s[lp + 'g/linear_0:b'] = (d,)
+        if l < spec.n_layers - 1:
+            for t in ('ne', 'same', 'anti'):
+                s[lp + f'u{t}/linear_0:w'] = (deeperwin_edge_width(spec, t, l), e)
+                s[lp + f'u{t}/linear_0:b'] = (e,)
+        d_in = d
+    s[BF_UP + ':w'] = (d, K * N)
+    s[BF_DN + ':w'] = (d, K * N)
+    return s
+
+
 def init_params(spec: AnsatzSpec, seed: int = 0) -> dict[str, np.ndarray]:
     """Ansatz.init equivalent (reference: src/deepqmc/types.py:119-131)."""
     rng = np.random.default_rng(seed)
     out = {}
     for name, shape in param_shapes(spec).items():
         leaf = name.rsplit(':', 1)[1]
-        if name == f'{ENV}:zetas' and spec.kind == 'paulinet':
+        if spec.kind == 'deeperwin' and leaf in ('w', 'b') and not name.startswith(ENV):
+            # init 'deeperwin' (hkext.py:66-80): VarianceScaling(1, fan_avg, uniform) weights, zero biases
+            lim = np.sqrt(3.0 / ((shape[0] + shape[1]) / 2)) if leaf == 'w' else 0.0
+            v = rng.uniform(-lim, lim, size=shape)
+        elif name == f'{ENV}:zetas' and spec.kind == 'paulinet':
             v = np.asarray(spec.env_zeta_init, dtype=np.float64)  # init_to_ones = false: z / (k + 1)
         elif name == f'{ENV}:pi' and spec.kind == 'paulinet':
             v = 1.0 + rng.standard_normal(shape) / np.sqrt(shape[0])

@@ -8,12 +8,13 @@ from __future__ import annotations
 
 import dataclasses
 
-__all__ = ['AnsatzSpec', 'psiformer_spec', 'ferminet_spec', 'transpsiformer_spec', 'paulinet_spec', 'paulinet_default_spec', 'log_dims']
+__all__ = ['AnsatzSpec', 'psiformer_spec', 'ferminet_spec', 'transpsiformer_spec', 'paulinet_spec', 'paulinet_default_spec',
+           'deeperwin_spec', 'log_dims']
 
 
 @dataclasses.dataclass(frozen=True)
 class AnsatzSpec:
-    kind: str  # 'psiformer' | 'ferminet' | 'transpsiformer' | 'paulinet'
+    kind: str  # 'psiformer' | 'ferminet' | 'transpsiformer' | 'paulinet' | 'deeperwin'
     n_up: int
     n_down: int
     n_nuc: int
@@ -57,6 +58,8 @@ class AnsatzSpec:
     # BackflowOp branches (wf/nn_wave_function.py:14-33,111-125): 'mult' in every shipped config; 'add' / 'both' add
     # cutoff(r_i) * |envelope_i| * 0.1 tanh(f_add / 4) (Psiformer / FermiNet kinds)
     backflow_transform: str = 'mult'
+    # DeepErwin (kind 'deeperwin'): width of the nuclear hk.Embed table that feeds h_ne (gnn/electron_gnn.py:513-514)
+    nuc_embedding_dim: int = 32
 
     @property
     def n_elec(self):
@@ -134,3 +137,20 @@ def paulinet_default_spec(hamil, **kw):
     d.update(kw)
     d.setdefault('charges', tuple(float(z) for z in hamil.mol.charges))
     return AnsatzSpec('paulinet', hamil.n_up, hamil.n_down, hamil.n_nuc, **d)
+
+
+def deeperwin_spec(hamil, **kw):
+    """reference: src/deepqmc/conf/ansatz/deeperwin.yaml -- the conv-GNN family with raw nucleus-electron features
+    ([|d|, d] for every nucleus, no projection), |d| on same / anti edges and [|d|, d] on ne edges, same-spin edges with
+    self-interaction, 4 layers of x <- tanh(g([x, mean_up x, mean_down x, conv_ee, conv_ne])) without residual, where
+    conv_ee = conv_same + conv_anti and the ne convolution uses the ne edge stream itself as filter (w_for_ne: false) on
+    h_ne of a 32-wide nuclear hk.Embed over atom types; separate deep edge MLPs u_same / u_anti / u_ne with normalised
+    residual; one-layer tanh w / h / u / g MLPs with bias; linear bias-free backflow; 32 full determinants, SumPool, no
+    cusp, no Jastrow; isotropic per-orbital spin-unrestricted envelopes exp(-softplus(zeta) |d|)."""
+    d = dict(embedding_dim=256, n_layers=4, n_determinants=32, edge_dim=32, cusp='none', full_determinant=True,
+             conf_coeff='sum', mult_act='identity', jastrow_layers=0, backflow_layers=1, backflow_bias=False,
+             gnn_embedding='features', gnn_update='concatenate', gnn_conv_ne=True, gnn_subnet_layers=1,
+             gnn_deep_edges=True, gnn_residual_normalize=False, gnn_g_bias=True, env_per_shell=False)
+    d.update(kw)
+    d.setdefault('charges', tuple(float(z) for z in hamil.mol.charges))
+    return AnsatzSpec('deeperwin', hamil.n_up, hamil.n_down, hamil.n_nuc, **d)

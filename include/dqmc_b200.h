@@ -88,6 +88,13 @@ typedef struct dqmc_config {
    * [d][2 K N] ('both': multiplicative head first), add_act = 0.1 tanh(x / 4), with_envelope = true.
    * Linear-head ansatz kinds (Psiformer, FermiNet, TransPsiformer) only. */
   int32_t backflow_add;
+  /* DeepErwin conv-GNN variant (conf/ansatz/deeperwin.yaml); all zero for the other kinds. */
+  int32_t gnn_sep_edges;    /* deep_features 'separate': one u MLP per edge type, entries "G<l>.u_<type>.<i>" */
+  int32_t gnn_self_edges;   /* self_interaction: the same-spin edges include (i, i), |d| = sqrt(eps) constant */
+  int32_t gnn_ne_identity;  /* w_for_ne = false: the ne edge stream is the filter of the ne convolution, and the
+                             * electron-electron convolutions enter the update as one sum conv_same + conv_anti ('ee') */
+  int32_t gnn_no_res;       /* electron_residual = false: x <- tanh(g(...)) */
+  int32_t gnn_edge_in[3];   /* raw feature widths of the same / anti / ne edges: 1 = [|d|], 4 = [|d|, d]; 0 reads 4 */
 } dqmc_config;
 
 typedef struct dqmc_engine* dqmc_handle;

@@ -17,7 +17,7 @@ The emulator replaces ex2.approx / rcp.approx / redux.sync by exact code: it che
 Usage:  python tools/emu_run_tests.py [--lib PATH] [--nobuild] [--asan] test_name[substring] [test_name ...]
         python tools/emu_run_tests.py --all-small          (every test small enough for the emulator, parity files)
 Tests come from test_gpu_parity.py, test_gpu_z_next_rows.py, test_gpu_ecp_cutoff.py, test_gpu_force.py, test_gpu_reverse_chunks.py,
-test_gpu_reverse_conformance.py, test_gpu_slater_conformance.py and test_gpu_zv_force.py; stacked parametrize marks run
+test_gpu_reverse_conformance.py, test_gpu_slater_conformance.py, test_gpu_zv_force.py and test_gpu_deeperwin.py; stacked parametrize marks run
 as their cartesian product, and `name[substring]` keeps the cases whose arguments' repr contains the substring.
 """
 import argparse
@@ -105,6 +105,7 @@ def main():
     import pytest
 
     pytest_param_type = type(pytest.param(0))
+    import test_gpu_deeperwin as DW
     import test_gpu_ecp_cutoff as EC
     import test_gpu_force as FC
     import test_gpu_parity as P
@@ -114,7 +115,7 @@ def main():
     import test_gpu_z_next_rows as Z
     import test_gpu_zv_force as ZV
 
-    P.DEV = Z.DEV = SC.DEV = EC.DEV = FC.DEV = RC.DEV = RV.DEV = ZV.DEV = 'cpu'
+    P.DEV = Z.DEV = SC.DEV = EC.DEV = FC.DEV = RC.DEV = RV.DEV = ZV.DEV = DW.DEV = 'cpu'
     torch.cuda.synchronize = lambda *args, **kw: None
     names = list(a.names)
     if a.all_small:
@@ -124,7 +125,8 @@ def main():
         name, _, sel = name.partition('[')
         sel = sel.rstrip(']')
         f = (getattr(Z, name, None) or getattr(P, name, None) or getattr(EC, name, None) or getattr(FC, name, None)
-             or getattr(RC, name, None) or getattr(RV, name, None) or getattr(ZV, name, None) or getattr(SC, name))
+             or getattr(RC, name, None) or getattr(RV, name, None) or getattr(ZV, name, None) or getattr(DW, name, None)
+             or getattr(SC, name))
         wants_tmp = 'tmp_path' in f.__code__.co_varnames[:f.__code__.co_argcount]
         # stacked parametrize marks: the cartesian product of their cases, passed by argument name
         axes = []
